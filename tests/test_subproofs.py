@@ -400,3 +400,54 @@ def test_prove_small_subproofs(hostsim, kind):
 @pytest.mark.parametrize('kind', ['equality', 'mult', 'pointadd'])
 def test_prove_small_subproofs_on_gpu(gpu_engine, kind):
     check_prove_small(gpu_engine.lib, kind, seed=91, B=5)
+
+
+@pytest.mark.gpu
+def test_subproof_chunk_loops_on_gpu(gpu_engine):
+    """The stand-alone paths cut a batch into chunks of 16384 rows (proveEquality, proveMult), 8192 (provePointAdd,
+    proveMembership, the small verifiers) or 4096 (verifyMembership).  One row past a chunk, every output row of a batch
+    of one repeated input row equals the output of a one-row call."""
+    L = gpu_engine.lib
+    tom = common.pg(L)
+    q = tom.order
+    P, po = common.make_params(L, 95, 8)
+    d = synth.Drbg(95, 'chunks')
+    i32 = lambda v: int(v).to_bytes(32, 'big')                               # noqa: E731
+    row = lambda b: np.frombuffer(b, np.uint8)[None, :].copy()                # noqa: E731
+    rep = lambda a, k: np.ascontiguousarray(np.repeat(a, k, axis=0))          # noqa: E731
+
+    def same(call, n):
+        """call(k) runs k copies of the input row; returns the outputs of the one-row call"""
+        one, many = call(1), call(n)
+        for a, b in zip(one, many):
+            assert b.shape[0] == n and (b == a[:1]).all()
+        return one
+
+    bl = [d.below(q) for _ in range(6)]
+    x, y = d.below(q), d.below(q)
+    Pp = p256.generator().mul(p256.new_scalar(d.below(p256.order)))
+    Qp = p256.generator().mul(p256.new_scalar(d.below(p256.order)))
+    inputs = {'equality': (row(i32(x) + i32(bl[0]) + i32(bl[1])), None, 3, 2, 16385),
+              'mult': (row(i32(x) + i32(y) + i32(x * y % q) + b''.join(i32(v) for v in bl[:3])), None, 7, 5, 16385),
+              'pointadd': (row(flat._pt(Pp, 65) + flat._pt(Qp, 65) + flat._pt(Pp.add(Qp), 65)), row(b''.join(i32(v) for v in bl)),
+                           38, 24, 8193)}
+    for kind, (ins, blind, pdraws, vdraws, n) in inputs.items():
+        tape = synth.random_tape(1, 32 * pdraws, seed=96)
+        com, proofs, st = same(lambda k: L.prove_sub_batch(kind, P, rep(ins, k), rep(tape, k), None if blind is None else rep(blind, k)), n)
+        assert st[0] == 0, kind
+        vt = synth.random_tape(1, 32 * vdraws, seed=97)
+        ok, vst = same(lambda k: L.verify_sub_batch(kind, P, rep(com, k), rep(proofs, k), rep(vt, k)), 8193)
+        assert ok[0] == 1 and vst[0] == 0, kind
+
+    ring_vals = [3, 5, 7, 11, 13]
+    ring = np.array([list(i32(v % q)) for v in ring_vals], np.uint8)
+    rs = synth.random_tape(1, 32, seed=98)
+    idx = np.array([3], np.uint32)
+    tape = synth.random_tape(1, 32 * 5 * 3, seed=99)
+    proofs, plen, st = same(lambda k: L.prove_membership_batch(P, rep(rs, k), rep(idx, k), ring, rep(tape, k)), 8193)
+    assert st[0] == 0
+    com = row(OG.gk_commit(po.ProofGroup, ring_vals[3] % q, int.from_bytes(rs[0].tobytes(), 'big')).to_bytes())
+    vt = synth.random_tape(1, 32 * (2 * 3 + 1), seed=100)
+    ok, vst = same(lambda k: L.verify_membership_batch(P, rep(com, k), ring, rep(proofs, k), rep(plen, k), rep(vt, k)), 4097)
+    assert ok[0] == 1 and vst[0] == 0
+    L.params_destroy(P)

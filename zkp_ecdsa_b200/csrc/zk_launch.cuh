@@ -2,7 +2,7 @@
 //
 // CUDA build (the product): every task runs as one thread of `zk_task_kernel<Task>` on the
 // library's stream; there is NO CPU execution path in that build.
-// ZKA_HOSTSIM build (tests only, compiled by tests/hostsim/build.sh with g++): the same task
+// ZKA_HOSTSIM build (tests only, compiled with g++ by __graft_entry__.build_hostsim): the same task
 // bodies are executed by a plain loop so the arithmetic/layout logic can be unit-tested in
 // the GPU-less CI container.  It is never part of libzkattest.so.
 #pragma once
@@ -198,10 +198,14 @@ inline bool is_device_ptr(const void*) { return false; }
 
 #endif
 
-// grow-only device buffer
+// grow-only device buffer, freed when it goes out of scope
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { dev_free(p); }
   template <class T>
   T* get(size_t count) {
     size_t bytes = count * sizeof(T);
@@ -213,10 +217,25 @@ struct DevBuf {
     }
     return reinterpret_cast<T*>(p);
   }
-  void release() {
-    dev_free(p);
-    p = nullptr;
-    cap = 0;
+};
+
+// Hands out the buffers of a pool in call order.  A pipeline takes its buffers in the same order on every call (a
+// buffer it does not need is taken at size 0), so each buffer of the pool keeps serving the same array and stops
+// growing after the first calls.
+struct Cursor {
+  DevBuf *next_, *end_;
+  template <size_t N>
+  explicit Cursor(DevBuf (&pool)[N]) : next_(pool), end_(pool + N) {}
+  DevBuf& next() {
+    if (next_ == end_) throw std::runtime_error("workspace pool exhausted");
+    return *next_++;
+  }
+  template <class T>
+  T* take(size_t count) { return next().get<T>(count); }
+  template <class T>   // null when not needed
+  T* take_if(bool need, size_t count) {
+    T* p = take<T>(need ? count : 0);
+    return need ? p : nullptr;
   }
 };
 

@@ -14,6 +14,7 @@
 #include <cmath>
 #include <mutex>
 #include <chrono>
+#include <memory>
 #include <thread>
 #include <string>
 #include <vector>
@@ -288,16 +289,29 @@ struct Lane {
   Event ev_small[2], ev_tape[2], ev_done[2], ev_out[2];
   Stream aux[2];            // verifier: the torsion guard and the P-256 part of the aggregate check run beside the tomEdwards256 MSM
   Event ev_fork, ev_join[2];
-  // workspace (grow-only)
-  DevBuf w[64];
-  DevBuf in[16], out[8];
-  DevBuf agg[48];   // workspace of the verifier's chunk-wide aggregate check (zk_verify_agg.cuh)
+  // workspace (grow-only pools, see Cursor): one chunk pass, the input and output staging buffers of each slot, and the
+  // verifier's chunk-wide aggregate check (zk_verify_agg.cuh: its fixed parts, and one pool per MSM as the two MSMs
+  // run side by side)
+  DevBuf w[51];
+  DevBuf in[2][8], out[2][3];
+  DevBuf agg[8], agg_tom[5 + 2 * AGG_MAX_LEVELS], agg_nist[5 + 2 * AGG_MAX_LEVELS];
   std::string err;
+  ~Lane() {
+    for (int i = 0; i < 2; i++) {
+      ev_destroy(ev_small[i]); ev_destroy(ev_tape[i]); ev_destroy(ev_done[i]); ev_destroy(ev_out[i]);
+    }
+    ev_destroy(ev_fork); ev_destroy(ev_join[0]); ev_destroy(ev_join[1]);
+    stream_destroy(cs_in);
+    stream_destroy(cs_out);
+    stream_destroy(aux[0]);
+    stream_destroy(aux[1]);
+    stream_destroy(st);
+  }
 };
 
 struct zka_ctx : Lane {
   int device = 0;
-  std::vector<Lane*> extra;   // lanes 1 .. nlanes-1 (lane 0 is the context itself)
+  std::vector<std::unique_ptr<Lane>> extra;   // lanes 1 .. nlanes-1 (lane 0 is the context itself)
   int nlanes = 3;             // ZKA_LANES
   DevBuf ring_in, ring_m;     // the ring of the current call (shared by all lanes, read-only while they run)
   Lane& lane(int i) { return i == 0 ? *this : *extra[i - 1]; }
@@ -340,6 +354,15 @@ int fail(zka_ctx* ctx, int code, const std::string& msg) {
   if (ctx) ctx->err = msg;
   return code;
 }
+// runs the body of an entry point: an exception (a CUDA error) becomes ZKA_E_CUDA with its message
+template <class Fn>
+int guarded(zka_ctx* ctx, Fn&& body) {
+  try {
+    return body();
+  } catch (const std::exception& e) {
+    return fail(ctx, ZKA_E_CUDA, e.what());
+  }
+}
 
 // ---- chunk-wide aggregate check of the verifier (zk_verify_agg.cuh) ------------------------------------------------
 struct AggPlan {
@@ -381,16 +404,16 @@ AggPlan agg_plan(double entries, int c_forced) {
 }
 // enqueue histogram, prefix sums, scatter, bucket sums and the reduction tree of one group; returns the root sums
 template <class Src>
-void agg_msm(Stream& st, DevBuf* A, const Src& src, const AggPlan& pl, const uint32_t* ctl, const uint32_t** rootA,
+void agg_msm(Stream& st, Cursor A, const Src& src, const AggPlan& pl, const uint32_t* ctl, const uint32_t** rootA,
              const uint32_t** rootB) {
   const AggDigits& D = pl.D;
   const int nwin = D.nwin, nb = D.nb, nseg = (nb + 1 + AGG_SEG - 1) / AGG_SEG;
   const size_t cap = (size_t)src.slots();
-  uint32_t* hist = A[0].get<uint32_t>((size_t)nwin * (nb + 1));
-  uint32_t* bstart = A[1].get<uint32_t>((size_t)nwin * (nb + 2));
-  uint32_t* segtot = A[2].get<uint32_t>((size_t)nwin * nseg);
-  uint32_t* sorted = A[3].get<uint32_t>((size_t)nwin * cap);
-  uint32_t* bsum = A[4].get<uint32_t>((size_t)nwin * nb * Src::PTW);
+  uint32_t* hist = A.take<uint32_t>((size_t)nwin * (nb + 1));
+  uint32_t* bstart = A.take<uint32_t>((size_t)nwin * (nb + 2));
+  uint32_t* segtot = A.take<uint32_t>((size_t)nwin * nseg);
+  uint32_t* sorted = A.take<uint32_t>((size_t)nwin * cap);
+  uint32_t* bsum = A.take<uint32_t>((size_t)nwin * nb * Src::PTW);
   dev_memset(st, hist, 0, (size_t)nwin * (nb + 1) * 4);
   launch(st, (long long)cap, AggHistTask<Src>{src, D, ctl, hist});
   launch(st, (long long)nwin * nseg, AggSegSumTask{ctl, hist, segtot, nb, nseg});
@@ -402,8 +425,8 @@ void agg_msm(Stream& st, DevBuf* A, const Src& src, const AggPlan& pl, const uin
   int nin = nb, ll = 0;
   for (int lv = 0; lv < pl.levels; lv++) {
     const int nout = nin >> pl.lm[lv];
-    uint32_t* oA = A[5 + 2 * lv].get<uint32_t>((size_t)nwin * nout * Src::PTW);
-    uint32_t* oB = A[6 + 2 * lv].get<uint32_t>((size_t)nwin * nout * Src::PTW);
+    uint32_t* oA = A.take<uint32_t>((size_t)nwin * nout * Src::PTW);
+    uint32_t* oB = A.take<uint32_t>((size_t)nwin * nout * Src::PTW);
     launch(st, (long long)nwin * nout, AggLevelTask<Src>{ctl, inA, inB, oA, oB, nin, pl.lm[lv], ll, nwin, D.top_shift});
     inA = oA; inB = oB; nin = nout; ll += pl.lm[lv];
   }
@@ -473,15 +496,12 @@ void build_p256_tab(zka_ctx* ctx, const uint32_t* base_aff_dev, FixedTable& out,
     uint32_t* d_hi = hi.get<uint32_t>((size_t)nwin * nh * P256_PROJ_WORDS);
     launch(st, nwin, P256RowsHiTask{d_pows, d_hi, d_rows, w});
     launch(st, (long long)nwin * nh, P256RowsLoTask{d_pows, d_hi, d_rows, w});
-    sync(st);
-    hi.release();
+    sync(st);   // hi is freed at the end of this block, before the normalisation
   } else {
     launch(st, nwin, P256RowsTask{d_pows, d_rows, w});
   }
   launch_p256_norm(st, d_rows, out.tab, nullptr, nullptr, (long long)(count));
   sync(st);
-  pows.release();
-  rows.release();
 }
 #if defined(ZKA_PG_WAR256)
 // war256 positional table [fb_windows(w)][fb_entries(w)] of affine points from one affine base (16 words, device)
@@ -500,8 +520,7 @@ void build_tom_tab(zka_ctx* ctx, const uint32_t* base_aff_dev, FixedTable& out) 
     uint32_t* d_hi = hi.get<uint32_t>((size_t)nwin * nh * P256_PROJ_WORDS);
     launch(st, nwin, WarRowsHiTask{d_pows, d_hi, d_rows, w});
     launch(st, (long long)nwin * nh, WarRowsLoTask{d_pows, d_hi, d_rows, w});
-    sync(st);
-    hi.release();
+    sync(st);   // hi is freed at the end of this block, before the normalisation
   } else {
     launch(st, nwin, WarRowsTask{d_pows, d_rows, w});
   }
@@ -510,8 +529,6 @@ void build_tom_tab(zka_ctx* ctx, const uint32_t* base_aff_dev, FixedTable& out) 
     launch(st, ((long long)count + ch - 1) / ch, WarNormTask{d_rows, out.tab, nullptr, nullptr, (int)count, ch});
   }
   sync(st);
-  pows.release();
-  rows.release();
 }
 #else
 // tomEdwards256 positional table [nwin][fb_entries(w)] from one image-curve affine base (18 words, device)
@@ -530,16 +547,13 @@ void build_tom_tab(zka_ctx* ctx, const uint32_t* base_aff_dev, FixedTable& out) 
     uint32_t* d_hi = hi.get<uint32_t>((size_t)nwin * nh * 36);
     launch(st, nwin, TomRowsHiTask{d_pows, d_hi, d_rows, w});
     launch(st, (long long)nwin * nh, TomRowsLoTask{d_pows, d_hi, d_rows, w});
-    sync(st);
-    hi.release();
+    sync(st);   // hi is freed at the end of this block, before the normalisation
   } else {
     launch(st, nwin, TomRowsTask{d_pows, d_rows, w});
   }
   // rows (E1 projective) -> entries of the prover's a = -1 image curve (v - w, v + w, 2 d2 w v)
   launch(st, (long long)(count + 15) / 16, TomTabE2Task{d_rows, out.tab, (int)count});
   sync(st);
-  pows.release();
-  rows.release();
 }
 
 #endif
@@ -553,10 +567,24 @@ const T* stage_in(Stream& st, DevBuf& buf, const T* p, size_t count) {
   copy_h2d(st, d, p, count * sizeof(T));
   return d;
 }
+
+// A caller output of `width` T per row.  Kernels write rows [b0, b0 + rows) in place when it is device memory, otherwise
+// into a staging buffer that copy_back then queues for the caller.
 template <class T>
-const T* stage_in(zka_ctx* ctx, DevBuf& buf, const T* p, size_t count) {
-  return stage_in(ctx->st, buf, p, count);
-}
+struct Output {
+  T* dst;
+  size_t width;
+  bool dev;
+  Output(T* p, size_t width) : dst(p), width(width), dev(is_device_ptr(p)) {}
+  T* rows(DevBuf& stage, uint32_t b0, size_t rows) const { return dev ? dst + b0 * width : stage.get<T>(rows * width); }
+  void copy_back(Stream& st, uint32_t b0, const T* d, size_t rows) const {
+    if (!dev) copy_d2h(st, dst + b0 * width, d, rows * width * sizeof(T));
+  }
+  // only the first `bytes` of each row
+  void copy_back_2d(Stream& st, uint32_t b0, const T* d, size_t rows, size_t bytes) const {
+    if (!dev) copy_d2h_2d(st, dst + b0 * width, width * sizeof(T), d, width * sizeof(T), bytes, rows);
+  }
+};
 
 // Chunk schedule of a call: boundaries off[0..nchunks] of the batch.  `cmax` = largest chunk, `lanes` = lanes that
 // will run.  Plain: near-equal chunks, at least one per lane when chunks of >= 256 proofs allow it.  Tapered (used
@@ -606,7 +634,7 @@ template <class Fn>
 void run_lanes(zka_ctx* ctx, int used, Fn fn) {
   if (used <= 1) { fn(0); return; }
   std::vector<std::thread> th;
-  std::vector<std::string> errs((size_t)used);
+  std::vector<std::exception_ptr> errs((size_t)used);
   for (int li = 1; li < used; li++)
     th.emplace_back([&, li] {
       try {
@@ -614,14 +642,110 @@ void run_lanes(zka_ctx* ctx, int used, Fn fn) {
         ZK_CUDA_CHECK(cudaSetDevice(ctx->device));
 #endif
         fn(li);
-      } catch (const std::exception& e) {
-        errs[(size_t)li] = e.what()[0] ? e.what() : "lane failed";
+      } catch (...) {
+        errs[(size_t)li] = std::current_exception();
       }
     });
-  try { fn(0); } catch (const std::exception& e) { errs[0] = e.what()[0] ? e.what() : "lane failed"; }
+  try { fn(0); } catch (...) { errs[0] = std::current_exception(); }
   for (auto& t : th) t.join();
   for (auto& e : errs)
-    if (!e.empty()) throw std::runtime_error(e);
+    if (e) std::rethrow_exception(e);
+}
+
+// ---- stage chains shared by the batched pipelines and the stand-alone sub-proof paths
+// The ring of a call on the device (RingPrepTask) and, for the prover, the GK Lagrange matrix (it depends only on n and
+// is cached per context).
+const uint32_t* prep_ring(zka_ctx* ctx, Stream& st, const uint8_t* ring, uint32_t N, int n, bool lagrange) {
+  const uint8_t* d_ring = stage_in(st, ctx->ring_in, ring, (size_t)N * 32);
+  uint32_t* ring_m = ctx->ring_m.get<uint32_t>(((size_t)1 << n) * 8);
+  launch(st, 1ll << n, RingPrepTask{d_ring, ring_m, (int)N});
+  if (lagrange && ctx->lag_n != n) {
+    launch(st, 1, GkLagrangeTask{ctx->lag.get<uint32_t>((size_t)n * n * 8), n});
+    ctx->lag_n = n;
+  }
+  return ring_m;
+}
+
+int gk_blocks(int n) { return 1 << (n - gk_block_bits(n)); }   // ring blocks of the GK polynomial kernels
+
+// the fields every prover shares: dimensions, tables, window bits
+ProveCtx prove_ctx(const zka_ctx* ctx, const zka_params* P, int B, int S, int N, int n) {
+  ProveCtx c;
+  memset(&c, 0, sizeof(c));
+  c.B = B; c.S = S; c.N = N; c.n = n;
+  c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
+  c.g_tab8 = ctx->g8.tab; c.h_tab8 = P->h8.tab; c.h_w = P->h_w;
+  c.g_tabw = ctx->gw.tab; c.g_w = ctx->p256_hw;
+  c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
+  c.tg_bytes = (const uint8_t*)ctx->tg_bytes.p;
+  c.gk_lag = (uint32_t*)ctx->lag.p;
+  return c;
+}
+// the same for every verifier
+VerifyCtx verify_ctx(const zka_ctx* ctx, const zka_params* P, int B, int S, int N, int n, int K, int mode) {
+  VerifyCtx c;
+  memset(&c, 0, sizeof(c));
+  c.B = B; c.S = S; c.N = N; c.n = n; c.K = K; c.mode = mode;
+  c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
+  c.g_tab8 = ctx->g8.tab; c.h_tab8 = P->h8.tab; c.h_w = P->h_w;
+  c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
+  c.tg_bytes = (const uint8_t*)ctx->tg_bytes.p;
+  return c;
+}
+
+// commitments of the first store: pkX, pkY and Tx, Ty of every repetition
+void prove_store1(Stream& st, const ProveCtx& c) {
+  const long long n1 = (long long)c.B * (2 + 2 * c.S);
+  launch(st, n1, JobsATask{c});
+  launch(st, n1, TomCommitTask{c.s1_jv, c.s1_jr, c.tg_tab, c.th_tab, c.s1_proj, c.tom_w, c.tom_nwin});
+  launch_tom_norm(st, c.s1_proj, c.s1_aff, c.s1_bytes, n1, 1);
+}
+// The c.M items of the 0-bit repetitions (pointAdd.ts:92-163 each), from their secrets to their bytes in the proof rows,
+// and the Groth-Kohlweiss commitments of the membership proof (gk.ts:129-176) with their encodings, behind the items in
+// the s2 arrays.  The stages of the two alternate (with host buffers the batched prover was measurably slower with one
+// chain after the other); provePointAdd alone runs only the items, proveMembership alone only the GK part.  gext: [M][GJOBS_PER_ITEM] g-parts of the item commitments;
+// c.gk_part: the block sums when the ring is cut into blocks.
+void prove_items_gk(Stream& st, const ProveCtx& c, uint32_t* gext, bool items, bool gk) {
+  const long long M = c.M, nj = M * JOBS_PER_ITEM, nd = M * DERS_PER_ITEM;
+  const long long Bn = (long long)c.B * c.n, ng = 4 * Bn;
+  const int nblk = gk_blocks(c.n);
+  const size_t g0 = c.s2_gk(0, 0);
+  if (items) {
+    launch(st, (M + ITEM_INV_CHUNK - 1) / ITEM_INV_CHUNK, ItemInvTask{c});
+    launch(st, M, ItemScalarsTask{c});
+  }
+  if (gk) {
+    launch(st, Bn, GkJobsTask{c});
+    launch(st, Bn * nblk, GkPolyTask{c});
+    if (nblk > 1) launch(st, Bn, GkPolyReduceTask{c});
+    launch(st, Bn, GkCdJobsTask{c});
+  }
+  if (items) {   // item jobs: g-parts once per distinct committed value, then r*h on top (TomCommitG/HTask)
+    launch(st, M * GJOBS_PER_ITEM, TomCommitGTask{c.s2_jv, c.tg_tab, gext, c.tom_w, c.tom_nwin});
+    launch(st, nj, TomCommitHTask{c.s2_jr, c.th_tab, gext, c.s2_proj, c.tom_w, c.tom_nwin});
+  }
+  if (gk)
+    launch(st, ng, TomCommitTask{c.s2_jv + g0 * 8, c.s2_jr + g0 * 8, c.tg_tab, c.th_tab, c.s2_proj + g0 * TOM_PROJ_WORDS, c.tom_w,
+                                 c.tom_nwin});
+  if (items) {
+    // only T1x, T1y (jobs 0, 1 of each item) are needed again as points (DerivedTask)
+    launch_tom_norm(st, c.s2_proj, c.s2_aff, c.s2_bytes, nj, 1, JOBS_PER_ITEM, 2);
+    launch(st, M, DerivedTask{c});
+    // derived points come from complete E1 additions, the GK commitments from the commit kernel (E2)
+    launch_tom_norm(st, c.s2_proj + nj * TOM_PROJ_WORDS, nullptr, c.s2_bytes + nj * BSTRIDE, nd, 0);
+  }
+  if (gk) launch_tom_norm(st, c.s2_proj + g0 * TOM_PROJ_WORDS, nullptr, c.s2_bytes + g0 * BSTRIDE, ng, 1);
+  if (items) {
+    launch(st, M * HASHES_PER_ITEM, ItemHashTask{c});
+    launch(st, M * 7, ItemEmitTask{c});
+  }
+}
+// the verifier's Groth-Kohlweiss chain (gk.ts:197-262): ring polynomial, relations, offsets of the GK entries of the rows
+void verify_gk(Stream& st, const VerifyCtx& c, uint32_t* gk_offs) {
+  const int nblk = gk_blocks(c.n), ngk = 4 * c.n + 1;
+  if (nblk > 1) launch(st, (long long)c.B * nblk, VGkSumTask{c});
+  launch(st, c.B, VGkTask{c});
+  launch(st, (long long)c.B * ngk, VGkOffsetsTask{c, gk_offs});
 }
 
 }  // namespace
@@ -636,7 +760,7 @@ const char* zka_last_error(const zka_ctx* ctx) { return ctx ? ctx->err.c_str() :
 uint64_t zka_launch_count(const zka_ctx* ctx) {
   if (!ctx) return 0;
   uint64_t n = ctx->st.launches + ctx->aux[0].launches + ctx->aux[1].launches;
-  for (const Lane* l : ctx->extra) n += l->st.launches + l->aux[0].launches + l->aux[1].launches;
+  for (const auto& l : ctx->extra) n += l->st.launches + l->aux[0].launches + l->aux[1].launches;
   return n;
 }
 
@@ -665,18 +789,18 @@ int zka_profile_reset(zka_ctx* ctx) {
 int zka_set_option(zka_ctx* ctx, const char* key, long value) {
   if (!ctx || !key || value < 1) return ZKA_E_ARG;
   const std::string k(key);
-  try {
+  return guarded(ctx, [&]() -> int {
     if (k == "lanes") {
       if (value > 8) return ZKA_E_ARG;
       while ((int)ctx->extra.size() + 1 < value) {
-        Lane* l = new Lane();
+        auto l = std::make_unique<Lane>();
         stream_create(l->st);
         stream_create(l->cs_in);
         stream_create(l->cs_out);
         stream_create(l->aux[0]);
         stream_create(l->aux[1]);
         l->st.profiling = ctx->st.profiling;
-        ctx->extra.push_back(l);
+        ctx->extra.push_back(std::move(l));
       }
       ctx->nlanes = (int)value;
     } else if (k == "chunk") {
@@ -691,10 +815,8 @@ int zka_set_option(zka_ctx* ctx, const char* key, long value) {
     } else {
       return ZKA_E_ARG;
     }
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
-  return 0;
+    return 0;
+  });
 }
 long long zka_stat(zka_ctx* ctx, const char* key) {
   if (!ctx || !key) return -1;
@@ -775,16 +897,17 @@ int zka_config(const zka_ctx* ctx, int* tom_w, int* tom_nwin, int* chunk) {
 int zka_init(int device, zka_ctx** out) {
   if (!out) return ZKA_E_ARG;
   *out = nullptr;
-  zka_ctx* ctx = new zka_ctx();
-  try {
 #if !defined(ZKA_HOSTSIM)
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0 || device >= ndev) {
-      cudaGetLastError();
-      delete ctx;
-      return ZKA_E_CUDA;   // no GPU: fail loudly, there is no CPU fallback
-    }
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0 || device >= ndev) {
+    cudaGetLastError();
+    return ZKA_E_CUDA;   // no GPU: fail loudly, there is no CPU fallback
+  }
+#endif
+  std::unique_ptr<zka_ctx> ctx(new zka_ctx());
+  const int rc = guarded(ctx.get(), [&] {
+#if !defined(ZKA_HOSTSIM)
     ZK_CUDA_CHECK(cudaSetDevice(device));
     ZK_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->st.s, cudaStreamNonBlocking));
 #endif
@@ -821,7 +944,7 @@ int zka_init(int device, zka_ctx** out) {
       if (const char* e = getenv("ZKA_LANES")) lanes = atoi(e);
       if (lanes < 1) lanes = 1;
       if (lanes > 8) lanes = 8;
-      if (zka_set_option(ctx, "lanes", lanes) != 0) throw std::runtime_error("lanes");
+      if (zka_set_option(ctx.get(), "lanes", lanes) != 0) throw std::runtime_error("lanes");
     }
     if (const char* e = getenv("ZKA_TAPE_SPLIT")) ctx->tape_split = atoi(e) != 0;
     if (const char* e = getenv("ZKA_AGG")) ctx->agg = atoi(e);
@@ -836,9 +959,9 @@ int zka_init(int device, zka_ctx** out) {
     DevBuf gen;
     uint32_t* d_gen = gen.get<uint32_t>(16 + TOM_AFF_WORDS);
     launch(ctx->st, 1, GenAffTask{d_gen, d_gen + 16});
-    build_p256_tab(ctx, d_gen, ctx->g8, 8);
-    build_p256_tab(ctx, d_gen, ctx->gw, ctx->p256_hw);
-    build_tom_tab(ctx, d_gen + 16, ctx->tg);
+    build_p256_tab(ctx.get(), d_gen, ctx->g8, 8);
+    build_p256_tab(ctx.get(), d_gen, ctx->gw, ctx->p256_hw);
+    build_tom_tab(ctx.get(), d_gen + 16, ctx->tg);
     // encoding of g (C_14 = params.g in pi_8, pointAdd.ts:144,220): normalise the table entry 1*g
     DevBuf proj, aff;
     uint32_t* d_proj = proj.get<uint32_t>(TOM_PROJ_WORDS);
@@ -847,59 +970,24 @@ int zka_init(int device, zka_ctx** out) {
     launch(ctx->st, 1, GProjTask{d_gen + 16, d_proj});
     launch_tom_norm(ctx->st, d_proj, d_aff, d_bytes, 1, 0);
     sync(ctx->st);
-    gen.release();
-    proj.release();
-    aff.release();
-  } catch (const std::exception& e) {
-    fprintf(stderr, "zka_init: %s\n", e.what());
-    delete ctx;
-    return ZKA_E_CUDA;
+    return 0;
+  });
+  if (rc) {
+    fprintf(stderr, "zka_init: %s\n", ctx->err.c_str());
+    return rc;
   }
-  *out = ctx;
+  *out = ctx.release();
   return 0;
 }
 
-void zka_shutdown(zka_ctx* ctx) {
-  if (!ctx) return;
-  ctx->g8.buf.release();
-  ctx->gw.buf.release();
-  ctx->tg.buf.release();
-  ctx->tg_bytes.release();
-  ctx->lag.release();
-  for (auto& b : ctx->w) b.release();
-  for (auto& b : ctx->in) b.release();
-  for (auto& b : ctx->out) b.release();
-  for (int li = 0; li < 1 + (int)ctx->extra.size(); li++)
-    for (auto& b : ctx->lane(li).agg) b.release();
-  ctx->ring_in.release();
-  ctx->ring_m.release();
-  for (int li = 0; li < 1 + (int)ctx->extra.size(); li++) {
-    Lane& l = ctx->lane(li);
-    if (li > 0) {
-      for (auto& b : l.w) b.release();
-      for (auto& b : l.in) b.release();
-      for (auto& b : l.out) b.release();
-    }
-    for (int i = 0; i < 2; i++) {
-      ev_destroy(l.ev_small[i]); ev_destroy(l.ev_tape[i]); ev_destroy(l.ev_done[i]); ev_destroy(l.ev_out[i]);
-    }
-    stream_destroy(l.cs_in);
-    stream_destroy(l.cs_out);
-    stream_destroy(l.aux[0]);
-    stream_destroy(l.aux[1]);
-    ev_destroy(l.ev_fork); ev_destroy(l.ev_join[0]); ev_destroy(l.ev_join[1]);
-    stream_destroy(l.st);
-  }
-  for (Lane* l : ctx->extra) delete l;
-  delete ctx;
-}
+void zka_shutdown(zka_ctx* ctx) { delete ctx; }
 
 int zka_params_create(zka_ctx* ctx, const uint8_t h_nist[65], const uint8_t h_proof[67], uint32_t sec_level,
                       zka_params** out) {
   if (!ctx || !h_nist || !h_proof || !out) return ZKA_E_ARG;
   if (sec_level < 1 || sec_level > MAX_REPS) return fail(ctx, ZKA_E_ARG, "sec_level must be in [1,80]");
-  try {
-    zka_params* P = new zka_params();
+  return guarded(ctx, [&] {
+    std::unique_ptr<zka_params> P(new zka_params());
     P->ctx = ctx;
     P->sec_level = sec_level;
     P->h_w = ctx->p256_hw;
@@ -920,26 +1008,15 @@ int zka_params_create(zka_ctx* ctx, const uint8_t h_nist[65], const uint8_t h_pr
     copy_d2h(ctx->st, hb, d_bad, 2);
     copy_d2h(ctx->st, hb + 2, d_inf, 1);
     sync(ctx->st);
-    if (hb[0] || hb[1] || hb[2]) {
-      delete P;
-      return fail(ctx, ZKA_E_ARG, "params: h point not on its group");
-    }
+    if (hb[0] || hb[1] || hb[2]) return fail(ctx, ZKA_E_ARG, "params: h point not on its group");
     build_p256_tab(ctx, d_an, P->h8, P->h_w);
     build_tom_tab(ctx, d_at, P->th);
-    for (DevBuf* b : {&bn, &bt, &an, &at, &bad, &inf}) b->release();
-    *out = P;
+    *out = P.release();
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
-void zka_params_destroy(zka_params* P) {
-  if (!P) return;
-  P->h8.buf.release();
-  P->th.buf.release();
-  delete P;
-}
+void zka_params_destroy(zka_params* P) { delete P; }
 
 size_t zka_proof_max_len(uint32_t ring_size, uint32_t sec_level) {
   return (size_t)proof_len((int)sec_level, ceil_log2(ring_size), (int)sec_level);
@@ -956,53 +1033,51 @@ int zka_tom_commit_batch(zka_ctx* ctx, const zka_params* P, uint32_t count, cons
                          uint8_t* out) {
   if (!ctx || !P || !v || !r || !out) return ZKA_E_ARG;
   if (count == 0) return 0;
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    const uint8_t* dv = stage_in(ctx, ctx->in[0], v, (size_t)count * 32);
-    const uint8_t* dr = stage_in(ctx, ctx->in[1], r, (size_t)count * 32);
-    uint32_t* jv = ctx->w[0].get<uint32_t>((size_t)count * 8);
-    uint32_t* jr = ctx->w[1].get<uint32_t>((size_t)count * 8);
-    uint32_t* proj = ctx->w[2].get<uint32_t>((size_t)count * TOM_PROJ_WORDS);
-    uint32_t* aff = ctx->w[3].get<uint32_t>((size_t)count * TOM_AFF_WORDS);
-    uint8_t* bytes = ctx->w[4].get<uint8_t>((size_t)count * BSTRIDE);
+    Cursor in(ctx->in[0]), w(ctx->w), ob(ctx->out[0]);
+    const uint8_t* dv = stage_in(st, in.next(), v, (size_t)count * 32);
+    const uint8_t* dr = stage_in(st, in.next(), r, (size_t)count * 32);
+    uint32_t* jv = w.take<uint32_t>((size_t)count * 8);
+    uint32_t* jr = w.take<uint32_t>((size_t)count * 8);
+    uint32_t* proj = w.take<uint32_t>((size_t)count * TOM_PROJ_WORDS);
+    uint32_t* aff = w.take<uint32_t>((size_t)count * TOM_AFF_WORDS);
+    uint8_t* bytes = w.take<uint8_t>((size_t)count * BSTRIDE);
+    const Output<uint8_t> o(out, WP);
+    uint8_t* packed = o.rows(ob.next(), 0, count);
     launch(st, count, CommitConvTask{dv, dr, jv, jr});
     launch(st, count, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, proj, ctx->tom_w, ctx->tom_nwin});
     launch_tom_norm(st, proj, aff, bytes, (long long)(count), 1);
-    if (is_device_ptr(out)) {
-      launch(st, count, PackTomTask{bytes, out});
-    } else {
-      uint8_t* packed = ctx->out[0].get<uint8_t>((size_t)count * WP);
-      launch(st, count, PackTomTask{bytes, packed});
-      copy_d2h(st, out, packed, (size_t)count * WP);
-    }
+    launch(st, count, PackTomTask{bytes, packed});
+    o.copy_back(st, 0, packed, count);
     sync(st);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 int zka_p256_mul_batch(zka_ctx* ctx, uint32_t count, const uint8_t* base, const uint8_t* k, uint8_t* out) {
   if (!ctx || !k || !out) return ZKA_E_ARG;
   if (count == 0) return 0;
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    const uint8_t* dk = stage_in(ctx, ctx->in[0], k, (size_t)count * 32);
-    const uint8_t* db = base ? stage_in(ctx, ctx->in[1], base, (size_t)count * 65) : nullptr;
-    uint32_t* proj = ctx->w[0].get<uint32_t>((size_t)count * P256_PROJ_WORDS);
-    uint32_t* aff = ctx->w[1].get<uint32_t>((size_t)count * P256_AFF_WORDS);
-    uint8_t* bytes = ctx->w[2].get<uint8_t>((size_t)count * BSTRIDE);
-    uint8_t* inf = ctx->w[3].get<uint8_t>(count);
-    uint32_t* rtab = nullptr;
-    uint8_t* binf = nullptr;
-    if (db) {
-      // per-base w=4 positional tables: the same path the prover uses for R (PhaseAP256Task)
-      uint32_t* baff = ctx->w[4].get<uint32_t>((size_t)count * 16);
-      uint8_t* bad = ctx->w[5].get<uint8_t>(count);
-      binf = ctx->w[6].get<uint8_t>(count);
-      uint32_t* pows = ctx->w[7].get<uint32_t>((size_t)count * RT_NWIN * P256_PROJ_WORDS);
-      uint32_t* rows = ctx->w[8].get<uint32_t>((size_t)count * RT_ENTRIES * P256_PROJ_WORDS);
-      rtab = ctx->w[9].get<uint32_t>((size_t)count * RT_ENTRIES * P256_AFF_WORDS);
+    Cursor in(ctx->in[0]), w(ctx->w), ob(ctx->out[0]);
+    const uint8_t* dk = stage_in(st, in.next(), k, (size_t)count * 32);
+    const uint8_t* db = stage_in(st, in.next(), base, (size_t)count * 65);
+    uint32_t* proj = w.take<uint32_t>((size_t)count * P256_PROJ_WORDS);
+    uint32_t* aff = w.take<uint32_t>((size_t)count * P256_AFF_WORDS);
+    uint8_t* bytes = w.take<uint8_t>((size_t)count * BSTRIDE);
+    uint8_t* inf = w.take<uint8_t>(count);
+    // with a base per row: per-base w=4 positional tables, the same path the prover uses for R (PhaseAP256Task)
+    const bool per_base = db != nullptr;
+    uint32_t* baff = w.take_if<uint32_t>(per_base, (size_t)count * 16);
+    uint8_t* bad = w.take_if<uint8_t>(per_base, count);
+    uint8_t* binf = w.take_if<uint8_t>(per_base, count);
+    uint32_t* pows = w.take_if<uint32_t>(per_base, (size_t)count * RT_NWIN * P256_PROJ_WORDS);
+    uint32_t* rows = w.take_if<uint32_t>(per_base, (size_t)count * RT_ENTRIES * P256_PROJ_WORDS);
+    uint32_t* rtab = w.take_if<uint32_t>(per_base, (size_t)count * RT_ENTRIES * P256_AFF_WORDS);
+    const Output<uint8_t> o(out, NP);
+    uint8_t* packed = o.rows(ob.next(), 0, count);
+    if (per_base) {
       launch(st, count, ParsePointsTask{db, nullptr, baff, nullptr, bad, binf});
       launch(st, count, P256PowsTask{baff, binf, pows, (int)count, RT_NWIN, RT_W});
       launch(st, (long long)count * RT_NWIN, P256RowsSignedTask{pows, rows});
@@ -1011,18 +1086,11 @@ int zka_p256_mul_batch(zka_ctx* ctx, uint32_t count, const uint8_t* base, const 
     }
     launch(st, count, P256MulTask{dk, ctx->g8.tab, rtab, binf, proj});
     launch_p256_norm(st, proj, aff, bytes, inf, (long long)(count));
-    if (is_device_ptr(out)) {
-      launch(st, count, PackP256Task{bytes, out});
-    } else {
-      uint8_t* packed = ctx->out[0].get<uint8_t>((size_t)count * NP);
-      launch(st, count, PackP256Task{bytes, packed});
-      copy_d2h(st, out, packed, (size_t)count * NP);
-    }
+    launch(st, count, PackP256Task{bytes, packed});
+    o.copy_back(st, 0, packed, count);
     sync(st);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 
@@ -1030,54 +1098,55 @@ int zka_field_op_batch(zka_ctx* ctx, int field, int op, uint32_t count, const ui
                        uint8_t* out) {
   if (!ctx || !a || !out || field < 0 || field > 2 || op < 0 || op > 4 || (op < 3 && !b)) return ZKA_E_ARG;
   if (count == 0) return 0;
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
+    Cursor in(ctx->in[0]), ob(ctx->out[0]);
     const int nb = field == 2 ? WCB : 32;
-    const uint8_t* da = stage_in(ctx, ctx->in[0], a, (size_t)count * nb);
-    const uint8_t* db = b ? stage_in(ctx, ctx->in[1], b, (size_t)count * nb) : nullptr;
-    uint8_t* dout = is_device_ptr(out) ? out : ctx->out[0].get<uint8_t>((size_t)count * nb);
+    const uint8_t* da = stage_in(st, in.next(), a, (size_t)count * nb);
+    const uint8_t* db = stage_in(st, in.next(), b, (size_t)count * nb);
+    const Output<uint8_t> o(out, nb);
+    uint8_t* dout = o.rows(ob.next(), 0, count);
     if (field == 0) launch(st, count, FieldOpTask<P256p, 32>{da, db, dout, op});
     else if (field == 1) launch(st, count, FieldOpTask<P256n, 32>{da, db, dout, op});
     else launch(st, count, FieldOpTask<PGp, WCB>{da, db, dout, op});
-    if (dout != out) copy_d2h(st, out, dout, (size_t)count * nb);
+    o.copy_back(st, 0, dout, count);
     sync(st);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 int zka_hash80_batch(zka_ctx* ctx, uint32_t count, const uint8_t* msgs, size_t msg_stride, const uint32_t* len,
                      uint8_t* out) {
   if (!ctx || !msgs || !len || !out) return ZKA_E_ARG;
   if (count == 0) return 0;
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    const uint8_t* dm = stage_in(ctx, ctx->in[0], msgs, (size_t)count * msg_stride);
-    const uint32_t* dl = stage_in(ctx, ctx->in[1], len, (size_t)count);
-    uint8_t* dout = is_device_ptr(out) ? out : ctx->out[0].get<uint8_t>((size_t)count * 10);
+    Cursor in(ctx->in[0]), ob(ctx->out[0]);
+    const uint8_t* dm = stage_in(st, in.next(), msgs, (size_t)count * msg_stride);
+    const uint32_t* dl = stage_in(st, in.next(), len, (size_t)count);
+    const Output<uint8_t> o(out, 10);
+    uint8_t* dout = o.rows(ob.next(), 0, count);
     launch(st, count, Hash80Task{dm, msg_stride, dl, dout});
-    if (dout != out) copy_d2h(st, out, dout, (size_t)count * 10);
+    o.copy_back(st, 0, dout, count);
     sync(st);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 int zka_params_generate(zka_ctx* ctx, const uint8_t rnd[64], uint8_t h_nist[65], uint8_t h_proof[67]) {
   if (!ctx || !rnd || !h_nist || !h_proof) return ZKA_E_ARG;
-  try {
+  return guarded(ctx, [&] {
     // h_nist = G * rnd0 (pedersen.ts:66-67 on p256); h_proof = g * rnd1 + 0 * g
     int rc = zka_p256_mul_batch(ctx, 1, nullptr, rnd, h_nist);
     if (rc) return rc;
     Stream& st = ctx->st;
-    uint32_t* jv = ctx->w[0].get<uint32_t>(8);
-    uint32_t* jr = ctx->w[1].get<uint32_t>(8);
-    uint32_t* proj = ctx->w[2].get<uint32_t>(TOM_PROJ_WORDS);
-    uint32_t* aff = ctx->w[3].get<uint32_t>(TOM_AFF_WORDS);
-    uint8_t* bytes = ctx->w[4].get<uint8_t>(BSTRIDE);
-    uint8_t* d_rnd = ctx->in[0].get<uint8_t>(32);
+    Cursor in(ctx->in[0]), w(ctx->w);
+    uint32_t* jv = w.take<uint32_t>(8);
+    uint32_t* jr = w.take<uint32_t>(8);
+    uint32_t* proj = w.take<uint32_t>(TOM_PROJ_WORDS);
+    uint32_t* aff = w.take<uint32_t>(TOM_AFF_WORDS);
+    uint8_t* bytes = w.take<uint8_t>(BSTRIDE);
+    uint8_t* d_rnd = in.take<uint8_t>(32);
     copy_h2d(st, d_rnd, rnd + 32, 32);
     launch(st, 1, GenConvTask{d_rnd, jv, jr});
     // v*g + 0*g: use the g table for both bases
@@ -1086,33 +1155,30 @@ int zka_params_generate(zka_ctx* ctx, const uint8_t rnd[64], uint8_t h_nist[65],
     copy_d2h(st, h_proof, bytes, WP);
     sync(st);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 int zka_key_to_int(zka_ctx* ctx, uint32_t count, const uint8_t* pk, uint8_t* x_out, int32_t* status) {
   if (!ctx || !pk || !x_out) return ZKA_E_ARG;
   if (count == 0) return 0;
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    const uint8_t* dp = stage_in(ctx, ctx->in[0], pk, (size_t)count * 65);
-    uint32_t* aff = ctx->w[0].get<uint32_t>((size_t)count * 16);
-    uint8_t* bad = ctx->w[1].get<uint8_t>(count);
-    uint8_t* inf = ctx->w[2].get<uint8_t>(count);
-    uint8_t* dx = ctx->out[0].get<uint8_t>((size_t)count * 32);
-    int32_t* ds = ctx->out[1].get<int32_t>(count);
+    Cursor in(ctx->in[0]), w(ctx->w), ob(ctx->out[0]);
+    const uint8_t* dp = stage_in(st, in.next(), pk, (size_t)count * 65);
+    uint32_t* aff = w.take<uint32_t>((size_t)count * 16);
+    uint8_t* bad = w.take<uint8_t>(count);
+    uint8_t* inf = w.take<uint8_t>(count);
+    const Output<uint8_t> xo(x_out, 32);
+    const Output<int32_t> so(status, 1);   // status is optional: without it the statuses stay in the staging buffer
+    uint8_t* dx = xo.rows(ob.next(), 0, count);
+    int32_t* ds = so.rows(ob.next(), 0, count);
     launch(st, count, ParsePointsTask{dp, nullptr, aff, nullptr, bad, inf});
     launch(st, count, KeyToIntTask{aff, bad, inf, dx, ds});
-    if (is_device_ptr(x_out)) copy_d2d(st, x_out, dx, (size_t)count * 32); else copy_d2h(st, x_out, dx, (size_t)count * 32);
-    if (status) {
-      if (is_device_ptr(status)) copy_d2d(st, status, ds, (size_t)count * 4); else copy_d2h(st, status, ds, (size_t)count * 4);
-    }
+    xo.copy_back(st, 0, dx, count);
+    if (status) so.copy_back(st, 0, ds, count);
     sync(st);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 // ------------------------------------------------------------------------------- prove
@@ -1132,26 +1198,18 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
   const int n = mode == 0 ? ceil_log2(N) : 0;
   if (proof_stride < (mode == 0 ? zka_proof_max_len(N, S) : (size_t)S * REP0_LEN)) return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len");
   if (tape_stride < (size_t)32 * (mode == 0 ? prove_draws(0, n, S) : draws_before_items(S))) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
-  try {
+  return guarded(ctx, [&] {
     // ring + Lagrange matrix: once per call, on lane 0, finished before the lanes start
+    const uint32_t* ring_m = nullptr;
     if (mode == 0) {
-      Stream& st0 = ctx->st;
-      const uint8_t* d_ring = stage_in(st0, ctx->ring_in, ring, (size_t)N * 32);
-      uint32_t* rm = ctx->ring_m.get<uint32_t>(((size_t)1 << n) * 8);
-      launch(st0, 1ll << n, RingPrepTask{d_ring, rm, (int)N});
-      if (ctx->lag_n != n) {   // depends only on n, cached per context
-        uint32_t* l = ctx->lag.get<uint32_t>((size_t)n * n * 8);
-        launch(st0, 1, GkLagrangeTask{l, n});
-        ctx->lag_n = n;
-      }
-      sync(st0);
+      ring_m = prep_ring(ctx, ctx->st, ring, N, n, true);
+      sync(ctx->st);
     }
-    const uint32_t* ring_m = (const uint32_t*)ctx->ring_m.p;
-    uint32_t* lag = (uint32_t*)ctx->lag.p;
-    const bool out_dev = is_device_ptr(proofs);
-    const bool len_dev = is_device_ptr(proof_len_out), st_dev = is_device_ptr(status);
+    const Output<uint8_t> po(proofs, proof_stride);
+    const Output<uint32_t> lo(proof_len_out, 1);
+    const Output<int32_t> so(status, 1);
     const int lanes = ctx->nlanes;
-    const bool all_dev = out_dev && is_device_ptr(tape);
+    const bool all_dev = po.dev && is_device_ptr(tape);
     const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)(all_dev ? ctx->chunk : std::min(ctx->chunk, ctx->host_chunk)), lanes, !all_dev);
     const uint32_t nchunks = (uint32_t)off.size() - 1;
     const int used = (int)std::min<uint32_t>((uint32_t)lanes, nchunks);
@@ -1165,31 +1223,31 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
     auto run_lane = [&](int li) {
       Lane& ln = ctx->lane(li);
       Stream& st = ln.st;
-      DevBuf* W = ln.w;
       struct ChunkIn { const uint8_t *msg_hash, *sig, *pk, *tape, *base, *s_in, *q_in; const uint32_t* which; } cin[2];
       auto issue_inputs = [&](uint32_t k, int slot) {
         const uint32_t b0 = off[k];
         const size_t Bc = off[k + 1] - b0;
         Stream& ci = ln.cs_in;
-        DevBuf* in = ln.in + 5 * slot;
+        Cursor in(ln.in[slot]);
+        DevBuf& tape_buf = in.next();   // first, like the verifier's proof rows: the largest inputs share one buffer
+        auto rows = [&](auto* p, size_t width) { return stage_in(ci, in.next(), p ? p + b0 * width : p, Bc * width); };
         ev_wait(ci, ln.ev_done[slot]);   // the chunk that used these staging buffers before has finished reading them
-        cin[slot].msg_hash = msg_hash ? stage_in(ci, in[0], msg_hash + (size_t)b0 * 32, Bc * 32) : nullptr;
-        cin[slot].sig = sig ? stage_in(ci, in[1], sig + (size_t)b0 * 64, Bc * 64) : nullptr;
-        cin[slot].pk = stage_in(ci, in[2], pk + (size_t)b0 * 65, Bc * 65);
-        cin[slot].which = which ? stage_in(ci, in[3], which + b0, Bc) : nullptr;
-        DevBuf* inx = ln.in + 10 + 3 * slot;
-        cin[slot].base = base ? stage_in(ci, inx[0], base + (size_t)b0 * 65, Bc * 65) : nullptr;
-        cin[slot].s_in = s_in ? stage_in(ci, inx[1], s_in + (size_t)b0 * 32, Bc * 32) : nullptr;
-        cin[slot].q_in = q_in ? stage_in(ci, inx[2], q_in + (size_t)b0 * 65, Bc * 65) : nullptr;
+        cin[slot].msg_hash = rows(msg_hash, 32);
+        cin[slot].sig = rows(sig, 64);
+        cin[slot].pk = rows(pk, 65);
+        cin[slot].which = rows(which, 1);
+        cin[slot].base = rows(base, 65);
+        cin[slot].s_in = rows(s_in, 32);
+        cin[slot].q_in = rows(q_in, 65);
         ev_record(ln.ev_small[slot], ci);
         if (is_device_ptr(tape)) {
           cin[slot].tape = tape + (size_t)b0 * tape_stride;
         } else if (!ctx->tape_split) {
-          cin[slot].tape = stage_in(ci, in[4], tape + (size_t)b0 * tape_stride, Bc * tape_stride);
+          cin[slot].tape = stage_in(ci, tape_buf, tape + (size_t)b0 * tape_stride, Bc * tape_stride);
         } else {
           // host tape: only the draws used before the challenge (3 + 4S of up to 3 + 44S + 5n) travel now; the
           // item and GK draws of each proof follow after the challenge, when their number is known
-          uint8_t* dt = in[4].get<uint8_t>(Bc * tape_stride);
+          uint8_t* dt = tape_buf.get<uint8_t>(Bc * tape_stride);
           const size_t pre = std::min(tape_stride, (size_t)32 * draws_before_items(S));
           copy_d2h_2d(ci, dt, tape_stride, tape + (size_t)b0 * tape_stride, tape_stride, pre, Bc);
           cin[slot].tape = dt;
@@ -1210,12 +1268,9 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         const double t_begin = ms_now();
         ev_wait(st, ln.ev_small[slot]);
         ev_wait(st, ln.ev_out[slot]);    // the proofs of chunk k-2 have left the output staging buffers
-        ProveCtx c;
-        memset(&c, 0, sizeof(c));
-        c.B = Bc; c.S = S; c.N = (int)N; c.n = n; c.M = 0;
+        ProveCtx c = prove_ctx(ctx, P, Bc, S, (int)N, n);
         c.mode = mode; c.head_len = mode == 0 ? HEAD_LEN : 0;
         c.base = cin[slot].base; c.s_in = cin[slot].s_in; c.q_in = cin[slot].q_in;
-        c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
         c.msg_hash = cin[slot].msg_hash;
         c.sig = cin[slot].sig;
         c.pk = cin[slot].pk;
@@ -1224,54 +1279,51 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         c.tape_stride = tape_stride;
         c.tape_draws = (uint32_t)(tape_stride / 32);
         c.ring_m = ring_m;
-        c.g_tab8 = ctx->g8.tab; c.h_tab8 = P->h8.tab; c.h_w = P->h_w;
-        c.g_tabw = ctx->gw.tab; c.g_w = ctx->p256_hw;
-        c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
-        c.tg_bytes = (const uint8_t*)ctx->tg_bytes.p;
         const size_t S1 = (size_t)S + 1;
         const size_t nA = (size_t)Bc * S1;
         const size_t n1 = (size_t)Bc * (2 + 2 * S);
-        c.s1 = W[0].get<uint32_t>((size_t)Bc * 8);
-        c.pk_aff = W[1].get<uint32_t>((size_t)Bc * 16);
-        c.q_aff = W[2].get<uint32_t>((size_t)Bc * 16);
-        c.q_inf = W[3].get<uint8_t>(Bc);
-        c.r_aff = W[4].get<uint32_t>((size_t)Bc * 16);
-        c.r_bytes = W[5].get<uint8_t>((size_t)Bc * BSTRIDE);
-        c.rpows = W[6].get<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
-        c.rrows = W[7].get<uint32_t>((size_t)Bc * KEY_CAP * P256_PROJ_WORDS);
-        c.rtab = W[8].get<uint32_t>((size_t)Bc * KEY_CAP * P256_AFF_WORDS);
-        c.pa_T = W[9].get<uint32_t>(nA * P256_PROJ_WORDS);
-        c.pa_A = W[10].get<uint32_t>(nA * P256_PROJ_WORDS);
-        c.pa_T_aff = W[11].get<uint32_t>(nA * 16);
-        c.pa_T_inf = W[12].get<uint8_t>(nA);
-        c.pa_A_aff = W[13].get<uint32_t>(nA * 16);
-        c.pa_A_bytes = W[14].get<uint8_t>(nA * BSTRIDE);
-        c.pa_A_inf = W[15].get<uint8_t>(nA);
-        c.s1_jv = W[16].get<uint32_t>(n1 * 8);
-        c.s1_jr = W[17].get<uint32_t>(n1 * 8);
-        c.s1_proj = W[18].get<uint32_t>(n1 * TOM_PROJ_WORDS);
-        c.s1_aff = W[19].get<uint32_t>(n1 * TOM_AFF_WORDS);
-        c.s1_bytes = W[20].get<uint8_t>(n1 * BSTRIDE);
-        c.chal = W[21].get<uint32_t>((size_t)Bc * 3);
-        c.zcount = W[22].get<uint32_t>(Bc);
-        c.item_base = W[23].get<uint32_t>(Bc);
-        c.item_total = W[24].get<uint32_t>(2);
-        c.rep_off = W[25].get<uint32_t>((size_t)Bc * S);
-        c.gk_off = W[26].get<uint32_t>(Bc);
-        c.gk_dv = W[27].get<uint32_t>((size_t)Bc * n * 8);
-        c.gk_lag = lag;
-        c.gk_x = W[28].get<uint32_t>((size_t)Bc * 3);
-        c.u12 = W[46].get<uint32_t>((size_t)Bc * 16);
-        c.tab_of = W[48].get<uint32_t>(Bc);
-        c.tab_rep = W[49].get<uint32_t>((size_t)Bc * 2);
-        c.tab_count = W[50].get<uint32_t>(2);
-        c.which_s = W[52].get<uint32_t>(Bc);
-        c.base_aff = mode == 0 ? c.pk_aff : W[53].get<uint32_t>((size_t)Bc * 16);
+        Cursor w(ln.w);
+        c.s1 = w.take<uint32_t>((size_t)Bc * 8);
+        c.pk_aff = w.take<uint32_t>((size_t)Bc * 16);
+        c.q_aff = w.take<uint32_t>((size_t)Bc * 16);
+        c.q_inf = w.take<uint8_t>(Bc);
+        c.r_aff = w.take<uint32_t>((size_t)Bc * 16);
+        c.r_bytes = w.take<uint8_t>((size_t)Bc * BSTRIDE);
+        c.rpows = w.take<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
+        c.rrows = w.take<uint32_t>((size_t)Bc * KEY_CAP * P256_PROJ_WORDS);
+        c.rtab = w.take<uint32_t>((size_t)Bc * KEY_CAP * P256_AFF_WORDS);
+        c.pa_T = w.take<uint32_t>(nA * P256_PROJ_WORDS);
+        c.pa_A = w.take<uint32_t>(nA * P256_PROJ_WORDS);
+        c.pa_T_aff = w.take<uint32_t>(nA * 16);
+        c.pa_T_inf = w.take<uint8_t>(nA);
+        c.pa_A_aff = w.take<uint32_t>(nA * 16);
+        c.pa_A_bytes = w.take<uint8_t>(nA * BSTRIDE);
+        c.pa_A_inf = w.take<uint8_t>(nA);
+        c.s1_jv = w.take<uint32_t>(n1 * 8);
+        c.s1_jr = w.take<uint32_t>(n1 * 8);
+        c.s1_proj = w.take<uint32_t>(n1 * TOM_PROJ_WORDS);
+        c.s1_aff = w.take<uint32_t>(n1 * TOM_AFF_WORDS);
+        c.s1_bytes = w.take<uint8_t>(n1 * BSTRIDE);
+        c.chal = w.take<uint32_t>((size_t)Bc * 3);
+        c.zcount = w.take<uint32_t>(Bc);
+        c.item_base = w.take<uint32_t>(Bc);
+        c.item_total = w.take<uint32_t>(2);
+        c.rep_off = w.take<uint32_t>((size_t)Bc * S);
+        c.gk_off = w.take<uint32_t>(Bc);
+        c.gk_dv = w.take<uint32_t>((size_t)Bc * n * 8);
+        c.gk_x = w.take<uint32_t>((size_t)Bc * 3);
+        c.u12 = w.take<uint32_t>((size_t)Bc * 16);
+        c.tab_of = w.take<uint32_t>(Bc);
+        c.tab_rep = w.take<uint32_t>((size_t)Bc * 2);
+        c.tab_count = w.take<uint32_t>(2);
+        c.which_s = w.take<uint32_t>(Bc);
+        uint32_t* base_aff = w.take_if<uint32_t>(mode == 1, (size_t)Bc * 16);
+        c.base_aff = mode == 0 ? c.pk_aff : base_aff;
         c.proof_stride = proof_stride;
-        DevBuf* ob = ln.out + 3 * slot;
-        c.proofs = out_dev ? proofs + (size_t)b0 * proof_stride : ob[0].get<uint8_t>((size_t)Bc * proof_stride);
-        c.proof_len = len_dev ? proof_len_out + b0 : ob[1].get<uint32_t>(Bc);
-        c.status = st_dev ? status + b0 : ob[2].get<int32_t>(Bc);
+        Cursor ob(ln.out[slot]);
+        c.proofs = po.rows(ob.next(), b0, Bc);
+        c.proof_len = lo.rows(ob.next(), b0, Bc);
+        c.status = so.rows(ob.next(), b0, Bc);
   
         // --- statement + per-proof tables of pk, then R = u1*G + u2*pk on the tables
         launch(st, Bc, PreKeyTask{c});
@@ -1307,9 +1359,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         launch_p256_norm(st, c.pa_T, c.pa_T_aff, nullptr, c.pa_T_inf, (long long)(nA));
         launch_p256_norm(st, c.pa_A, c.pa_A_aff, c.pa_A_bytes, c.pa_A_inf, (long long)(nA));
         if (mode == 1) launch(st, Bc, ExpStatementTask{c});
-        launch(st, (long long)n1, JobsATask{c});
-        launch(st, (long long)n1, TomCommitTask{c.s1_jv, c.s1_jr, c.tg_tab, c.th_tab, c.s1_proj, c.tom_w, c.tom_nwin});
-        launch_tom_norm(st, c.s1_proj, c.s1_aff, c.s1_bytes, (long long)(n1), 1);
+        prove_store1(st, c);
         // --- challenge, layout
         launch(st, Bc, ExpChallengeTask{c});
         launch(st, 1, ScanTask{c});
@@ -1335,68 +1385,43 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         const size_t max_len = mode == 0 ? (size_t)proof_len((int)tot2[1], n, S)
                                          : (size_t)tot2[1] * REP0_LEN + (size_t)(S - (int)tot2[1]) * REP1_LEN;
         c.M = (int)M;
-        c.item_b = W[29].get<uint32_t>(M);
-        c.item_i = W[30].get<uint32_t>(M);
-        c.item_k = W[31].get<uint32_t>(M);
-        c.pb_T1 = W[32].get<uint32_t>((size_t)M * P256_PROJ_WORDS);
-        c.pb_T1_aff = W[33].get<uint32_t>((size_t)M * 16);
-        c.pb_T1_inf = W[34].get<uint8_t>(M);
+        c.item_b = w.take<uint32_t>(M);
+        c.item_i = w.take<uint32_t>(M);
+        c.item_k = w.take<uint32_t>(M);
+        c.pb_T1 = w.take<uint32_t>((size_t)M * P256_PROJ_WORDS);
+        c.pb_T1_aff = w.take<uint32_t>((size_t)M * 16);
+        c.pb_T1_inf = w.take<uint8_t>(M);
         const size_t n2 = c.s2_count();
-        c.s2_jv = W[35].get<uint32_t>(n2 * 8);
-        c.s2_jr = W[36].get<uint32_t>(n2 * 8);
-        c.s2_proj = W[37].get<uint32_t>(n2 * TOM_PROJ_WORDS);
-        c.s2_aff = W[38].get<uint32_t>(n2 * TOM_AFF_WORDS);
-        c.s2_bytes = W[39].get<uint8_t>(n2 * BSTRIDE);
-        c.secrets = W[42].get<uint32_t>((size_t)M * SECRETS_PER_ITEM * 8);
-        c.item_inv = W[47].get<uint32_t>((size_t)M * 8);
-        c.item_chal = W[43].get<uint32_t>((size_t)M * HASHES_PER_ITEM * 3);
+        c.s2_jv = w.take<uint32_t>(n2 * 8);
+        c.s2_jr = w.take<uint32_t>(n2 * 8);
+        c.s2_proj = w.take<uint32_t>(n2 * TOM_PROJ_WORDS);
+        c.s2_aff = w.take<uint32_t>(n2 * TOM_AFF_WORDS);
+        c.s2_bytes = w.take<uint8_t>(n2 * BSTRIDE);
+        c.secrets = w.take<uint32_t>((size_t)M * SECRETS_PER_ITEM * 8);
+        c.item_inv = w.take<uint32_t>((size_t)M * 8);
+        c.item_chal = w.take<uint32_t>((size_t)M * HASHES_PER_ITEM * 3);
+        c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * n * gk_blocks(n) * 8);
+        uint32_t* gext = w.take<uint32_t>((size_t)M * GJOBS_PER_ITEM * TOM_EXT_WORDS);
         launch(st, Bc, ItemsTask{c});
         // --- phase B
         launch(st, M, PhaseBP256Task{c});
         launch_p256_norm(st, c.pb_T1, c.pb_T1_aff, nullptr, c.pb_T1_inf, (long long)(M));
-        launch(st, ((long long)M + ITEM_INV_CHUNK - 1) / ITEM_INV_CHUNK, ItemInvTask{c});
-        launch(st, M, ItemScalarsTask{c});
-        launch(st, (long long)Bc * n, GkJobsTask{c});
-        {
-          const int nblk = 1 << (n - gk_block_bits(n));
-          c.gk_part = nblk > 1 ? W[51].get<uint32_t>((size_t)Bc * n * nblk * 8) : nullptr;
-          launch(st, (long long)Bc * n * nblk, GkPolyTask{c});
-          if (nblk > 1) launch(st, (long long)Bc * n, GkPolyReduceTask{c});
-        }
-        launch(st, (long long)Bc * n, GkCdJobsTask{c});
-        {
-          const size_t nj = (size_t)M * JOBS_PER_ITEM, nd = (size_t)M * DERS_PER_ITEM, ng = (size_t)Bc * 4 * n;
-          const size_t g0 = nj + nd;
-          // item jobs: g-parts once per distinct committed value, then r*h on top (TomCommitG/HTask)
-          uint32_t* gext = W[45].get<uint32_t>((size_t)M * GJOBS_PER_ITEM * TOM_EXT_WORDS);
-          launch(st, (long long)M * GJOBS_PER_ITEM, TomCommitGTask{c.s2_jv, c.tg_tab, gext, c.tom_w, c.tom_nwin});
-          launch(st, (long long)nj, TomCommitHTask{c.s2_jr, c.th_tab, gext, c.s2_proj, c.tom_w, c.tom_nwin});
-          launch(st, (long long)ng, TomCommitTask{c.s2_jv + g0 * 8, c.s2_jr + g0 * 8, c.tg_tab, c.th_tab,
-                                                   c.s2_proj + g0 * TOM_PROJ_WORDS, c.tom_w, c.tom_nwin});
-          // only T1x, T1y (jobs 0, 1 of each item) are needed again as points (DerivedTask)
-          launch_tom_norm(st, c.s2_proj, c.s2_aff, c.s2_bytes, (long long)(nj), 1, JOBS_PER_ITEM, 2);
-          launch(st, M, DerivedTask{c});
-          // derived points come from complete E1 additions, the GK commitments from the commit kernel (E2)
-          launch_tom_norm(st, c.s2_proj + nj * TOM_PROJ_WORDS, nullptr, c.s2_bytes + nj * BSTRIDE, (long long)nd, 0);
-          launch_tom_norm(st, c.s2_proj + g0 * TOM_PROJ_WORDS, nullptr, c.s2_bytes + g0 * BSTRIDE, (long long)ng, 1);
-        }
-        launch(st, (long long)M * HASHES_PER_ITEM, ItemHashTask{c});
-        launch(st, (long long)M * 7, ItemEmitTask{c});
+        prove_items_gk(st, c, gext, true, true);
         launch(st, (long long)nA, RepEmitTask{c});
         if (mode == 0) launch(st, Bc, GkEmitTask{c});
         launch(st, (long long)Bc * FIN_PARTS, FinalizeTask{c});
         // --- results: on the output stream, behind this chunk's last kernel
         ev_record(ln.ev_done[slot], st);
         if (ctx->progress && k_this < ctx->progress_cap) notify_progress(st, ctx->progress + k_this);
-        if (!out_dev || !len_dev || !st_dev) {
+        if (!po.dev || !lo.dev || !so.dev) {
           Stream& co = ln.cs_out;
           ev_wait(co, ln.ev_done[slot]);
           // only the bytes up to the longest proof of the chunk are copied back (rows are stride-padded)
           // (one cudaMemcpyAsync per row with its exact length: 8192 driver calls per step cost more than
           // the ~25 % of padding they save)
-          if (!out_dev) copy_d2h_2d(co, proofs + (size_t)b0 * proof_stride, proof_stride, c.proofs, proof_stride, max_len, Bc);
-          if (!len_dev) copy_d2h(co, proof_len_out + b0, c.proof_len, (size_t)Bc * 4);
-          if (!st_dev) copy_d2h(co, status + b0, c.status, (size_t)Bc * 4);
+          po.copy_back_2d(co, b0, c.proofs, Bc, max_len);
+          lo.copy_back(co, b0, c.proof_len, Bc);
+          so.copy_back(co, b0, c.status, Bc);
           ev_record(ln.ev_out[slot], co);
         }
         if (trace) {
@@ -1414,9 +1439,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
     };
     run_lanes(ctx, used, run_lane);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 int zka_prove_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
@@ -1449,70 +1472,51 @@ int zka_prove_membership_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, co
   const int n = ceil_log2(N);
   if (proof_stride < (size_t)gk_len(n)) return fail(ctx, ZKA_E_ARG, "proof_stride < GK block length");
   if (tape_stride < (size_t)32 * 5 * n) return fail(ctx, ZKA_E_ARG, "tape_stride < 32 * 5n");
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    DevBuf* W = ctx->w;
-    const uint8_t* d_ring = stage_in(st, ctx->ring_in, ring, (size_t)N * 32);
-    uint32_t* ring_m = ctx->ring_m.get<uint32_t>(((size_t)1 << n) * 8);
-    launch(st, 1ll << n, RingPrepTask{d_ring, ring_m, (int)N});
-    if (ctx->lag_n != n) {
-      uint32_t* l = ctx->lag.get<uint32_t>((size_t)n * n * 8);
-      launch(st, 1, GkLagrangeTask{l, n});
-      ctx->lag_n = n;
-    }
+    const uint32_t* ring_m = prep_ring(ctx, st, ring, N, n, true);
+    const Output<uint8_t> po(proofs, proof_stride);
+    const Output<uint32_t> lo(proof_len, 1);
+    const Output<int32_t> so(status, 1);
     const size_t it_stride = 96 + tape_stride;   // internal tape: [pad, com.r, pad] then the caller's draws (S = 0: GK draws start at 3)
     const uint32_t chunk = 8192;
     for (uint32_t b0 = 0; b0 < B; b0 += chunk) {
       const int Bc = (int)std::min<uint32_t>(chunk, B - b0);
-      const uint8_t* d_cr = stage_in(st, ctx->in[0], com_r + (size_t)b0 * 32, (size_t)Bc * 32);
-      const uint32_t* d_idx = stage_in(st, ctx->in[1], index + b0, (size_t)Bc);
-      const uint8_t* d_tape = stage_in(st, ctx->in[2], tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
-      ProveCtx c;
-      memset(&c, 0, sizeof(c));
-      c.B = Bc; c.S = 0; c.N = (int)N; c.n = n; c.M = 0;
-      c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
+      Cursor in(ctx->in[0]), w(ctx->w), ob(ctx->out[0]);
+      const uint8_t* d_cr = stage_in(st, in.next(), com_r + (size_t)b0 * 32, (size_t)Bc * 32);
+      const uint32_t* d_idx = stage_in(st, in.next(), index + b0, (size_t)Bc);
+      const uint8_t* d_tape = stage_in(st, in.next(), tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
+      ProveCtx c = prove_ctx(ctx, P, Bc, 0, (int)N, n);
       c.which = d_idx;
       c.ring_m = ring_m;
-      c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
-      uint8_t* itape = W[0].get<uint8_t>((size_t)Bc * it_stride);
+      uint8_t* itape = w.take<uint8_t>((size_t)Bc * it_stride);
       c.tape = itape; c.tape_stride = it_stride; c.tape_draws = (uint32_t)(it_stride / 32);
-      c.which_s = W[1].get<uint32_t>(Bc);
-      c.zcount = W[2].get<uint32_t>(Bc);
-      c.gk_off = W[3].get<uint32_t>(Bc);
-      c.gk_dv = W[4].get<uint32_t>((size_t)Bc * n * 8);
-      c.gk_lag = (uint32_t*)ctx->lag.p;
-      c.gk_x = W[5].get<uint32_t>((size_t)Bc * 3);
+      c.which_s = w.take<uint32_t>(Bc);
+      c.zcount = w.take<uint32_t>(Bc);
+      c.gk_off = w.take<uint32_t>(Bc);
+      c.gk_dv = w.take<uint32_t>((size_t)Bc * n * 8);
+      c.gk_x = w.take<uint32_t>((size_t)Bc * 3);
       const size_t ng = (size_t)Bc * 4 * n;
-      c.s2_jv = W[6].get<uint32_t>(ng * 8);
-      c.s2_jr = W[7].get<uint32_t>(ng * 8);
-      c.s2_proj = W[8].get<uint32_t>(ng * TOM_PROJ_WORDS);
-      c.s2_bytes = W[9].get<uint8_t>(ng * BSTRIDE);
+      c.s2_jv = w.take<uint32_t>(ng * 8);
+      c.s2_jr = w.take<uint32_t>(ng * 8);
+      c.s2_proj = w.take<uint32_t>(ng * TOM_PROJ_WORDS);
+      c.s2_bytes = w.take<uint8_t>(ng * BSTRIDE);
+      c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * n * gk_blocks(n) * 8);
       c.proof_stride = proof_stride;
-      c.proofs = is_device_ptr(proofs) ? proofs + (size_t)b0 * proof_stride : ctx->out[0].get<uint8_t>((size_t)Bc * proof_stride);
-      c.proof_len = is_device_ptr(proof_len) ? proof_len + b0 : ctx->out[1].get<uint32_t>(Bc);
-      c.status = is_device_ptr(status) ? status + b0 : ctx->out[2].get<int32_t>(Bc);
+      c.proofs = po.rows(ob.next(), b0, Bc);
+      c.proof_len = lo.rows(ob.next(), b0, Bc);
+      c.status = so.rows(ob.next(), b0, Bc);
       launch(st, Bc, GkAloneSetupTask{c, d_cr, d_tape, tape_stride, itape});
-      launch(st, (long long)Bc * n, GkJobsTask{c});
-      {
-        const int nblk = 1 << (n - gk_block_bits(n));
-        c.gk_part = nblk > 1 ? W[10].get<uint32_t>((size_t)Bc * n * nblk * 8) : nullptr;
-        launch(st, (long long)Bc * n * nblk, GkPolyTask{c});
-        if (nblk > 1) launch(st, (long long)Bc * n, GkPolyReduceTask{c});
-      }
-      launch(st, (long long)Bc * n, GkCdJobsTask{c});
-      launch(st, (long long)ng, TomCommitTask{c.s2_jv, c.s2_jr, c.tg_tab, c.th_tab, c.s2_proj, c.tom_w, c.tom_nwin});
-      launch_tom_norm(st, c.s2_proj, nullptr, c.s2_bytes, (long long)ng, 1);
+      prove_items_gk(st, c, nullptr, false, true);
       launch(st, Bc, GkEmitTask{c});
       launch(st, (long long)Bc * FIN_PARTS, FinalizeTask{c});
-      if (!is_device_ptr(proofs)) copy_d2h_2d(st, proofs + (size_t)b0 * proof_stride, proof_stride, c.proofs, proof_stride, (size_t)gk_len(n), Bc);
-      if (!is_device_ptr(proof_len)) copy_d2h(st, proof_len + b0, c.proof_len, (size_t)Bc * 4);
-      if (!is_device_ptr(status)) copy_d2h(st, status + b0, c.status, (size_t)Bc * 4);
+      po.copy_back_2d(st, b0, c.proofs, Bc, (size_t)gk_len(n));
+      lo.copy_back(st, b0, c.proof_len, Bc);
+      so.copy_back(st, b0, c.status, Bc);
       sync(st);
     }
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 // proveEquality / proveMult alone (kind 0 / 1): see SubProveJobsTask
@@ -1523,36 +1527,35 @@ static int prove_sub(zka_ctx* ctx, const zka_params* P, int kind, uint32_t B, co
   const int ns = kind == 0 ? 3 : 6, nd = kind == 0 ? 3 : 7, J = kind == 0 ? SUBP_EQ_JOBS : SUBP_MULT_JOBS;
   const int nc = kind == 0 ? 2 : 3, plen = kind == 0 ? EQ_LEN : MULT_LEN;
   if (tape_stride < (size_t)32 * nd) return fail(ctx, ZKA_E_ARG, "tape_stride too small for this sub-proof");
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    DevBuf* W = ctx->w;
+    const Output<uint8_t> co(commitments, (size_t)nc * WP), po(proofs, plen);
+    const Output<int32_t> so(status, 1);
     const uint32_t chunk = 16384;
     for (uint32_t b0 = 0; b0 < B; b0 += chunk) {
       const int Bc = (int)std::min<uint32_t>(chunk, B - b0);
-      const uint8_t* d_sc = stage_in(st, ctx->in[0], scalars + (size_t)b0 * ns * 32, (size_t)Bc * ns * 32);
-      const uint8_t* d_tape = stage_in(st, ctx->in[1], tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
+      Cursor in(ctx->in[0]), w(ctx->w), ob(ctx->out[0]);
+      const uint8_t* d_sc = stage_in(st, in.next(), scalars + (size_t)b0 * ns * 32, (size_t)Bc * ns * 32);
+      const uint8_t* d_tape = stage_in(st, in.next(), tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
       const size_t nj = (size_t)Bc * J;
-      uint32_t* jv = W[0].get<uint32_t>(nj * 8);
-      uint32_t* jr = W[1].get<uint32_t>(nj * 8);
-      uint32_t* proj = W[2].get<uint32_t>(nj * TOM_PROJ_WORDS);
-      uint8_t* bytes = W[3].get<uint8_t>(nj * BSTRIDE);
-      const bool cd = is_device_ptr(commitments), pd = is_device_ptr(proofs), sd = is_device_ptr(status);
-      uint8_t* d_com = cd ? commitments + (size_t)b0 * nc * WP : ctx->out[0].get<uint8_t>((size_t)Bc * nc * WP);
-      uint8_t* d_prf = pd ? proofs + (size_t)b0 * plen : ctx->out[1].get<uint8_t>((size_t)Bc * plen);
-      int32_t* d_st = sd ? status + b0 : ctx->out[2].get<int32_t>(Bc);
+      uint32_t* jv = w.take<uint32_t>(nj * 8);
+      uint32_t* jr = w.take<uint32_t>(nj * 8);
+      uint32_t* proj = w.take<uint32_t>(nj * TOM_PROJ_WORDS);
+      uint8_t* bytes = w.take<uint8_t>(nj * BSTRIDE);
+      uint8_t* d_com = co.rows(ob.next(), b0, Bc);
+      uint8_t* d_prf = po.rows(ob.next(), b0, Bc);
+      int32_t* d_st = so.rows(ob.next(), b0, Bc);
       launch(st, Bc, SubProveJobsTask{kind, d_sc, d_tape, tape_stride, jv, jr, d_st});
       launch(st, (long long)nj, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, proj, ctx->tom_w, ctx->tom_nwin});
       launch_tom_norm(st, proj, nullptr, bytes, (long long)nj, 1);
       launch(st, Bc, SubProveEmitTask{kind, d_sc, d_tape, tape_stride, jr, bytes, d_com, d_prf, d_st});
-      if (!cd) copy_d2h(st, commitments + (size_t)b0 * nc * WP, d_com, (size_t)Bc * nc * WP);
-      if (!pd) copy_d2h(st, proofs + (size_t)b0 * plen, d_prf, (size_t)Bc * plen);
-      if (!sd) copy_d2h(st, status + b0, d_st, (size_t)Bc * 4);
+      co.copy_back(st, b0, d_com, Bc);
+      po.copy_back(st, b0, d_prf, Bc);
+      so.copy_back(st, b0, d_st, Bc);
       sync(st);
     }
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 int zka_prove_equality_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* scalars, const uint8_t* tape,
                              size_t tape_stride, uint8_t* commitments, uint8_t* proofs, int32_t* status) {
@@ -1569,85 +1572,69 @@ int zka_prove_pointadd_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, cons
   if (!ctx || !P || !points || !blinders || !tape || !commitments || !proofs || !status) return ZKA_E_ARG;
   if (B == 0) return 0;
   if (tape_stride < (size_t)32 * 38) return fail(ctx, ZKA_E_ARG, "tape_stride < 32 * 38");
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    DevBuf* W = ctx->w;
     const size_t it_stride = (size_t)32 * (9 + 38);
     const size_t row_stride = REP0_LEN;
+    const Output<uint8_t> co(commitments, 6 * WP), po(proofs, PA_LEN);
+    const Output<int32_t> so(status, 1);
     const uint32_t chunk = 8192;
     for (uint32_t b0 = 0; b0 < B; b0 += chunk) {
       const int Bc = (int)std::min<uint32_t>(chunk, B - b0);
-      const uint8_t* d_pts = stage_in(st, ctx->in[0], points + (size_t)b0 * 195, (size_t)Bc * 195);
-      const uint8_t* d_bl = stage_in(st, ctx->in[1], blinders + (size_t)b0 * 192, (size_t)Bc * 192);
-      const uint8_t* d_tape = stage_in(st, ctx->in[2], tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
-      ProveCtx c;
-      memset(&c, 0, sizeof(c));
-      c.B = Bc; c.S = 1; c.N = 2; c.n = 0; c.M = Bc; c.mode = 1; c.head_len = 0;
-      c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
-      c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
-      c.tg_bytes = (const uint8_t*)ctx->tg_bytes.p;
-      uint8_t* itape = W[0].get<uint8_t>((size_t)Bc * it_stride);
+      Cursor in(ctx->in[0]), w(ctx->w), ob(ctx->out[0]);
+      const uint8_t* d_pts = stage_in(st, in.next(), points + (size_t)b0 * 195, (size_t)Bc * 195);
+      const uint8_t* d_bl = stage_in(st, in.next(), blinders + (size_t)b0 * 192, (size_t)Bc * 192);
+      const uint8_t* d_tape = stage_in(st, in.next(), tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
+      ProveCtx c = prove_ctx(ctx, P, Bc, 1, 2, 0);
+      c.M = Bc; c.mode = 1; c.head_len = 0;
+      uint8_t* itape = w.take<uint8_t>((size_t)Bc * it_stride);
       c.tape = itape; c.tape_stride = it_stride; c.tape_draws = (uint32_t)(it_stride / 32);
       const size_t n1 = (size_t)Bc * 4, n2 = (size_t)Bc * (JOBS_PER_ITEM + DERS_PER_ITEM);
-      c.s1 = W[1].get<uint32_t>((size_t)Bc * 8);
-      c.pk_aff = W[2].get<uint32_t>((size_t)Bc * 16);
-      c.pa_T_aff = W[3].get<uint32_t>((size_t)Bc * 2 * 16);
-      c.pa_T_inf = W[4].get<uint8_t>((size_t)Bc * 2);
-      c.pa_A_inf = W[5].get<uint8_t>((size_t)Bc * 2);
-      c.pb_T1_aff = W[6].get<uint32_t>((size_t)Bc * 16);
-      c.pb_T1_inf = W[7].get<uint8_t>(Bc);
-      c.chal = W[8].get<uint32_t>((size_t)Bc * 3);
-      c.zcount = W[9].get<uint32_t>(Bc);
-      c.item_base = W[10].get<uint32_t>(Bc);
-      c.item_b = W[11].get<uint32_t>(Bc);
-      c.item_i = W[12].get<uint32_t>(Bc);
-      c.item_k = W[13].get<uint32_t>(Bc);
-      c.rep_off = W[14].get<uint32_t>(Bc);
-      c.s1_jv = W[15].get<uint32_t>(n1 * 8);
-      c.s1_jr = W[16].get<uint32_t>(n1 * 8);
-      c.s1_proj = W[17].get<uint32_t>(n1 * TOM_PROJ_WORDS);
-      c.s1_aff = W[18].get<uint32_t>(n1 * TOM_AFF_WORDS);
-      c.s1_bytes = W[19].get<uint8_t>(n1 * BSTRIDE);
-      c.s2_jv = W[20].get<uint32_t>(n2 * 8);
-      c.s2_jr = W[21].get<uint32_t>(n2 * 8);
-      c.s2_proj = W[22].get<uint32_t>(n2 * TOM_PROJ_WORDS);
-      c.s2_aff = W[23].get<uint32_t>(n2 * TOM_AFF_WORDS);
-      c.s2_bytes = W[24].get<uint8_t>(n2 * BSTRIDE);
-      c.secrets = W[25].get<uint32_t>((size_t)Bc * SECRETS_PER_ITEM * 8);
-      c.item_inv = W[26].get<uint32_t>((size_t)Bc * 8);
-      c.item_chal = W[27].get<uint32_t>((size_t)Bc * HASHES_PER_ITEM * 3);
-      uint32_t* gext = W[28].get<uint32_t>((size_t)Bc * GJOBS_PER_ITEM * TOM_EXT_WORDS);
+      c.s1 = w.take<uint32_t>((size_t)Bc * 8);
+      c.pk_aff = w.take<uint32_t>((size_t)Bc * 16);
+      c.pa_T_aff = w.take<uint32_t>((size_t)Bc * 2 * 16);
+      c.pa_T_inf = w.take<uint8_t>((size_t)Bc * 2);
+      c.pa_A_inf = w.take<uint8_t>((size_t)Bc * 2);
+      c.pb_T1_aff = w.take<uint32_t>((size_t)Bc * 16);
+      c.pb_T1_inf = w.take<uint8_t>(Bc);
+      c.chal = w.take<uint32_t>((size_t)Bc * 3);
+      c.zcount = w.take<uint32_t>(Bc);
+      c.item_base = w.take<uint32_t>(Bc);
+      c.item_b = w.take<uint32_t>(Bc);
+      c.item_i = w.take<uint32_t>(Bc);
+      c.item_k = w.take<uint32_t>(Bc);
+      c.rep_off = w.take<uint32_t>(Bc);
+      c.s1_jv = w.take<uint32_t>(n1 * 8);
+      c.s1_jr = w.take<uint32_t>(n1 * 8);
+      c.s1_proj = w.take<uint32_t>(n1 * TOM_PROJ_WORDS);
+      c.s1_aff = w.take<uint32_t>(n1 * TOM_AFF_WORDS);
+      c.s1_bytes = w.take<uint8_t>(n1 * BSTRIDE);
+      c.s2_jv = w.take<uint32_t>(n2 * 8);
+      c.s2_jr = w.take<uint32_t>(n2 * 8);
+      c.s2_proj = w.take<uint32_t>(n2 * TOM_PROJ_WORDS);
+      c.s2_aff = w.take<uint32_t>(n2 * TOM_AFF_WORDS);
+      c.s2_bytes = w.take<uint8_t>(n2 * BSTRIDE);
+      c.secrets = w.take<uint32_t>((size_t)Bc * SECRETS_PER_ITEM * 8);
+      c.item_inv = w.take<uint32_t>((size_t)Bc * 8);
+      c.item_chal = w.take<uint32_t>((size_t)Bc * HASHES_PER_ITEM * 3);
+      uint32_t* gext = w.take<uint32_t>((size_t)Bc * GJOBS_PER_ITEM * TOM_EXT_WORDS);
       c.proof_stride = row_stride;
-      c.proofs = W[29].get<uint8_t>((size_t)Bc * row_stride);
-      c.proof_len = W[30].get<uint32_t>(Bc);
-      const bool cd = is_device_ptr(commitments), pd = is_device_ptr(proofs), sd = is_device_ptr(status);
-      c.status = sd ? status + b0 : ctx->out[2].get<int32_t>(Bc);
-      uint8_t* d_com = cd ? commitments + (size_t)b0 * 6 * WP : ctx->out[0].get<uint8_t>((size_t)Bc * 6 * WP);
-      uint8_t* d_prf = pd ? proofs + (size_t)b0 * PA_LEN : ctx->out[1].get<uint8_t>((size_t)Bc * PA_LEN);
+      c.proofs = w.take<uint8_t>((size_t)Bc * row_stride);
+      c.proof_len = w.take<uint32_t>(Bc);
+      uint8_t* d_com = co.rows(ob.next(), b0, Bc);
+      uint8_t* d_prf = po.rows(ob.next(), b0, Bc);
+      c.status = so.rows(ob.next(), b0, Bc);
       launch(st, Bc, PaddSetupTask{c, d_pts, d_bl, d_tape, tape_stride, itape});
-      launch(st, (long long)n1, JobsATask{c});
-      launch(st, (long long)n1, TomCommitTask{c.s1_jv, c.s1_jr, c.tg_tab, c.th_tab, c.s1_proj, c.tom_w, c.tom_nwin});
-      launch_tom_norm(st, c.s1_proj, c.s1_aff, c.s1_bytes, (long long)n1, 1);
-      launch(st, ((long long)Bc + ITEM_INV_CHUNK - 1) / ITEM_INV_CHUNK, ItemInvTask{c});
-      launch(st, Bc, ItemScalarsTask{c});
-      const size_t nj = (size_t)Bc * JOBS_PER_ITEM, nd = (size_t)Bc * DERS_PER_ITEM;
-      launch(st, (long long)Bc * GJOBS_PER_ITEM, TomCommitGTask{c.s2_jv, c.tg_tab, gext, c.tom_w, c.tom_nwin});
-      launch(st, (long long)nj, TomCommitHTask{c.s2_jr, c.th_tab, gext, c.s2_proj, c.tom_w, c.tom_nwin});
-      launch_tom_norm(st, c.s2_proj, c.s2_aff, c.s2_bytes, (long long)nj, 1, JOBS_PER_ITEM, 2);
-      launch(st, Bc, DerivedTask{c});
-      launch_tom_norm(st, c.s2_proj + nj * TOM_PROJ_WORDS, nullptr, c.s2_bytes + nj * BSTRIDE, (long long)nd, 0);
-      launch(st, (long long)Bc * HASHES_PER_ITEM, ItemHashTask{c});
-      launch(st, (long long)Bc * 7, ItemEmitTask{c});
+      prove_store1(st, c);
+      prove_items_gk(st, c, gext, true, false);
       launch(st, Bc, PaddExtractTask{c, d_com, d_prf});
-      if (!cd) copy_d2h(st, commitments + (size_t)b0 * 6 * WP, d_com, (size_t)Bc * 6 * WP);
-      if (!pd) copy_d2h(st, proofs + (size_t)b0 * PA_LEN, d_prf, (size_t)Bc * PA_LEN);
-      if (!sd) copy_d2h(st, status + b0, c.status, (size_t)Bc * 4);
+      co.copy_back(st, b0, d_com, Bc);
+      po.copy_back(st, b0, d_prf, Bc);
+      so.copy_back(st, b0, c.status, Bc);
       sync(st);
     }
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 size_t zka_verify_tape_len_ex(uint32_t ring_size, uint32_t sec_level, uint32_t samples) {
@@ -1689,15 +1676,14 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
   const int n = ceil_log2(N);
   if (tape_stride < (mode == 1 ? (size_t)V_IDX_PAD + (size_t)32 * 25 * K : verify_tape_len(n, S, K)))
     return fail(ctx, ZKA_E_ARG, "tape_stride < zka_verify_tape_len");
-  try {
+  return guarded(ctx, [&] {
+    const uint32_t* ring_m = nullptr;
     if (mode == 0) {
-      Stream& st0 = ctx->st;
-      const uint8_t* d_ring = stage_in(st0, ctx->ring_in, ring, (size_t)N * 32);
-      uint32_t* rm = ctx->ring_m.get<uint32_t>(((size_t)1 << n) * 8);
-      launch(st0, 1ll << n, RingPrepTask{d_ring, rm, (int)N});
-      sync(st0);
+      ring_m = prep_ring(ctx, ctx->st, ring, N, n, false);
+      sync(ctx->st);
     }
-    const uint32_t* ring_m = (const uint32_t*)ctx->ring_m.p;
+    const Output<uint8_t> oo(ok, 1);
+    const Output<int32_t> so(status, 1);
     const int lanes = ctx->nlanes;
     const bool all_dev = is_device_ptr(proofs) && is_device_ptr(tape);
     // (two equal chunks per lane instead of the tapered host schedule: no gain at batch 8192, slower at batch 1024)
@@ -1718,25 +1704,26 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       // full bandwidth (with a copy stream per lane the first chunks and the prefetched ones were all in flight at once).
       std::lock_guard<std::mutex> copy_lock(ctx->copy_mu);
       Stream& ci = ctx->cs_in;
-      DevBuf* in = ln.in + 8 * slot;
+      Cursor in(ln.in[slot]);
+      DevBuf& rows_buf = in.next();   // first, like the prover's tape: the largest inputs share one buffer
       const uint32_t b0 = off[kk];
       const size_t Bc = off[kk + 1] - b0;
       VIn v;
-      v.msg = msg_hash ? stage_in(ci, in[0], msg_hash + (size_t)b0 * 32, Bc * 32) : nullptr;
+      v.msg = stage_in(ci, in.next(), msg_hash ? msg_hash + (size_t)b0 * 32 : nullptr, Bc * 32);
       if (is_device_ptr(proofs) || is_device_ptr(proof_len)) {
-        v.proofs = stage_in(ci, in[1], proofs + (size_t)b0 * proof_stride, Bc * proof_stride);
+        v.proofs = stage_in(ci, rows_buf, proofs + (size_t)b0 * proof_stride, Bc * proof_stride);
       } else {
         // host rows: only the bytes up to the longest proof of the chunk cross PCIe (rows are stride-padded;
         // a length above the stride is rejected by VLayoutTask without reading the row)
         size_t w = 0;
         for (size_t i = 0; i < Bc; i++) w = std::max<size_t>(w, proof_len[b0 + i]);
         w = std::min(proof_stride, (w + 15) & ~(size_t)15);
-        uint8_t* dp = in[1].get<uint8_t>(Bc * proof_stride);
+        uint8_t* dp = rows_buf.get<uint8_t>(Bc * proof_stride);
         copy_d2h_2d(ci, dp, proof_stride, proofs + (size_t)b0 * proof_stride, proof_stride, w, Bc);
         v.proofs = dp;
       }
-      v.plen = stage_in(ci, in[2], proof_len + b0, Bc);
-      v.tape = stage_in(ci, in[4], tape + (size_t)b0 * tape_stride, Bc * tape_stride);
+      v.plen = stage_in(ci, in.next(), proof_len + b0, Bc);
+      v.tape = stage_in(ci, in.next(), tape + (size_t)b0 * tape_stride, Bc * tape_stride);
       ev_record(ln.ev_small[slot], ci);
       return v;
     };
@@ -1747,7 +1734,6 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
     auto run_lane = [&](int li) {
       Lane& ln = ctx->lane(li);
       Stream& st = ln.st;
-      DevBuf* W = ln.w;
       uint32_t k = (uint32_t)li;
       if (k >= nchunks) return;
       int slot = 0;
@@ -1762,11 +1748,8 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       const uint32_t b0 = off[k];
       const int Bc = (int)(off[k + 1] - b0);
       const double t_begin = trace ? ms_now() : 0.0;
-      VerifyCtx c;
-      memset(&c, 0, sizeof(c));
-      c.B = Bc; c.S = S; c.N = (int)N; c.n = n; c.K = K; c.mode = mode;
+      VerifyCtx c = verify_ctx(ctx, P, Bc, S, (int)N, n, K, mode);
       c.q_ext = q_ext ? q_ext + (size_t)b0 * NP : nullptr;
-      c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
       c.msg_hash = cur.msg;
       c.proofs = cur.proofs;
       c.proof_stride = proof_stride;
@@ -1774,59 +1757,62 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       c.tape = cur.tape;
       c.tape_stride = tape_stride;
       c.ring_m = ring_m;
-      c.g_tab8 = ctx->g8.tab; c.h_tab8 = P->h8.tab; c.h_w = P->h_w;
-      c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
-      c.tg_bytes = (const uint8_t*)ctx->tg_bytes.p;
       double t_in = 0.0;
       if (trace) { sync(st); t_in = ms_now(); }
       const size_t ns = (size_t)Bc * K;
       const int ET = c.ent_tom(), EN = c.ent_nist(), SG = c.segs();
       const int ngk = 4 * n + 1;
-      c.rep_off = W[0].get<uint32_t>((size_t)Bc * S);
-      c.gk_off = W[1].get<uint32_t>(Bc);
-      c.tagbits = W[2].get<uint32_t>((size_t)Bc * 3);
-      c.chal = W[3].get<uint32_t>((size_t)Bc * 3);
-      c.gk_ok_len = W[4].get<uint8_t>(Bc);
-      c.r_aff = W[5].get<uint32_t>((size_t)Bc * 16);
-      c.q_aff = W[6].get<uint32_t>((size_t)Bc * 16);
-      c.q_inf = W[7].get<uint8_t>(Bc);
-      c.rpows = W[8].get<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
-      c.rrows = W[9].get<uint32_t>((size_t)Bc * RT_ENTRIES * P256_PROJ_WORDS);
-      c.rtab = W[10].get<uint32_t>((size_t)Bc * RT_ENTRIES * P256_AFF_WORDS);
-      c.samp_idx = W[11].get<uint32_t>(ns);
-      c.samp_draw = W[12].get<uint32_t>(ns);
-      c.sp_T = W[13].get<uint32_t>(ns * P256_PROJ_WORDS);
-      c.sp_T_aff = W[14].get<uint32_t>(ns * 16);
-      c.sp_T_inf = W[15].get<uint8_t>(ns);
-      c.ta_jv = W[16].get<uint32_t>(ns * 2 * 8);
-      c.ta_jr = W[17].get<uint32_t>(ns * 2 * 8);
-      c.ta_proj = W[18].get<uint32_t>(ns * 2 * TOM_PROJ_WORDS);
-      c.ta_aff = W[19].get<uint32_t>(ns * 2 * TOM_AFF_WORDS);
-      c.td_proj = W[20].get<uint32_t>(ns * DERS_PER_ITEM * TOM_PROJ_WORDS);
-      c.td_aff = W[21].get<uint32_t>(ns * DERS_PER_ITEM * TOM_AFF_WORDS);
-      c.td_bytes = W[22].get<uint8_t>(ns * DERS_PER_ITEM * BSTRIDE);
-      c.item_chal = W[23].get<uint32_t>(ns * HASHES_PER_ITEM * 3);
-      c.ent_scalar = W[24].get<uint32_t>((size_t)Bc * ET * 8);
-      c.ent_off = W[25].get<uint32_t>((size_t)Bc * ET);
-      c.ent_pre = W[26].get<uint32_t>((size_t)Bc * ET * TOM_PRE_WORDS);
-      c.ent_cnt = W[27].get<uint32_t>(ns);
-      c.part = W[28].get<uint32_t>(ns * V_PART_WORDS);
-      c.nent_scalar = W[29].get<uint32_t>((size_t)Bc * EN * 8);
-      c.nent_aff = W[30].get<uint32_t>((size_t)Bc * EN * 16);
-      c.nent_skip = W[31].get<uint8_t>((size_t)Bc * EN);
-      c.gk_scalar = W[32].get<uint32_t>((size_t)Bc * ngk * 8);
-      c.gk_pre = W[33].get<uint32_t>((size_t)Bc * ngk * TOM_PRE_WORDS);
-      uint32_t* gk_offs = W[34].get<uint32_t>((size_t)Bc * ngk);
-      c.fx_jv = W[35].get<uint32_t>((size_t)Bc * 2 * 8);
-      c.fx_jr = W[36].get<uint32_t>((size_t)Bc * 2 * 8);
-      c.fx_proj = W[37].get<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
-      c.nfix = W[38].get<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
-      c.win_w = W[39].get<uint32_t>((size_t)Bc * SG * MSM_NWIN * 36);
-      c.win_g = W[42].get<uint32_t>((size_t)Bc * MSM_NWIN * 36);
-      c.win_n = W[43].get<uint32_t>((size_t)Bc * MSM_NWIN_N * P256_PROJ_WORDS);
-      c.id_flags = W[44].get<uint8_t>((size_t)Bc * 3);
-      c.ok = is_device_ptr(ok) ? ok + b0 : ln.out[0].get<uint8_t>(Bc);
-      c.status = is_device_ptr(status) ? status + b0 : ln.out[1].get<int32_t>(Bc);
+      Cursor w(ln.w);
+      c.rep_off = w.take<uint32_t>((size_t)Bc * S);
+      c.gk_off = w.take<uint32_t>(Bc);
+      c.tagbits = w.take<uint32_t>((size_t)Bc * 3);
+      c.chal = w.take<uint32_t>((size_t)Bc * 3);
+      c.gk_ok_len = w.take<uint8_t>(Bc);
+      c.r_aff = w.take<uint32_t>((size_t)Bc * 16);
+      c.q_aff = w.take<uint32_t>((size_t)Bc * 16);
+      c.q_inf = w.take<uint8_t>(Bc);
+      c.rpows = w.take<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
+      c.rrows = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_PROJ_WORDS);
+      c.rtab = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_AFF_WORDS);
+      c.samp_idx = w.take<uint32_t>(ns);
+      c.samp_draw = w.take<uint32_t>(ns);
+      c.sp_T = w.take<uint32_t>(ns * P256_PROJ_WORDS);
+      c.sp_T_aff = w.take<uint32_t>(ns * 16);
+      c.sp_T_inf = w.take<uint8_t>(ns);
+      c.ta_jv = w.take<uint32_t>(ns * 2 * 8);
+      c.ta_jr = w.take<uint32_t>(ns * 2 * 8);
+      c.ta_proj = w.take<uint32_t>(ns * 2 * TOM_PROJ_WORDS);
+      c.ta_aff = w.take<uint32_t>(ns * 2 * TOM_AFF_WORDS);
+      c.td_proj = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_PROJ_WORDS);
+      c.td_aff = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_AFF_WORDS);
+      c.td_bytes = w.take<uint8_t>(ns * DERS_PER_ITEM * BSTRIDE);
+      c.item_chal = w.take<uint32_t>(ns * HASHES_PER_ITEM * 3);
+      c.ent_scalar = w.take<uint32_t>((size_t)Bc * ET * 8);
+      c.ent_off = w.take<uint32_t>((size_t)Bc * ET);
+      c.ent_pre = w.take<uint32_t>((size_t)Bc * ET * TOM_PRE_WORDS);
+      c.ent_cnt = w.take<uint32_t>(ns);
+      c.part = w.take<uint32_t>(ns * V_PART_WORDS);
+      // the small per-proof arrays before the entries and windows: the prover of this lane has small arrays at the
+      // same places of the pool, so these share its buffers without growing them much
+      c.fx_jv = w.take<uint32_t>((size_t)Bc * 2 * 8);
+      c.fx_jr = w.take<uint32_t>((size_t)Bc * 2 * 8);
+      c.fx_proj = w.take<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
+      c.nfix = w.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
+      c.id_flags = w.take<uint8_t>((size_t)Bc * 3);
+      c.gk_tape_bad = w.take_if<uint8_t>(mode == 0, Bc);
+      c.nent_scalar = w.take<uint32_t>((size_t)Bc * EN * 8);
+      c.nent_aff = w.take<uint32_t>((size_t)Bc * EN * 16);
+      c.nent_skip = w.take<uint8_t>((size_t)Bc * EN);
+      c.gk_scalar = w.take<uint32_t>((size_t)Bc * ngk * 8);
+      c.gk_pre = w.take<uint32_t>((size_t)Bc * ngk * TOM_PRE_WORDS);
+      uint32_t* gk_offs = w.take<uint32_t>((size_t)Bc * ngk);
+      c.win_w = w.take<uint32_t>((size_t)Bc * SG * MSM_NWIN * 36);
+      c.win_g = w.take<uint32_t>((size_t)Bc * MSM_NWIN * 36);
+      c.win_n = w.take<uint32_t>((size_t)Bc * MSM_NWIN_N * P256_PROJ_WORDS);
+      c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * gk_blocks(n) * 8);
+      Cursor ob(ln.out[0]);
+      c.ok = oo.rows(ob.next(), b0, Bc);
+      c.status = so.rows(ob.next(), b0, Bc);
 
       launch(st, Bc, VLayoutTask{c});
       launch(st, (long long)Bc * (S + 1), VValidateTask{c});
@@ -1845,20 +1831,11 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       // the Groth-Kohlweiss chain (ring polynomial, relations, offsets) only needs the layout: it runs on a side stream
       // beside the sampled-repetition chain; its tape-range status is folded in by VReduceTask (same precedence)
       const bool gk_fork = mode == 0 && !st.profiling;
-      Stream& sg = gk_fork ? ln.aux[1] : st;
-      auto gk_chain = [&] {
-        const int nblk = 1 << (n - gk_block_bits(n));
-        c.gk_part = nblk > 1 ? W[51].get<uint32_t>((size_t)Bc * nblk * 8) : nullptr;
-        if (nblk > 1) launch(sg, (long long)Bc * nblk, VGkSumTask{c});
-        launch(sg, Bc, VGkTask{c});
-        launch(sg, (long long)Bc * ngk, VGkOffsetsTask{c, gk_offs});
-      };
-      if (mode == 0) c.gk_tape_bad = W[54].get<uint8_t>(Bc);
       if (gk_fork) {
         ev_record(ln.ev_fork, st);
-        ev_wait(sg, ln.ev_fork);
-        gk_chain();
-        ev_record(ln.ev_join[1], sg);
+        ev_wait(ln.aux[1], ln.ev_fork);
+        verify_gk(ln.aux[1], c, gk_offs);
+        ev_record(ln.ev_join[1], ln.aux[1]);
       }
       launch(st, (long long)ns, VSampleP256Task{c});
       launch_p256_norm(st, c.sp_T, c.sp_T_aff, nullptr, c.sp_T_inf, (long long)(ns));
@@ -1872,7 +1849,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       launch(st, (long long)ns, VRelationsTask{c});
       if (mode == 0) {
         if (gk_fork) ev_wait(st, ln.ev_join[1]);
-        else gk_chain();
+        else verify_gk(st, c, gk_offs);
       }
       launch(st, Bc, VReduceTask{c});
       launch(st, (long long)Bc * ET, VParseEntriesTask{c.proofs, proof_stride, c.ent_off, c.ent_pre, ET});
@@ -1883,8 +1860,18 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       // return at once
       uint32_t* ctl = nullptr;
       if (ctx->agg && mode == 0) {
-        DevBuf* A = ln.agg;
-        ctl = A[0].get<uint32_t>(AGG_CTL_WORDS);
+        Cursor A(ln.agg);
+        const int fgroups = (Bc * 2 + 63) / 64, ngroups = (Bc + 31) / 32, ngroups2 = (ngroups + 31) / 32;
+        ctl = A.take<uint32_t>(AGG_CTL_WORDS);
+#if !defined(ZKA_PG_WAR256)
+        uint32_t* tpart = A.take<uint32_t>((size_t)Bc * (K + 1) * 2 * PG_EXT_WORDS);
+#endif
+        uint32_t* fpart = A.take<uint32_t>((size_t)fgroups * 16);
+        uint32_t* fjv = A.take<uint32_t>(8);
+        uint32_t* fjr = A.take<uint32_t>(8);
+        uint32_t* fproj = A.take<uint32_t>(TOM_PROJ_WORDS);
+        uint32_t* npart = A.take<uint32_t>((size_t)ngroups * P256_PROJ_WORDS);
+        uint32_t* npart2 = A.take_if<uint32_t>(ngroups > 32, (size_t)ngroups2 * P256_PROJ_WORDS);
         dev_memset(st, ctl, 0, AGG_CTL_WORDS * 4);
         launch(st, Bc, AggGateTask{c, ctl});
         const AggTomSrc tsrc{c.ent_scalar, c.ent_pre, c.ent_cnt, c.gk_scalar, c.gk_pre, Bc, ET, K, ngk};
@@ -1902,25 +1889,17 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
           ev_wait(sb, ln.ev_fork);
         }
 #if !defined(ZKA_PG_WAR256)
-        {   // cofactor 4: no small-order components, or the per-proof path decides
-          uint32_t* tpart = A[46].get<uint32_t>((size_t)Bc * (K + 1) * 2 * PG_EXT_WORDS);
-          launch(sa, (long long)Bc * (K + 1) * 2, AggTorsionPartTask{tsrc, ctl, tpart});
-          launch(sa, Bc, AggTorsionTask{tpart, ctl, K});
-        }
+        // cofactor 4: no small-order components, or the per-proof path decides
+        launch(sa, (long long)Bc * (K + 1) * 2, AggTorsionPartTask{tsrc, ctl, tpart});
+        launch(sa, Bc, AggTorsionTask{tpart, ctl, K});
 #endif
         const AggPlan tp = agg_plan((double)Bc * (0.5 * K * V_ENT_PER_SAMPLE + 2 + ngk), ctx->agg_c);
         const AggPlan np = agg_plan((double)Bc * EN, 0);
         ctx->agg_c_last = tp.D.c;
         const uint32_t *tA, *tB, *nA, *nB;
-        agg_msm(st, A + 1, tsrc, tp, ctl, &tA, &tB);
-        agg_msm(sb, A + 20, nsrc, np, ctl, &nA, &nB);
+        agg_msm(st, Cursor(ln.agg_tom), tsrc, tp, ctl, &tA, &tB);
+        agg_msm(sb, Cursor(ln.agg_nist), nsrc, np, ctl, &nA, &nB);
         // fixed-base parts: one commitment for the summed tomEdwards256 scalars, a two-level sum of the P-256 points
-        const int fgroups = (Bc * 2 + 63) / 64, ngroups = (Bc + 31) / 32;
-        uint32_t* fpart = A[40].get<uint32_t>((size_t)fgroups * 16);
-        uint32_t* fjv = A[41].get<uint32_t>(8);
-        uint32_t* fjr = A[42].get<uint32_t>(8);
-        uint32_t* fproj = A[43].get<uint32_t>(TOM_PROJ_WORDS);
-        uint32_t* npart = A[44].get<uint32_t>((size_t)ngroups * P256_PROJ_WORDS);
         launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, fpart, Bc});
         launch(st, 1, AggFixSumTask{ctl, fpart, fjv, fjr, fgroups});
         launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom_w, c.tom_nwin});
@@ -1928,10 +1907,9 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
         int nleft = ngroups;            // second level: at most Bc / 1024 partial sums reach the final thread
         const uint32_t* nsum = npart;
         if (nleft > 32) {
-          uint32_t* npart2 = A[45].get<uint32_t>((size_t)((nleft + 31) / 32) * P256_PROJ_WORDS);
-          launch(sb, (nleft + 31) / 32, AggNistFixPartTask{ctl, npart, npart2, nleft});
+          launch(sb, ngroups2, AggNistFixPartTask{ctl, npart, npart2, nleft});
           nsum = npart2;
-          nleft = (nleft + 31) / 32;
+          nleft = ngroups2;
         }
         if (fork) {
           ev_record(ln.ev_join[0], sa);
@@ -1956,8 +1934,8 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
                                                MsmP256CombineTask{c.win_n, c.nfix, c.id_flags}, Bc, Bp, ctl});
       }
       launch(st, Bc, VFinalTask{c});
-      if (!is_device_ptr(ok)) copy_d2h(st, ok + b0, c.ok, (size_t)Bc);
-      if (!is_device_ptr(status)) copy_d2h(st, status + b0, c.status, (size_t)Bc * 4);
+      oo.copy_back(st, b0, c.ok, Bc);
+      so.copy_back(st, b0, c.status, Bc);
       uint32_t hctl[AGG_CTL_WORDS] = {0, 0, 0, 0};
       if (ctl) copy_d2h(st, hctl, ctl, sizeof(hctl));
       const double t_enq = trace ? ms_now() : 0.0;
@@ -1979,9 +1957,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
     run_lanes(ctx, used, run_lane);
     sync(ctx->cs_in);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 // ------------------------------------------------------------------ stand-alone sub-proof verifiers
@@ -1993,32 +1969,26 @@ int zka_verify_exp_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const ui
                          int32_t* status) {
   if (!ctx || !P || !base || !com || !px || !py || !proofs || !proof_len || !tape || !ok || !status || proof_stride == 0) return ZKA_E_ARG;
   if (B == 0) return 0;
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    DevBuf bufs[8];
-    const uint8_t* d_base = stage_in(st, bufs[0], base, (size_t)B * NP);
-    const uint8_t* d_com = stage_in(st, bufs[1], com, (size_t)B * NP);
-    const uint8_t* d_px = stage_in(st, bufs[2], px, (size_t)B * WP);
-    const uint8_t* d_py = stage_in(st, bufs[3], py, (size_t)B * WP);
-    const uint8_t* d_q = q ? stage_in(st, bufs[4], q, (size_t)B * NP) : nullptr;
-    const uint8_t* d_body = stage_in(st, bufs[5], proofs, (size_t)B * proof_stride);
-    const uint32_t* d_len = stage_in(st, bufs[6], proof_len, (size_t)B);
-    const uint8_t* d_tape = stage_in(st, bufs[7], tape, (size_t)B * tape_stride);
+    DevBuf bufs[10];   // not the lane's staging buffers: verify_impl stages through those
+    Cursor in(bufs);
+    const uint8_t* d_base = stage_in(st, in.next(), base, (size_t)B * NP);
+    const uint8_t* d_com = stage_in(st, in.next(), com, (size_t)B * NP);
+    const uint8_t* d_px = stage_in(st, in.next(), px, (size_t)B * WP);
+    const uint8_t* d_py = stage_in(st, in.next(), py, (size_t)B * WP);
+    const uint8_t* d_q = stage_in(st, in.next(), q, (size_t)B * NP);
+    const uint8_t* d_body = stage_in(st, in.next(), proofs, (size_t)B * proof_stride);
+    const uint32_t* d_len = stage_in(st, in.next(), proof_len, (size_t)B);
+    const uint8_t* d_tape = stage_in(st, in.next(), tape, (size_t)B * tape_stride);
     const size_t row_stride = (HEAD_LEN + proof_stride + 15) & ~(size_t)15;
-    DevBuf rows, rlen;
-    uint8_t* d_rows = rows.get<uint8_t>((size_t)B * row_stride);
-    uint32_t* d_rlen = rlen.get<uint32_t>(B);
+    uint8_t* d_rows = in.take<uint8_t>((size_t)B * row_stride);
+    uint32_t* d_rlen = in.take<uint32_t>(B);
     const int pieces = (int)((row_stride + 63) / 64);
     launch(st, (long long)B * pieces, VAssembleTask{d_base, d_com, d_px, d_py, d_body, proof_stride, d_len, d_rows, row_stride, d_rlen, pieces});
     sync(st);
-    const int rc = verify_impl(ctx, P, B, nullptr, nullptr, 2, d_rows, row_stride, d_rlen, d_tape, tape_stride, ok, status, samples, 1, d_q);
-    for (auto& b : bufs) b.release();
-    rows.release();
-    rlen.release();
-    return rc;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+    return verify_impl(ctx, P, B, nullptr, nullptr, 2, d_rows, row_stride, d_rlen, d_tape, tape_stride, ok, status, samples, 1, d_q);
+  });
 }
 
 // verifyMembership(ProofGroup params, com, ring, proof) (gk.ts:197-262) for B commitments over one ring.
@@ -2031,70 +2001,58 @@ int zka_verify_membership_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, c
   if (N < 2 || N > (1u << 20)) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
   const int n = ceil_log2(N);
   if (tape_stride < (size_t)32 * (2 * n + 1)) return fail(ctx, ZKA_E_ARG, "tape_stride < 32 * (2n + 1)");
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    DevBuf* W = ctx->w;
     DevBuf bufs[4];
-    const uint8_t* d_ring = stage_in(st, ctx->ring_in, ring, (size_t)N * 32);
-    uint32_t* ring_m = ctx->ring_m.get<uint32_t>(((size_t)1 << n) * 8);
-    launch(st, 1ll << n, RingPrepTask{d_ring, ring_m, (int)N});
+    const uint32_t* ring_m = prep_ring(ctx, st, ring, N, n, false);
+    const Output<uint8_t> oo(ok, 1);
+    const Output<int32_t> so(status, 1);
     const size_t row_stride = (HEAD_LEN + proof_stride + 15) & ~(size_t)15;
     const int pieces = (int)((row_stride + 63) / 64);
     const int ngk = 4 * n + 1;
     const uint32_t chunk = 4096;
     for (uint32_t b0 = 0; b0 < B; b0 += chunk) {
       const int Bc = (int)std::min<uint32_t>(chunk, B - b0);
-      const uint8_t* d_com = stage_in(st, bufs[0], com + (size_t)b0 * WP, (size_t)Bc * WP);
-      const uint8_t* d_body = stage_in(st, bufs[1], proofs + (size_t)b0 * proof_stride, (size_t)Bc * proof_stride);
-      const uint32_t* d_len = stage_in(st, bufs[2], proof_len + b0, (size_t)Bc);
-      VerifyCtx c;
-      memset(&c, 0, sizeof(c));
-      c.B = Bc; c.S = (int)P->sec_level; c.N = (int)N; c.n = n; c.K = 1; c.mode = 2;
-      c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
-      c.tape = stage_in(st, bufs[3], tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
+      Cursor in(bufs), w(ctx->w), ob(ctx->out[0]);
+      const uint8_t* d_com = stage_in(st, in.next(), com + (size_t)b0 * WP, (size_t)Bc * WP);
+      const uint8_t* d_body = stage_in(st, in.next(), proofs + (size_t)b0 * proof_stride, (size_t)Bc * proof_stride);
+      const uint32_t* d_len = stage_in(st, in.next(), proof_len + b0, (size_t)Bc);
+      VerifyCtx c = verify_ctx(ctx, P, Bc, (int)P->sec_level, (int)N, n, 1, 2);
+      c.tape = stage_in(st, in.next(), tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
       c.tape_stride = tape_stride;
       c.ring_m = ring_m;
-      c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
-      uint8_t* d_rows = W[0].get<uint8_t>((size_t)Bc * row_stride);
-      uint32_t* d_rlen = W[1].get<uint32_t>(Bc);
+      uint8_t* d_rows = w.take<uint8_t>((size_t)Bc * row_stride);
+      uint32_t* d_rlen = w.take<uint32_t>(Bc);
       c.proofs = d_rows; c.proof_stride = row_stride; c.proof_len = d_rlen;
-      c.gk_off = W[2].get<uint32_t>(Bc);
-      c.gk_ok_len = W[3].get<uint8_t>(Bc);
-      c.gk_scalar = W[4].get<uint32_t>((size_t)Bc * ngk * 8);
-      c.gk_pre = W[5].get<uint32_t>((size_t)Bc * ngk * TOM_PRE_WORDS);
-      uint32_t* gk_offs = W[6].get<uint32_t>((size_t)Bc * ngk);
-      c.fx_jv = W[7].get<uint32_t>((size_t)Bc * 2 * 8);
-      c.fx_jr = W[8].get<uint32_t>((size_t)Bc * 2 * 8);
-      c.fx_proj = W[9].get<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
-      c.win_g = W[10].get<uint32_t>((size_t)Bc * MSM_NWIN * 36);
-      c.id_flags = W[11].get<uint8_t>((size_t)Bc * 3);
-      c.ok = is_device_ptr(ok) ? ok + b0 : ctx->out[0].get<uint8_t>(Bc);
-      c.status = is_device_ptr(status) ? status + b0 : ctx->out[1].get<int32_t>(Bc);
+      c.gk_off = w.take<uint32_t>(Bc);
+      c.gk_ok_len = w.take<uint8_t>(Bc);
+      c.gk_scalar = w.take<uint32_t>((size_t)Bc * ngk * 8);
+      c.gk_pre = w.take<uint32_t>((size_t)Bc * ngk * TOM_PRE_WORDS);
+      uint32_t* gk_offs = w.take<uint32_t>((size_t)Bc * ngk);
+      c.fx_jv = w.take<uint32_t>((size_t)Bc * 2 * 8);
+      c.fx_jr = w.take<uint32_t>((size_t)Bc * 2 * 8);
+      c.fx_proj = w.take<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
+      c.win_g = w.take<uint32_t>((size_t)Bc * MSM_NWIN * 36);
+      c.id_flags = w.take<uint8_t>((size_t)Bc * 3);
+      c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * gk_blocks(n) * 8);
+      c.ok = oo.rows(ob.next(), b0, Bc);
+      c.status = so.rows(ob.next(), b0, Bc);
       launch(st, (long long)Bc * pieces, VAssembleTask{nullptr, nullptr, d_com, nullptr, d_body, proof_stride, d_len, d_rows, row_stride, d_rlen, pieces});
       launch(st, Bc, VGkOnlyLayoutTask{c});
       dev_memset(st, c.fx_jv, 0, (size_t)Bc * 2 * 8 * 4);
       dev_memset(st, c.fx_jr, 0, (size_t)Bc * 2 * 8 * 4);
-      {
-        const int nblk = 1 << (n - gk_block_bits(n));
-        c.gk_part = nblk > 1 ? W[12].get<uint32_t>((size_t)Bc * nblk * 8) : nullptr;
-        if (nblk > 1) launch(st, (long long)Bc * nblk, VGkSumTask{c});
-      }
-      launch(st, Bc, VGkTask{c});
-      launch(st, (long long)Bc * ngk, VGkOffsetsTask{c, gk_offs});
+      verify_gk(st, c, gk_offs);
       launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, row_stride, gk_offs, c.gk_pre, ngk});
       launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin});
       launch(st, (long long)Bc * MSM_NWIN, MsmTomWindowTask{c.gk_scalar, c.gk_pre, nullptr, ngk, 0, 0, ngk, V_SEG, 1, c.win_g});
       launch(st, Bc, MsmTomCombineTask{c.win_g, c.fx_proj, c.id_flags, 2, 0, 0});
       launch(st, Bc, VGkOnlyFinalTask{c});
-      if (!is_device_ptr(ok)) copy_d2h(st, ok + b0, c.ok, (size_t)Bc);
-      if (!is_device_ptr(status)) copy_d2h(st, status + b0, c.status, (size_t)Bc * 4);
+      oo.copy_back(st, b0, c.ok, Bc);
+      so.copy_back(st, b0, c.status, Bc);
       sync(st);
     }
-    for (auto& b : bufs) b.release();
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 
 // verifyEquality / verifyMult / verifyPointAdd alone (kind = 0 / 1 / 2): fixed-size inputs and proofs
@@ -2103,28 +2061,30 @@ static int verify_sub(zka_ctx* ctx, const zka_params* P, int kind, uint32_t B, c
   if (!ctx || !P || !points || !proofs || !tape || !ok || !status) return ZKA_E_ARG;
   if (B == 0) return 0;
   if (tape_stride < (size_t)32 * sub_draws(kind)) return fail(ctx, ZKA_E_ARG, "tape_stride too small for this sub-proof");
-  try {
+  return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    DevBuf* W = ctx->w;
     const int la = sub_points(kind) * WP, lc = sub_proof_len(kind), ne = sub_entries(kind);
     const size_t stride = (size_t)(la + lc + 15) & ~(size_t)15;
+    const Output<uint8_t> oo(ok, 1);
+    const Output<int32_t> so(status, 1);
     const uint32_t chunk = 8192;
     for (uint32_t b0 = 0; b0 < B; b0 += chunk) {
       const int Bc = (int)std::min<uint32_t>(chunk, B - b0);
-      const uint8_t* d_pts = stage_in(st, ctx->in[0], points + (size_t)b0 * la, (size_t)Bc * la);
-      const uint8_t* d_prf = stage_in(st, ctx->in[1], proofs + (size_t)b0 * lc, (size_t)Bc * lc);
-      const uint8_t* d_tape = stage_in(st, ctx->in[2], tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
-      uint8_t* rows = W[0].get<uint8_t>((size_t)Bc * stride);
-      uint32_t* ent_scalar = W[1].get<uint32_t>((size_t)Bc * SUB_ENT_MAX * 8);
-      uint32_t* ent_off = W[2].get<uint32_t>((size_t)Bc * SUB_ENT_MAX);
-      uint32_t* ent_pre = W[3].get<uint32_t>((size_t)Bc * SUB_ENT_MAX * TOM_PRE_WORDS);
-      uint32_t* fx_jv = W[4].get<uint32_t>((size_t)Bc * 2 * 8);
-      uint32_t* fx_jr = W[5].get<uint32_t>((size_t)Bc * 2 * 8);
-      uint32_t* fx_proj = W[6].get<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
-      uint32_t* win = W[7].get<uint32_t>((size_t)Bc * MSM_NWIN * 36);
-      uint8_t* flags = W[8].get<uint8_t>((size_t)Bc * 3);
-      uint8_t* d_ok = is_device_ptr(ok) ? ok + b0 : ctx->out[0].get<uint8_t>(Bc);
-      int32_t* d_st = is_device_ptr(status) ? status + b0 : ctx->out[1].get<int32_t>(Bc);
+      Cursor in(ctx->in[0]), w(ctx->w), ob(ctx->out[0]);
+      const uint8_t* d_pts = stage_in(st, in.next(), points + (size_t)b0 * la, (size_t)Bc * la);
+      const uint8_t* d_prf = stage_in(st, in.next(), proofs + (size_t)b0 * lc, (size_t)Bc * lc);
+      const uint8_t* d_tape = stage_in(st, in.next(), tape + (size_t)b0 * tape_stride, (size_t)Bc * tape_stride);
+      uint8_t* rows = w.take<uint8_t>((size_t)Bc * stride);
+      uint32_t* ent_scalar = w.take<uint32_t>((size_t)Bc * SUB_ENT_MAX * 8);
+      uint32_t* ent_off = w.take<uint32_t>((size_t)Bc * SUB_ENT_MAX);
+      uint32_t* ent_pre = w.take<uint32_t>((size_t)Bc * SUB_ENT_MAX * TOM_PRE_WORDS);
+      uint32_t* fx_jv = w.take<uint32_t>((size_t)Bc * 2 * 8);
+      uint32_t* fx_jr = w.take<uint32_t>((size_t)Bc * 2 * 8);
+      uint32_t* fx_proj = w.take<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
+      uint32_t* win = w.take<uint32_t>((size_t)Bc * MSM_NWIN * 36);
+      uint8_t* flags = w.take<uint8_t>((size_t)Bc * 3);
+      uint8_t* d_ok = oo.rows(ob.next(), b0, Bc);
+      int32_t* d_st = so.rows(ob.next(), b0, Bc);
       launch(st, (long long)Bc * (la + lc), VConcatTask{d_pts, d_prf, la, lc, rows, stride});
       launch(st, Bc, VSubProofTask{kind, rows, stride, d_tape, tape_stride, (const uint8_t*)ctx->tg_bytes.p, ent_scalar, ent_off,
                                    fx_jv, fx_jr, d_st, d_ok});
@@ -2133,14 +2093,12 @@ static int verify_sub(zka_ctx* ctx, const zka_params* P, int kind, uint32_t B, c
       launch(st, (long long)Bc * MSM_NWIN, MsmTomWindowTask{ent_scalar, ent_pre, nullptr, SUB_ENT_MAX, 0, 0, ne, V_SEG, 1, win});
       launch(st, Bc, MsmTomCombineTask{win, fx_proj, flags, 2, 1, 1});
       launch(st, Bc, VSubFinalTask{d_st, flags, d_ok});
-      if (!is_device_ptr(ok)) copy_d2h(st, ok + b0, d_ok, (size_t)Bc);
-      if (!is_device_ptr(status)) copy_d2h(st, status + b0, d_st, (size_t)Bc * 4);
+      oo.copy_back(st, b0, d_ok, Bc);
+      so.copy_back(st, b0, d_st, Bc);
       sync(st);
     }
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 int zka_verify_equality_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* points, const uint8_t* proofs,
                               const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status) {
@@ -2165,7 +2123,7 @@ int pack_common(zka_ctx* ctx, uint32_t B, uint8_t* rows, size_t stride, const ui
   if (!is_device_ptr(rows) || !is_device_ptr(len) || !is_device_ptr(packed) || !is_device_ptr(offsets))
     return fail(ctx, ZKA_E_ARG, "zka_proofs_pack/unpack take device pointers");
 #endif
-  try {
+  return guarded(ctx, [&] {
     Stream tmp;          // borrowed stream (not owned, never destroyed here); launch counters go to lane 0
     Stream* st = &ctx->st;
 #if !defined(ZKA_HOSTSIM)
@@ -2178,9 +2136,7 @@ int pack_common(zka_ctx* ctx, uint32_t B, uint8_t* rows, size_t stride, const ui
     else launch(*st, (long long)B * pieces, PackCopyTask{rows, stride, len, offsets, packed, cap, pieces, dir});
     if (st == &tmp) ctx->st.launches += tmp.launches; else sync(*st);
     return 0;
-  } catch (const std::exception& e) {
-    return fail(ctx, ZKA_E_CUDA, e.what());
-  }
+  });
 }
 }  // namespace
 
