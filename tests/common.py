@@ -65,6 +65,53 @@ def check_p256_mul(L, seed=0, count=6):
         assert out[i].tobytes() == enc(bases[i].mul(p256.new_scalar(v))), i
 
 
+def small_x_point(g, start=1):
+    """(x, y) on the Weierstrass group g with the smallest x >= start, by trial (p = 3 mod 4: y = r^((p+1)/4))."""
+    p = g.p
+    assert p % 4 == 3
+    x = start
+    while True:
+        r = (x * x * x + g.a * x + g.b) % p
+        y = pow(r, (p + 1) // 4, p)
+        if y * y % p == r:
+            return x, y
+        x += 1
+
+
+def noncanonical_enc(g, x, y):
+    """SEC1 encoding of (x, y) with the x coordinate written as x + p: still on the curve mod p.  weier.ts:74-89 has
+    no range check, so the reference accepts it as the point (x, y); edwards.ts:70-86 rejects it."""
+    cs = g.size_field_bytes()
+    return b'\x04' + (x + g.p).to_bytes(cs, 'big') + y.to_bytes(cs, 'big')
+
+
+def noncanonical_tampers(good):
+    """(kind, proof) pairs: a valid proof with one point replaced by a non-canonical encoding of another on-curve
+    point — the P-256 `A` of the first repetition, and the proof-group keyXcom."""
+    g = flat.PROOF_GROUP
+    out = []
+    for kind, grp, off in (('p256 A', p256, flat.HEAD_LEN + 1), ('proof group keyXcom', g, 2 * flat.NP)):
+        x, y = small_x_point(p256) if grp is p256 else grp.gen
+        enc = noncanonical_enc(grp, x, y)
+        p = good.copy()
+        p[off:off + len(enc)] = np.frombuffer(enc, np.uint8)
+        out.append((kind, p))
+    return out
+
+
+def check_noncanonical_p256(L):
+    """A P-256 point given with x + p (p256_mul_batch base, keyToInt) equals the point (x, y), as in the reference."""
+    x, y = small_x_point(p256)
+    enc = noncanonical_enc(p256, x, y)
+    pt = p256.deserialize_point(enc)
+    ks = [1, 2, 0xf0, p256.order - 1]
+    out = L.p256_mul_batch(np.array([list(enc)] * len(ks), np.uint8), be(ks, 32))
+    for i, k in enumerate(ks):
+        assert out[i].tobytes() == pt.mul(p256.new_scalar(k)).to_bytes(), i
+    xs, st = L.key_to_int(np.array([list(enc)], np.uint8))
+    assert st[0] == 0 and int.from_bytes(xs[0].tobytes(), 'big') == OZ.key_to_int(enc) == x
+
+
 def make_params(L, seed=0, sec_level=80):
     rnd = synth.params_rnd(seed)
     hn, hp = L.params_generate(rnd)
@@ -104,10 +151,11 @@ def oracle_proof(po, wl, tape, b):
     return pr, tp
 
 
-def check_prove_parity(L, B=2, N=6, seed=3, sec_level=80):
+def check_prove_parity(L, B=2, N=6, seed=3, sec_level=80, make_tape=synth.random_tape):
+    """make_tape(rows, stride, seed): synth.random_tape, or synth.edge_tape (edge scalars in every draw)."""
     P, po = make_params(L, seed, sec_level)
     wl = synth.Workload(B=B, N=N, seed=seed)
-    tape = synth.random_tape(B, L.prove_tape_len(N, sec_level), seed=seed + 100)
+    tape = make_tape(B, L.prove_tape_len(N, sec_level), seed=seed + 100)
     proofs, plen, status = run_prove(L, P, wl, tape, sec_level)
     assert (status == 0).all(), status
     n = max(1, (N - 1).bit_length())
@@ -154,16 +202,18 @@ def oracle_verdict(po, msg, ring_ints, proof_bytes, vtape_row, N, sec_level=80):
         return 'err'
 
 
-def check_verify_parity(L, N=6, seed=3, tampers=24, sec_level=80):
-    """Valid proofs verify; tampered inputs give the oracle's decision (throw / false / true)."""
+def check_verify_parity(L, N=6, seed=3, tampers=24, sec_level=80, make_tape=synth.random_tape, make_vtape=None):
+    """Valid proofs verify; tampered inputs give the oracle's decision (throw / false / true).  make_vtape(rows,
+    stride, ring_size, sec_level, seed): verify_tape.random_verify_tape (default) or edge_verify_tape."""
     from zkp_ecdsa_b200 import verify_tape as VT
+    make_vtape = make_vtape or VT.random_verify_tape
     P, po = make_params(L, seed, sec_level)
     wl = synth.Workload(B=2, N=N, seed=seed)
-    tape = synth.random_tape(2, L.prove_tape_len(N, sec_level), seed=seed + 100)
+    tape = make_tape(2, L.prove_tape_len(N, sec_level), seed=seed + 100)
     proofs, plen, status = run_prove(L, P, wl, tape, sec_level)
     assert (status == 0).all()
     vts = L.verify_tape_len(N, sec_level)
-    vt = VT.random_verify_tape(2, vts, N, sec_level, seed=seed + 7)
+    vt = make_vtape(2, vts, N, sec_level, seed=seed + 7)
     ok, st = run_verify(L, P, wl.msg_hash, wl.ring, proofs, plen, vt)
     assert list(ok) == [1, 1] and list(st) == [0, 0]
     ring_ints = wl.ring_ints()
@@ -191,8 +241,12 @@ def check_verify_parity(L, N=6, seed=3, tampers=24, sec_level=80):
         else:
             p[int(rng.integers(264, ln - 1200))] ^= 1
         cases.append((p, msg, ring))
+    # non-canonical coordinates: a Weierstrass point parses (the proof is then false), a tomEdwards256 one throws
+    noncanon = noncanonical_tampers(good)
+    for _, p in noncanon:
+        cases.append((p, wl.msg_hash[0].copy(), wl.ring.copy()))
     T = len(cases)
-    vt2 = VT.random_verify_tape(T, vts, N, sec_level, seed=seed + 9)
+    vt2 = make_vtape(T, vts, N, sec_level, seed=seed + 9)
     agree = 0
     for k, (p, msg, ring) in enumerate(cases):
         arr = np.zeros((1, max(len(p), 1)), np.uint8)
@@ -201,19 +255,24 @@ def check_verify_parity(L, N=6, seed=3, tampers=24, sec_level=80):
         got = 'err' if st[0] else bool(ok[0])
         exp = oracle_verdict(po, msg.tobytes(), [int.from_bytes(ring[i].tobytes(), 'big') for i in range(N)],
                              p.tobytes(), vt2[k].tobytes(), N, sec_level)
-        assert got == exp, (k, k % 8, got, int(st[0]), exp)
+        kind = noncanon[k - tampers][0] if k >= tampers else k % 8
+        if k >= tampers and kind != 'p256 A':   # the encoding itself decides: throw on tomEdwards256, parse on war256
+            assert exp == ('err' if flat.PROOF_GROUP is tom else False), (kind, exp)
+        assert got == exp, (k, kind, got, int(st[0]), exp)
         agree += 1
     L.params_destroy(P)
     return agree
 
 
-def check_verify_samples(L, K, N=5, seed=5, sec_level=80, B=2, tampers=4, oracle='python'):
+def check_verify_samples(L, K, N=5, seed=5, sec_level=80, B=2, tampers=4, oracle='python', make_tape=synth.random_tape,
+                         make_vtape=None):
     """zka_verify_batch_ex with `K` sampled repetitions (verifyExp's secparam, exp.ts:233-262) against the oracle's
     verdicts on valid and tampered proofs under identical randomness.  oracle = 'python' or a ZkaLib of oracle/cpu."""
     from zkp_ecdsa_b200 import verify_tape as VT
+    make_vtape = make_vtape or VT.random_verify_tape
     P, po = make_params(L, seed, sec_level)
     wl = synth.Workload(B=B, N=N, seed=seed)
-    tape = synth.random_tape(B, L.prove_tape_len(N, sec_level), seed=seed + 100)
+    tape = make_tape(B, L.prove_tape_len(N, sec_level), seed=seed + 100)
     proofs, plen, status = run_prove(L, P, wl, tape, sec_level)
     assert (status == 0).all()
     vts = L.verify_tape_len_ex(N, sec_level, K)
@@ -229,7 +288,7 @@ def check_verify_samples(L, K, N=5, seed=5, sec_level=80, B=2, tampers=4, oracle
             msg[int(rng.integers(0, 32))] ^= 1
         cases.append((p, msg))
     T = len(cases)
-    vt = VT.random_verify_tape(T, vts, N, sec_level, seed=seed + 9)
+    vt = make_vtape(T, vts, N, sec_level, seed=seed + 9)
     ps = L.proof_max_len(N, sec_level)
     arr = np.zeros((T, ps), np.uint8)
     lens = np.zeros(T, np.uint32)

@@ -30,7 +30,8 @@ def test_whole_proof_bytes_equal_python_oracle(cpu_port):
 
 
 def test_verify_decisions_equal_python_oracle(cpu_port):
-    assert common.check_verify_parity(cpu_port, N=6, seed=3, tampers=16, sec_level=20) == 16
+    # 16 random tampers + the 2 non-canonical point encodings
+    assert common.check_verify_parity(cpu_port, N=6, seed=3, tampers=16, sec_level=20) == 18
 
 
 @pytest.mark.parametrize('tag', ['a', 'b', 'c', 'd'])

@@ -105,6 +105,32 @@ def test_key_to_int(hostsim):
         assert int.from_bytes(x[b].tobytes(), 'big') == OZ.key_to_int(wl.pk[b].tobytes())
 
 
+def check_edge_tapes(L, seed, sec_prove=16, sec_verify=20, cs=(0, 4, 9, 13, 16)):
+    """Every 32-byte draw of the prover and verifier tapes an edge scalar (1, m-1, the top 2^-32 of the range, single
+    bits, windows all 2^(w-1) or 2^(w-1)+1): commitment scalars, blinders, k's, GK draws and the verifier's MSM
+    randomizers go through the table lookups, the per-proof MSMs and the aggregate MSM at every window width `cs`."""
+    from functools import partial
+    edge = lambda sec: partial(synth.edge_tape, sec_level=sec)  # noqa: E731
+    common.check_prove_parity(L, B=2, N=5, seed=seed, sec_level=sec_prove, make_tape=edge(sec_prove))
+    common.check_verify_parity(L, N=5, seed=seed + 1, tampers=6, sec_level=sec_verify, make_tape=edge(sec_verify),
+                               make_vtape=VT.edge_verify_tape)
+    import test_verify_aggregate as tva
+    tva.check_aggregate(L, B=3, N=6, seed=seed + 2, cs=cs, ks=(33,), make_tape=edge(80), make_vtape=VT.edge_verify_tape)
+
+
+def test_edge_tapes(hostsim):
+    check_edge_tapes(hostsim, 201)
+
+
+def test_edge_tapes_war256(hostsim_war):
+    check_edge_tapes(hostsim_war, 211)
+
+
+def test_noncanonical_p256_coordinates(hostsim):
+    """x + p for a point with a small x: p256_mul_batch and keyToInt treat it as (x, y), as the reference does."""
+    common.check_noncanonical_p256(hostsim)
+
+
 def test_multi_chunk_batches_equal_single_chunk():
     """A batch larger than the pipeline chunk is processed in several passes: same bytes."""
     import os

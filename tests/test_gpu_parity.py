@@ -18,6 +18,7 @@ def test_hash80(gpu_engine):
 
 def test_p256_mul(gpu_engine):
     common.check_p256_mul(gpu_engine.lib, count=12)
+    common.check_noncanonical_p256(gpu_engine.lib)
 
 
 def test_params_and_commit(gpu_engine):
@@ -131,6 +132,39 @@ def test_alternate_code_paths_on_gpu():
         common.check_verify_parity(eng.lib, N=2100, sec_level=20, seed=43, tampers=4)
     finally:
         eng.close()
+
+
+def test_edge_tapes_on_gpu(gpu_engine, gpu_engine_war):
+    """Edge scalars in every prover and verifier tape draw (synth.edge_tape, verify_tape.edge_verify_tape) at SecLevel
+    80: proofs against the Python oracle, verdicts against oracle/cpu, the aggregate MSM at its default window and
+    c = 4, 9, 13, 16 — with the default table windows, with 14 / 11-bit windows, and on the war256 build."""
+    import os
+    from functools import partial
+    from zkp_ecdsa_b200 import api, verify_tape as VT
+    import test_verify_aggregate as tva
+    e80 = partial(synth.edge_tape, sec_level=80)
+    os.environ.update(ZKA_TOM_W='14', ZKA_P256_HW='11')
+    try:
+        narrow = api.Engine(device=0)
+    finally:
+        for k in ('ZKA_TOM_W', 'ZKA_P256_HW'):
+            os.environ.pop(k, None)
+    try:
+        for L in (gpu_engine.lib, narrow.lib):
+            common.check_prove_parity(L, B=2, N=6, seed=301, make_tape=e80)
+            common.check_verify_samples(L, 20, N=5, seed=302, tampers=4, oracle=_cpu_port(), make_tape=e80,
+                                        make_vtape=VT.edge_verify_tape)
+            # the chunk of test_edge_cases.test_edge_tapes (3 proofs the reference accepts: some edge prover tapes give a
+            # proof that the reference's own verifier rejects, and then so does this library)
+            tva.check_aggregate(L, B=3, N=6, seed=203, cs=(0, 4, 9, 13, 16), ks=(33,), make_tape=e80,
+                                make_vtape=VT.edge_verify_tape)
+    finally:
+        narrow.close()
+    L = gpu_engine_war.lib
+    common.check_prove_parity(L, B=2, N=6, seed=311, make_tape=e80)
+    common.check_verify_parity(L, N=6, seed=312, tampers=4, make_tape=e80, make_vtape=VT.edge_verify_tape)
+    tva.check_aggregate(L, B=3, N=6, seed=213, cs=(0, 4, 9, 13, 16), ks=(33,), make_tape=e80,
+                        make_vtape=VT.edge_verify_tape)
 
 
 # ---------------------------------------------------------------------------------- round 2

@@ -8,18 +8,20 @@ from zkp_ecdsa_b200 import synth
 from zkp_ecdsa_b200 import verify_tape as VT
 
 
-def _batch(L, B, N, seed, sec_level=80):
+def _batch(L, B, N, seed, sec_level=80, make_tape=synth.random_tape, make_vtape=VT.random_verify_tape):
     P, po = common.make_params(L, seed, sec_level)
     wl = synth.Workload(B=B, N=N, seed=seed)
-    tape = synth.random_tape(B, L.prove_tape_len(N, sec_level), seed=seed + 100)
+    tape = make_tape(B, L.prove_tape_len(N, sec_level), seed=seed + 100)
     proofs, plen, status = common.run_prove(L, P, wl, tape, sec_level)
     assert (status == 0).all()
-    vt = VT.random_verify_tape(B, L.verify_tape_len(N, sec_level), N, sec_level, seed=seed + 7)
+    vt = make_vtape(B, L.verify_tape_len(N, sec_level), N, sec_level, seed=seed + 7)
     return P, wl, proofs, plen, vt
 
 
-def check_aggregate(L, B=5, N=6, seed=31, cs=(0, 4, 7, 11), ks=(33,)):
-    P, wl, proofs, plen, vt = _batch(L, B, N, seed)
+def check_aggregate(L, B=5, N=6, seed=31, cs=(0, 4, 7, 11), ks=(33,), make_tape=synth.random_tape,
+                    make_vtape=VT.random_verify_tape):
+    """make_tape / make_vtape: the prover and verifier tape makers (random, or edge scalars in every draw)."""
+    P, wl, proofs, plen, vt = _batch(L, B, N, seed, make_tape=make_tape, make_vtape=make_vtape)
     try:
         for c in cs:
             if c:
@@ -30,7 +32,7 @@ def check_aggregate(L, B=5, N=6, seed=31, cs=(0, 4, 7, 11), ks=(33,)):
             assert L.stat('agg_pass') > p0 and L.stat('agg_fail') == f0, c      # decided by the aggregate
         # other sample counts (verifyExp's secparam): 33 and all 80 repetitions = 2 / 4 MSM segments per proof
         for K in ks:
-            vtk = VT.random_verify_tape(B, L.verify_tape_len_ex(N, 80, K), N, 80, seed=seed + K)
+            vtk = make_vtape(B, L.verify_tape_len_ex(N, 80, K), N, 80, seed=seed + K)
             okk = np.zeros(B, np.uint8)
             stk = np.zeros(B, np.int32)
             p0, f0 = L.stat('agg_pass'), L.stat('agg_fail')

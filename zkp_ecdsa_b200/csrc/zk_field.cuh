@@ -6,7 +6,7 @@
 //   FpP256  p256.p  (8 limbs, strict  [0,p))   P-256 coordinates AND tomEdwards256 scalars
 //                                              (tom.order == p256.p, src/curves/instances.ts:48)
 //   FnP256  p256.n  (8 limbs, strict  [0,n))   P-256 scalars
-//   FpTom   tom.p   (9 limbs, LAZY    [0,2^12 p)) tomEdwards256 coordinates; 258-bit prime,
+//   FpTom   tom.p   (9 limbs, LAZY    [0,2^13 p)) tomEdwards256 coordinates; 258-bit prime,
 //                                              R = 2^288 leaves 30 bits of headroom so
 //                                              add/sub never reduce and mul needs no final
 //                                              conditional subtraction.
@@ -158,7 +158,7 @@ template <class F>
 struct Field {
   static constexpr int N = F::N;
 
-  // canonical reduce of a lazy value (< 2^12 p) or a strict value (< 2p) into [0,p)
+  // canonical reduce of a lazy value (< 2^14 p) or a strict value (< 2p) into [0,p)
   ZK_HD static void reduce(uint32_t* a) {
     if (F::kLazy) {
       // value < 2^14 p: subtract 2^k p for k = 13..0 when possible (branch-free selects)

@@ -138,13 +138,15 @@ struct VerifyCtx {
 
 // ---- small helpers ------------------------------------------------------------------------
 #if defined(ZKA_PG_WAR256)
-// parse a war256 point encoding (SEC1 uncompressed, weier.ts:74-89: 0x04 tag, coordinates < p, on curve) -> affine
-// Montgomery; returns validity.  (The identity has no 65-byte encoding in a proof slot: tag 0x00 is malformed here.)
+// parse a war256 point encoding (SEC1 uncompressed, weier.ts:74-89: 0x04 tag, on curve) -> affine Montgomery; returns
+// validity.  Like p256_parse, and like the reference (no range check; the curve equation is checked mod p), a
+// coordinate in [p, 2^256) stands for its residue.  (The identity has no 65-byte encoding in a proof slot: tag 0x00 is
+// malformed here.)
 ZK_HD bool tom_parse(uint32_t* xm, uint32_t* ym, const uint8_t* b) {
   uint32_t x[8], y[8];
   limbs_from_be<8>(x, b + 1, 32);
   limbs_from_be<8>(y, b + 33, 32);
-  const bool ok = (b[0] == 0x04) && lt_p<FpWar>(x) && lt_p<FpWar>(y);
+  const bool ok = b[0] == 0x04;
   reduce_once<FpWar>(x);
   reduce_once<FpWar>(y);
   Warp::to_mont(xm, x);

@@ -21,6 +21,10 @@
 // tomEdwards256 has cofactor 4: a chunk in which some proof's points carry a small-order component also goes to the
 // per-proof path (AggTorsionTask), because such components of two proofs could cancel in the sum.
 #pragma once
+#include <string.h>
+
+#include <cmath>
+
 #include "zk_verify.cuh"
 
 namespace zk {
@@ -69,6 +73,45 @@ ZK_HD int agg_digit(const uint32_t* kp, int w, int c) {   // kp[10]
   const int pos = w * c, wi = pos >> 5, sh = pos & 31;
   const uint64_t v = (uint64_t)kp[wi] | ((uint64_t)kp[wi + 1] << 32);
   return (int)((uint32_t)(v >> sh) & ((1u << c) - 1u)) - (1 << (c - 1));
+}
+
+// ---- host: the plan of one aggregate MSM ---------------------------------------------------------------------------
+struct AggPlan {
+  AggDigits D;
+  int levels;
+  int lm[AGG_MAX_LEVELS];   // log2 fan-in of every level of the bucket reduction (sum = c - 1)
+};
+// window bits from a cost model fitted to profiles/agg_window_sweep_r2i.md: ceil(258/c) windows x (entries / warp
+// efficiency + 3 x 2^(c-1) bucket-tree additions); the warp efficiency accounts for the spread of the bucket sizes inside
+// a warp (Poisson: about mean + sigma)
+inline AggPlan agg_plan(double entries, int c_forced) {
+  int best = 4;
+  double best_cost = 1e300;
+  for (int c = 4; c <= 16; c++) {
+    const double nb = (double)(1u << (c - 1)), load = entries / nb;
+    const double eff = load / (load + std::sqrt(load > 1.0 ? load : 1.0));
+    const double cost = std::ceil(258.0 / c) * (entries / (eff > 0.05 ? eff : 0.05) + 3.0 * nb);
+    if (cost < best_cost) { best_cost = cost; best = c; }
+  }
+  const int c = c_forced ? c_forced : best;
+  AggPlan pl;
+  memset(&pl, 0, sizeof(pl));
+  pl.D.c = c;
+  pl.D.nwin = (258 + c - 1) / c;
+  pl.D.nb = 1 << (c - 1);
+  for (int j = 0; j < pl.D.nwin; j++) {   // offs = sum_j 2^(c-1) 2^(c j)
+    const int pos = c * j + c - 1;
+    pl.D.offs[pos >> 5] |= 1u << (pos & 31);
+  }
+  // top window: digits 0 .. top_max, spread over 2^top_shift sub-buckets each
+  const int tb = 256 - c * (pl.D.nwin - 1);
+  const int top_max = 1 << (tb > 0 ? tb : 0);
+  pl.D.top_shift = 0;
+  while (((top_max + 1) << (pl.D.top_shift + 1)) <= pl.D.nb) pl.D.top_shift++;
+  const int bits = c - 1;
+  pl.levels = (bits + AGG_FAN_BITS - 1) / AGG_FAN_BITS;
+  for (int i = 0; i < pl.levels; i++) pl.lm[i] = bits / pl.levels + (i < bits % pl.levels ? 1 : 0);
+  return pl;
 }
 
 // ---- entry sources: slot -> (used?, scalar, point) ---------------------------------------------------------------

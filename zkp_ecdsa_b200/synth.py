@@ -74,6 +74,31 @@ def random_tape(rows: int, stride: int, seed: int) -> np.ndarray:
     return t
 
 
+def edge_scalars(modulus: int) -> list:
+    """Non-zero scalars below `modulus` where digit recoders and carry chains go wrong: 1, m-1, m-2, 2^256 - 2^224 (the
+    low end of the range random draws never reach), single bits, windows all equal to 2^(w-1) or 2^(w-1) + 1 for the
+    table / MSM widths in use (4..22 bits), all-ones runs, alternating bits."""
+    v = {1, 2, modulus - 1, modulus - 2, 0xffffffff << 224, (0xffffffff << 224) + 1, (1 << 255) - 1}
+    v |= {1 << b for b in range(0, 256, 7)} | {(1 << b) - 1 for b in range(8, 256, 31)}
+    for w in (4, 5, 6, 8, 9, 11, 13, 14, 16, 20, 22):
+        for base in (1 << (w - 1), (1 << (w - 1)) + 1):
+            v.add(sum(base << (w * j) for j in range(256 // w + 1)) & ((1 << 256) - 1))
+    v |= {int('55' * 32, 16), int('aa' * 32, 16), int('0f' * 32, 16)}
+    return sorted(x for x in v if 0 < x < modulus)
+
+
+def edge_tape(rows: int, stride: int, seed: int, sec_level: int = 80) -> np.ndarray:
+    """A prover tape (layout of random_tape) whose every 32-byte draw is an edge scalar legal for that draw's modulus
+    (draw_modulus); rows and draws cycle through the catalogue at different offsets."""
+    t = random_tape(rows, stride, seed)
+    cats = {m: edge_scalars(m) for m in (P256_N, P256_P)}
+    for r in range(rows):
+        for k in range(stride // 32):
+            c = cats[draw_modulus(k, sec_level)]
+            t[r, 32 * k:32 * k + 32] = np.frombuffer(c[(k * 5 + r * 11 + seed) % len(c)].to_bytes(32, 'big'), np.uint8)
+    return t
+
+
 class Workload:
     """B signing instances sharing one ring of N key x-coordinates."""
 

@@ -33,6 +33,20 @@ def random_verify_tape(rows: int, stride: int, ring_size: int, sec_level: int = 
     return t
 
 
+def edge_verify_tape(rows: int, stride: int, ring_size: int, sec_level: int = 80, seed: int = 0) -> np.ndarray:
+    """random_verify_tape with every 32-byte draw (GK drains and exp drains) replaced by an edge scalar below p256.n,
+    legal for both moduli (synth.edge_scalars); the index bytes stay as random_verify_tape makes them."""
+    from .synth import P256_N, edge_scalars
+    t = random_verify_tape(rows, stride, ring_size, sec_level, seed)
+    g = 32 * (2 * ceil_log2(ring_size) + 1)
+    cat = edge_scalars(P256_N)
+    offs = [o for o in range(0, g, 32)] + [o for o in range(g + IDX_PAD, stride - 31, 32)]
+    for r in range(rows):
+        for i, o in enumerate(offs):
+            t[r, o:o + 32] = np.frombuffer(cat[(i * 3 + r * 13 + seed) % len(cat)].to_bytes(32, 'big'), np.uint8)
+    return t
+
+
 def oracle_stream(tape_row: bytes, ring_size: int, sec_level: int = 80) -> bytes:
     """The byte stream the reference's rnd() calls would consume for this structured tape:
     GK draws, then one byte per generateIndices draw, then the packed 32-byte exp drains."""
