@@ -468,5 +468,12 @@ template <class F>
 ZK_HD bool lt_p(const uint32_t* a) {
   return !geq_p<F>(a);
 }
+// reduce a raw 256-bit integer mod the field prime (inputs < 2^256 < 2p for all our moduli)
+template <class F>
+ZK_HD void reduce_once(uint32_t* a) {
+  uint32_t t[8];
+  uint32_t br = sub_p<F>(t, a);
+  csel_n<8>(a, br == 0, t, a);
+}
 
 }  // namespace zk

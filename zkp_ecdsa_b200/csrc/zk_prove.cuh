@@ -18,7 +18,7 @@
 //  * all commitments of all repetitions of all proofs of a stage form ONE batch; the
 //    Fiat-Shamir hashes are the only sequencing points.
 #pragma once
-#include "zk_ops.cuh"
+#include "zk_sigma.cuh"
 
 namespace zk {
 
@@ -135,14 +135,6 @@ ZK_HD bool draw_checked(uint32_t* r, const ProveCtx& c, int b, int draw) {
     return false;
   }
   return true;
-}
-
-// reduce a raw 256-bit integer mod the field prime (inputs < 2^256 < 2p for all our moduli)
-template <class F>
-ZK_HD void reduce_once(uint32_t* a) {
-  uint32_t t[8];
-  uint32_t br = sub_p<F>(t, a);
-  csel_n<8>(a, br == 0, t, a);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -706,30 +698,28 @@ struct ItemScalarsTask {
 // Stage 6b — derived commitments by point addition (pointAdd.ts:137-159). One thread per item.
 struct DerivedTask {
   ProveCtx c;
+  struct Store {   // derived point d of item `it`, projective (the address is formed at each store)
+    const ProveCtx& c;
+    int it;
+    ZK_HD void operator()(int d, const TomPt& p) const { tom_st_xyz(c.s2_proj + c.s2_der(it, d) * TOM_PROJ_WORDS, p.x, p.y, p.z); }
+  };
   ZK_HD void ldaff(TomPt& p, const uint32_t* aff, size_t idx) const {
     uint32_t x[PGL], y[PGL];
     ld<PGL>(x, aff + idx * TOM_AFF_WORDS);
     ld<PGL>(y, aff + idx * TOM_AFF_WORDS + PGL);
     tom_from_affine(p, x, y);
   }
-  ZK_HD void stp(size_t idx, const TomPt& p) const {
-    uint32_t* o = c.s2_proj + idx * TOM_PROJ_WORDS;
-    tom_st_xyz(o, p.x, p.y, p.z);
-  }
   ZK_HD void operator()(int it) const {
     const int b = c.item_b[it], i = c.item_i[it];
-    TomPt pkX, pkY, Tx, Ty, T1x, T1y, n, r;
+    TomPt pkX, pkY, Tx, Ty, T1x, T1y;
     ldaff(pkX, c.s1_aff, c.s1_pt(b, 0));
     ldaff(pkY, c.s1_aff, c.s1_pt(b, 1));
     ldaff(Tx, c.s1_aff, c.s1_pt(b, 2 + 2 * i));
     ldaff(Ty, c.s1_aff, c.s1_pt(b, 3 + 2 * i));
     ldaff(T1x, c.s2_aff, c.s2_job(it, JOB_T1X));
     ldaff(T1y, c.s2_aff, c.s2_job(it, JOB_T1Y));
-    tom_neg(n, T1x); tom_add(r, pkX, n); stp(c.s2_der(it, DER_C7), r);    // C7 = C2 - C1
-    tom_neg(n, T1y); tom_add(r, pkY, n); stp(c.s2_der(it, DER_C9), r);    // C9 = C5 - C4
-    tom_neg(n, Tx);  tom_add(r, T1x, n); stp(c.s2_der(it, DER_C12), r);   // C12 = C1 - C3
-    tom_add(r, Tx, T1x); tom_add(r, r, pkX); stp(c.s2_der(it, DER_CINTX), r);
-    tom_add(r, Ty, T1y); stp(c.s2_der(it, DER_CINTY), r);
+    // statement of the repetition's PointAddProof: C1..C6 = T1x pkX Tx T1y pkY Ty (exp.ts:199-210)
+    point_add_derived(Store{c, it}, T1x, pkX, Tx, T1y, pkY, Ty);
   }
 };
 
@@ -745,18 +735,12 @@ struct ItemHashTask {
     ZK_HD const uint8_t* operator()(int k, int& len) const {
       len = WP;
       const ProveCtx& C = *c;
-      if (h < 4) {
-        if (k >= 3) return pt(C.s2_job(it, JOB_MULT0 + 6 * h + (k - 3)));   // C4 Ax Ay Az A4_1 A4_2
-        // Cx, Cy, Cz per MultProof (pointAdd.ts:145-156)
-        if (h == 0) return k == 0 ? pt(C.s2_der(it, DER_C7)) : k == 1 ? pt(C.s2_job(it, JOB_C8)) : C.tg_bytes;
-        if (h == 1) return k == 0 ? pt(C.s2_job(it, JOB_C8)) : k == 1 ? pt(C.s2_der(it, DER_C9)) : pt(C.s2_job(it, JOB_C10));
-        if (h == 2) return k == 2 ? pt(C.s2_job(it, JOB_C11)) : pt(C.s2_job(it, JOB_C10));
-        return k == 0 ? pt(C.s2_job(it, JOB_C10)) : k == 1 ? pt(C.s2_der(it, DER_C12)) : pt(C.s2_job(it, JOB_C13));
+      const int ns = h < PA_MULTS ? 3 : 2;   // the statement (zk_sigma.cuh wiring), then the sub-proof's own points
+      if (k < ns) {
+        const int com = h < PA_MULTS ? pa_mult_com(h, k) : pa_eq_com(h - PA_MULTS, k);
+        return pa_com_bytes(com, pt(C.s2_der(it, 0)), C.tg_bytes, pt(C.s2_job(it, JOB_C8)), BSTRIDE);
       }
-      const int e = h - 4;
-      if (k == 0) return pt(C.s2_job(it, e == 0 ? JOB_C11 : JOB_C13));
-      if (k == 1) return pt(C.s2_der(it, e == 0 ? DER_CINTX : DER_CINTY));
-      return pt(C.s2_job(it, JOB_EQ0 + 2 * e + (k - 2)));
+      return pt(C.s2_job(it, (h < PA_MULTS ? JOB_MULT0 + 6 * h : JOB_EQ0 + 2 * (h - PA_MULTS)) + (k - ns)));
     }
   };
   ZK_HD void operator()(int t) const {

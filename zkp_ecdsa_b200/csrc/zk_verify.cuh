@@ -27,13 +27,13 @@
 //                            bit 1: relA (mod p256.n), relTx, relTy (mod tom.order)            = 3 draws
 //                            bit 0: relA (mod p256.n), then pi8(5) pi10(5) pi11(5) pix(2) pi13(5) piy(2) = 25 draws
 #pragma once
-#include "zk_prove.cuh"   // reduce_once, shared item layout
+#include "zk_prove.cuh"   // shared item layout, the sigma-protocol layer (zk_sigma.cuh)
 
 namespace zk {
 
 enum : int {
   V_SAMPLES = 20,              // default number of sampled repetitions: the literal secparam of zkpAttestList.ts:177
-  V_ENT_PER_SAMPLE = 34,       // variable tomEdwards256 points of one sampled 0-bit repetition
+  V_ENT_PER_SAMPLE = 2 + PA_ENTRIES,   // 34 variable tomEdwards256 points of one sampled 0-bit repetition: Tx, Ty, PointAddProof
   V_SEG = 20,                  // sampled repetitions per MSM segment (one window thread walks <= V_ENT_SEG entries)
   V_ENT_SEG = V_SEG * V_ENT_PER_SAMPLE + 2,       // 682 (+ keyXcom, keyYcom ride with segment 0)
   V_IDX_PAD = 96,
@@ -137,37 +137,6 @@ struct VerifyCtx {
 };
 
 // ---- small helpers ------------------------------------------------------------------------
-#if defined(ZKA_PG_WAR256)
-// parse a war256 point encoding (SEC1 uncompressed, weier.ts:74-89: 0x04 tag, on curve) -> affine Montgomery; returns
-// validity.  Like p256_parse, and like the reference (no range check; the curve equation is checked mod p), a
-// coordinate in [p, 2^256) stands for its residue.  (The identity has no 65-byte encoding in a proof slot: tag 0x00 is
-// malformed here.)
-ZK_HD bool tom_parse(uint32_t* xm, uint32_t* ym, const uint8_t* b) {
-  uint32_t x[8], y[8];
-  limbs_from_be<8>(x, b + 1, 32);
-  limbs_from_be<8>(y, b + 33, 32);
-  const bool ok = b[0] == 0x04;
-  reduce_once<FpWar>(x);
-  reduce_once<FpWar>(y);
-  Warp::to_mont(xm, x);
-  Warp::to_mont(ym, y);
-  return ok && war_on_curve(xm, ym);
-}
-#else
-// parse a tomEdwards256 point encoding -> image-curve affine Montgomery; returns validity
-// (edwards.ts:70-86: 0x04 tag, coordinates < p, on curve)
-ZK_HD bool tom_parse(uint32_t* xm, uint32_t* ym, const uint8_t* b) {
-  uint32_t x[9], y[9], sa[9];
-  limbs_from_be<9>(x, b + 1, 33);
-  limbs_from_be<9>(y, b + 34, 33);
-  bool ok = (b[0] == 0x04) && lt_p<FpTom>(x) && lt_p<FpTom>(y);
-  Tomp::to_mont(xm, x);
-  Tomp::to_mont(ym, y);
-  tom_const(sa, TOM_SQRTA);
-  Tomp::mul(xm, xm, sa);
-  return ok && tom_on_curve(xm, ym);
-}
-#endif
 // P-256 point encoding -> affine Montgomery. identity (65 zero bytes) -> inf.
 ZK_HD bool p256_parse(P256Aff& a, bool& inf, const uint8_t* b) {
   uint32_t x[8], y[8];
@@ -185,14 +154,6 @@ ZK_HD bool p256_parse(P256Aff& a, bool& inf, const uint8_t* b) {
 ZK_HD bool nscalar_parse(uint32_t* r, const uint8_t* b) {   // 32 bytes, mod p256.n
   limbs_from_be<8>(r, b, 32);
   return lt_p<FnP256>(r);
-}
-ZK_HD bool wscalar_parse(uint32_t* r, const uint8_t* b) {   // WS bytes (33 tomEdwards256 / 32 war256), mod the group order
-  limbs_from_be<8>(r, b + (WS - 32), 32);
-  return (WS == 32 || b[0] == 0) && lt_p<FpP256>(r);
-}
-ZK_HD bool vdraw(uint32_t* r, const uint8_t* p, bool nist) {
-  limbs_from_be<8>(r, p, 32);
-  return nist ? lt_p<FnP256>(r) : lt_p<FpP256>(r);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -294,18 +255,6 @@ struct VLayoutTask {
 // ---------------------------------------------------------------------------------------------
 struct VValidateTask {
   VerifyCtx c;
-  ZK_HD bool wpts(const uint8_t* p, int k) const {
-    bool ok = true;
-    uint32_t x[PGL], y[PGL];
-    for (int i = 0; i < k; i++) ok = tom_parse(x, y, p + (size_t)i * WP) && ok;
-    return ok;
-  }
-  ZK_HD bool wscs(const uint8_t* p, int k) const {
-    bool ok = true;
-    uint32_t r[8];
-    for (int i = 0; i < k; i++) ok = wscalar_parse(r, p + (size_t)i * WS) && ok;
-    return ok;
-  }
   // (one thread per (proof, slot, part-of-repetition) was slower — more threads re-reading
   //  the same headers; kept at one thread per (proof, slot))
   ZK_HD void operator()(int t) const {
@@ -319,36 +268,24 @@ struct VValidateTask {
     bool inf;
     if (slot == c.S) {
       ok = p256_parse(a, inf, pr + NP) && ok;             // comS1 (R is checked in VLayoutTask)
-      ok = wpts(pr + 2 * NP, 2) && ok;                    // keyXcom keyYcom
+      ok = valid_points(pr + 2 * NP, 2) && ok;            // keyXcom keyYcom
       if (c.mode != 1) {
         const uint8_t* g = pr + c.gk_off[b];
-        const int n = g[0];
-        ok = wpts(g + 1, 4 * n) && ok;
-        ok = wscs(g + 1 + (size_t)4 * n * WP, 3 * n + 1) && ok;
+        ok = valid_gk(g, g[0]) && ok;
       }
     } else {
       const uint8_t* rep = pr + c.rep_off[(size_t)b * c.S + slot];
       ok = p256_parse(a, inf, rep + 1) && ok;
-      ok = wpts(rep + 1 + NP, 2) && ok;
+      ok = valid_points(rep + 1 + NP, 2) && ok;
       const uint8_t* body = rep + REP_HEAD;
       ok = nscalar_parse(r, body) && ok;
       ok = nscalar_parse(r, body + NS) && ok;
       if (rep[0]) {
-        ok = wscs(body + 2 * NS, 2) && ok;
+        ok = valid_scalars(body + 2 * NS, 2) && ok;
       } else {
         const uint8_t* pa = body + 2 * NS;
-        ok = wpts(pa, 4) && ok;
-        for (int m = 0; m < 4; m++) {
-          const uint8_t* mp = pa + 4 * WP + m * MULT_LEN;
-          ok = wpts(mp, 6) && ok;
-          ok = wscs(mp + 6 * WP, 7) && ok;
-        }
-        for (int e = 0; e < 2; e++) {
-          const uint8_t* ep = pa + 4 * WP + 4 * MULT_LEN + e * EQ_LEN;
-          ok = wpts(ep, 2) && ok;
-          ok = wscs(ep + 2 * WP, 3) && ok;
-        }
-        ok = wscs(pa + PA_LEN, 2) && ok;
+        ok = valid_point_add(pa) && ok;
+        ok = valid_scalars(pa + PA_LEN, 2) && ok;
       }
     }
     if (!ok) ZK_SET_STATUS(c.status + b, ZKA_ERR_MALFORMED);
@@ -442,7 +379,7 @@ struct VSampleJobsTask {
   }
 };
 
-// V6 — C7, C9, C12, Cint, Cint2 (pointAdd.ts:213-215,236,248) by point addition. Per (proof, j).
+// V6 — C7, C9, C12, Cint, Cint2 (pointAdd.ts:213-215,236,248) by point addition (point_add_derived). Per (proof, j).
 struct VDerivedTask {
   VerifyCtx c;
   ZK_HD void frombytes(TomPt& p, const uint8_t* b) const {
@@ -450,16 +387,12 @@ struct VDerivedTask {
     tom_parse(x, y, b);
     tom_from_affine(p, x, y);
   }
-  ZK_HD void stp(size_t idx, const TomPt& p) const {
-    uint32_t* o = c.td_proj + idx * TOM_PROJ_WORDS;
-    tom_st_xyz(o, p.x, p.y, p.z);
-  }
   ZK_HD void operator()(int t) const {
     const int b = t / c.K;
     const int i = c.samp_idx[t];
     const uint8_t* pr = c.proof_of(b);
     const uint8_t* rep = pr + c.rep_off[(size_t)b * c.S + i];
-    TomPt pkX, pkY, Tx, Ty, T1x, T1y, n, r;
+    TomPt pkX, pkY, Tx, Ty, T1x, T1y;
     frombytes(pkX, pr + 2 * NP);
     frombytes(pkY, pr + 2 * NP + WP);
     frombytes(Tx, rep + 1 + NP);
@@ -469,15 +402,11 @@ struct VDerivedTask {
     tom_from_affine(T1x, x, y);
     ld<PGL>(x, c.ta_aff + c.ta_pt(t, 1) * TOM_AFF_WORDS); ld<PGL>(y, c.ta_aff + c.ta_pt(t, 1) * TOM_AFF_WORDS + PGL);
     tom_from_affine(T1y, x, y);
-    tom_neg(n, T1x); tom_add(r, pkX, n); stp(c.td_pt(t, DER_C7), r);
-    tom_neg(n, T1y); tom_add(r, pkY, n); stp(c.td_pt(t, DER_C9), r);
-    tom_neg(n, Tx);  tom_add(r, T1x, n); stp(c.td_pt(t, DER_C12), r);
-    tom_add(r, Tx, T1x); tom_add(r, r, pkX); stp(c.td_pt(t, DER_CINTX), r);
-    tom_add(r, T1y, Ty); stp(c.td_pt(t, DER_CINTY), r);
+    point_add_derived(DerivedProj{c.td_proj, c.td_pt(t, 0)}, T1x, pkX, Tx, T1y, pkY, Ty);   // exp.ts:331-341
   }
 };
 
-// V7 — the six challenges of a sampled 0-bit repetition (mult.ts:156, equality.ts:101).
+// V7 — the six challenges of a sampled 0-bit repetition (mult.ts:156, equality.ts:101), h in HASHES_PER_ITEM order.
 // One thread per (proof, j, h).
 struct VItemHashTask {
   VerifyCtx c;
@@ -487,46 +416,18 @@ struct VItemHashTask {
     const int i = c.samp_idx[sample];
     const uint8_t* rep = c.proof_of(b) + c.rep_off[(size_t)b * c.S + i];
     uint32_t c3[3] = {0, 0, 0};
-    if (!rep[0]) {
-      const uint8_t* pa = rep + REP_HEAD + 2 * NS;
-      const uint8_t* C8 = pa, *C10 = pa + WP, *C11 = pa + 2 * WP, *C13 = pa + 3 * WP;
-      const uint8_t* der = c.td_bytes + c.td_pt(sample, 0) * BSTRIDE;
-      Sha256 s;
-      s.init();
-      if (h < 4) {
-        const uint8_t *cx, *cy, *cz;
-        if (h == 0)      { cx = der + DER_C7 * BSTRIDE; cy = C8; cz = c.tg_bytes; }
-        else if (h == 1) { cx = C8; cy = der + DER_C9 * BSTRIDE; cz = C10; }
-        else if (h == 2) { cx = C10; cy = C10; cz = C11; }
-        else             { cx = C10; cy = der + DER_C12 * BSTRIDE; cz = C13; }
-        s.update(cx, WP); s.update(cy, WP); s.update(cz, WP);
-        s.update(pa + 4 * WP + h * MULT_LEN, 6 * WP);     // C4 Ax Ay Az A4_1 A4_2 are contiguous
-      } else {
-        const int e = h - 4;
-        s.update(e == 0 ? C11 : C13, WP);
-        s.update(der + (e == 0 ? DER_CINTX : DER_CINTY) * BSTRIDE, WP);
-        s.update(pa + 4 * WP + 4 * MULT_LEN + e * EQ_LEN, 2 * WP);
-      }
-      s.final80(c3);
-    }
+    if (!rep[0]) pa_challenge(c3, h, c.td_bytes + c.td_pt(sample, 0) * BSTRIDE, c.tg_bytes, rep + REP_HEAD + 2 * NS);
     st<3>(c.item_chal + (size_t)t * 3, c3);
   }
 };
 
 // ---------------------------------------------------------------------------------------------
 // V8 — relations of one sampled repetition folded into (variable-point scalars, fixed-base
-// partial sums).  All arithmetic mod q = tom.order in Montgomery form.  Per (proof, j).
+// partial sums); a 0-bit repetition's PointAddProof through fold_point_add (zk_sigma.cuh).
+// All arithmetic mod q = tom.order in Montgomery form.  Per (proof, j).
 // ---------------------------------------------------------------------------------------------
 struct VRelationsTask {
   VerifyCtx c;
-  // entry e of sample j of proof b
-  ZK_HD void ent(int b, int j, int e, const uint32_t* s_mont, uint32_t off) const {
-    uint32_t v[8];
-    Tomq::from_mont(v, s_mont);
-    const size_t idx = (size_t)b * c.ent_tom() + (size_t)j * V_ENT_PER_SAMPLE + e;
-    st<8>(c.ent_scalar + idx * 8, v);
-    c.ent_off[idx] = off;
-  }
   ZK_HD void operator()(int t) const {
     using F = Tomq;
     using Fn = P256n;
@@ -538,12 +439,15 @@ struct VRelationsTask {
     const uint8_t* body = rep + REP_HEAD;
     const uint8_t* dr = c.exp_tape(b) + (size_t)32 * c.samp_draw[t];
     uint32_t* part = c.part + (size_t)t * V_PART_WORDS;
-    uint32_t gW[8], hW[8], pX[8], pY[8], sR[8], sH[8], sC[8];
-    zero_n<8>(gW); zero_n<8>(hW); zero_n<8>(pX); zero_n<8>(pY); zero_n<8>(sR); zero_n<8>(sH); zero_n<8>(sC);
-    bool tape_ok = true;
+    const Entries out{c.ent_scalar, c.ent_off};
+    const size_t e0 = (size_t)b * c.ent_tom() + (size_t)j * V_ENT_PER_SAMPLE;   // Tx, Ty, then the PointAddProof's points
+    SigmaFold f;
+    uint32_t pX[8], pY[8], sR[8], sH[8], sC[8];
+    zero_n<8>(f.gW); zero_n<8>(f.hW); zero_n<8>(pX); zero_n<8>(pY); zero_n<8>(sR); zero_n<8>(sH); zero_n<8>(sC);
+    f.tape_ok = true;
     // --- multiN: relA (exp.ts:273-279 / 306-316)
     uint32_t rho[8], rm[8], s[8], sm[8], t0[8], t1[8];
-    tape_ok = vdraw(rho, dr, true) && tape_ok;
+    f.tape_ok = vdraw(rho, dr, true) && f.tape_ok;
     Fn::to_mont(rm, rho);
     nscalar_parse(s, body);            // alpha | z
     Fn::to_mont(sm, s);
@@ -560,142 +464,49 @@ struct VRelationsTask {
     }
     // coordinates of T / T1 as proof-group scalars
     uint32_t sx[8], sy[8];
-    ld<8>(sx, c.sp_T_aff + (size_t)t * 16);
-    ld<8>(sy, c.sp_T_aff + (size_t)t * 16 + 8);
     const uint32_t offTx = roff + 1 + NP, offTy = offTx + WP;
     if (rep[0]) {
       // relTx, relTy (exp.ts:284-298): sx g + beta2 h - Tx ; sy g + beta3 h - Ty
       uint32_t b2[8], b3[8], neg[8], z[8];
+      ld<8>(sx, c.sp_T_aff + (size_t)t * 16);
+      ld<8>(sy, c.sp_T_aff + (size_t)t * 16 + 8);
       zero_n<8>(z);
       wscalar_parse(b2, body + 2 * NS);
       wscalar_parse(b3, body + 2 * NS + WS);
-      tape_ok = vdraw(rho, dr + 32, false) && tape_ok;
+      f.tape_ok = vdraw(rho, dr + 32, false) && f.tape_ok;
       F::to_mont(rm, rho);
-      F::mul(t0, rm, sx); F::add(gW, gW, t0);
-      F::to_mont(t1, b2); F::mul(t0, rm, t1); F::add(hW, hW, t0);
-      F::sub(neg, z, rm); ent(b, j, 0, neg, offTx);
-      tape_ok = vdraw(rho, dr + 64, false) && tape_ok;
+      F::mul(t0, rm, sx); F::add(f.gW, f.gW, t0);
+      F::to_mont(t1, b2); F::mul(t0, rm, t1); F::add(f.hW, f.hW, t0);
+      F::sub(neg, z, rm); out.put_m(e0 + 0, neg, offTx);
+      f.tape_ok = vdraw(rho, dr + 64, false) && f.tape_ok;
       F::to_mont(rm, rho);
-      F::mul(t0, rm, sy); F::add(gW, gW, t0);
-      F::to_mont(t1, b3); F::mul(t0, rm, t1); F::add(hW, hW, t0);
-      F::sub(neg, z, rm); ent(b, j, 1, neg, offTy);
+      F::mul(t0, rm, sy); F::add(f.gW, f.gW, t0);
+      F::to_mont(t1, b3); F::mul(t0, rm, t1); F::add(f.hW, f.hW, t0);
+      F::sub(neg, z, rm); out.put_m(e0 + 1, neg, offTy);
       c.ent_cnt[t] = 2;
     } else {
+      // aggregatePointAdd(T1x, T1y, pkX, pkY, Tx, Ty) (exp.ts:331-341): C1..C6 = T1x pkX Tx T1y pkY Ty
       const uint8_t* pa = body + 2 * NS;
-      const uint32_t offPa = roff + REP_HEAD + 2 * NS;
-      uint32_t r1[8], r2[8], r1m[8], r2m[8];
-      wscalar_parse(r1, pa + PA_LEN);
-      wscalar_parse(r2, pa + PA_LEN + WS);
-      F::to_mont(r1m, r1);
-      F::to_mont(r2m, r2);
-      // accumulated coefficients of the primitive points
-      uint32_t cTx[8], cTy[8], cC8[8], cC10[8], cC11[8], cC13[8];
-      zero_n<8>(cTx); zero_n<8>(cTy); zero_n<8>(cC8); zero_n<8>(cC10); zero_n<8>(cC11); zero_n<8>(cC13);
-      // helper lambdas are avoided (host/device portability): explicit code per target kind
-      // kind: 0 C7, 1 C8, 2 g(C14), 3 C9, 4 C10, 5 C11, 6 C12, 7 C13, 8 CintX, 9 CintY
-#define ZK_ADD_TERM(kind, coef)                                                              \
-  do {                                                                                       \
-    const int _k = (kind);                                                                   \
-    if (_k == 1) F::add(cC8, cC8, coef);                                                     \
-    else if (_k == 4) F::add(cC10, cC10, coef);                                              \
-    else if (_k == 5) F::add(cC11, cC11, coef);                                              \
-    else if (_k == 7) F::add(cC13, cC13, coef);                                              \
-    else if (_k == 2) F::add(gW, gW, coef);                                                  \
-    else if (_k == 0) { /* C7 = pkX - T1x */                                                 \
-      F::add(pX, pX, coef); F::mul(t0, coef, sx); F::sub(gW, gW, t0); F::mul(t0, coef, r1m); F::sub(hW, hW, t0); \
-    } else if (_k == 3) { /* C9 = pkY - T1y */                                               \
-      F::add(pY, pY, coef); F::mul(t0, coef, sy); F::sub(gW, gW, t0); F::mul(t0, coef, r2m); F::sub(hW, hW, t0); \
-    } else if (_k == 6) { /* C12 = T1x - Tx */                                               \
-      F::mul(t0, coef, sx); F::add(gW, gW, t0); F::mul(t0, coef, r1m); F::add(hW, hW, t0); F::sub(cTx, cTx, coef); \
-    } else if (_k == 8) { /* Cint = Tx + T1x + pkX */                                        \
-      F::add(cTx, cTx, coef); F::add(pX, pX, coef); F::mul(t0, coef, sx); F::add(gW, gW, t0); F::mul(t0, coef, r1m); F::add(hW, hW, t0); \
-    } else { /* Cint2 = T1y + Ty */                                                          \
-      F::add(cTy, cTy, coef); F::mul(t0, coef, sy); F::add(gW, gW, t0); F::mul(t0, coef, r2m); F::add(hW, hW, t0); \
-    }                                                                                        \
-  } while (0)
-      int d = 1;   // draw index inside the sample (0 was relA)
-      // order of aggregation: pi8, pi10, pi11, pix, pi13, piy (pointAdd.ts:221-253)
-      for (int step = 0; step < 6; step++) {
-        const bool is_eq = (step == 3 || step == 5);
-        uint32_t cc[8], cm[8], c3[3];
-        if (!is_eq) {
-          const int m = step < 3 ? step : 3;
-          const int kx = m == 0 ? 0 : (m == 1 ? 1 : 4);      // Cx: C7, C8, C10, C10
-          const int ky = m == 0 ? 1 : (m == 1 ? 3 : (m == 2 ? 4 : 6));   // Cy: C8, C9, C10, C12
-          const int kz = m == 0 ? 2 : (m == 1 ? 4 : (m == 2 ? 5 : 7));   // Cz: g, C10, C11, C13
-          ld<3>(c3, c.item_chal + ((size_t)t * HASHES_PER_ITEM + m) * 3);
-          challenge_to_limbs(cc, c3);
-          F::to_mont(cm, cc);
-          const uint8_t* mp = pa + 4 * WP + m * MULT_LEN;
-          const uint32_t offM = offPa + 4 * WP + m * MULT_LEN;
-          uint32_t ts[7][8];
-          for (int q = 0; q < 7; q++) { wscalar_parse(ts[q], mp + 6 * WP + q * WS); F::to_mont(ts[q], ts[q]); }
-          // ts: t_x t_y t_z t_rx t_ry t_rz t_r4
-          uint32_t rr[5][8];
-          for (int q = 0; q < 5; q++) { tape_ok = vdraw(rho, dr + 32 * (d + q), false) && tape_ok; F::to_mont(rr[q], rho); }
-          d += 5;
-          uint32_t coef[8], neg[8], z[8];
-          zero_n<8>(z);
-          // rho1: t_x g + t_rx h + c Cx - A_x
-          F::mul(t0, rr[0], ts[0]); F::add(gW, gW, t0);
-          F::mul(t0, rr[0], ts[3]); F::add(hW, hW, t0);
-          F::mul(coef, rr[0], cm); ZK_ADD_TERM(kx, coef);
-          F::sub(neg, z, rr[0]); ent(b, j, 6 + 6 * m + 1, neg, offM + WP);
-          // rho2: t_y g + t_ry h + c Cy - A_y
-          F::mul(t0, rr[1], ts[1]); F::add(gW, gW, t0);
-          F::mul(t0, rr[1], ts[4]); F::add(hW, hW, t0);
-          F::mul(coef, rr[1], cm);
-          // rho5: t_x Cy + c C_4 - A_4_2   (Cy coefficient joins rho2's)
-          F::mul(t0, rr[4], ts[0]); F::add(coef, coef, t0);
-          ZK_ADD_TERM(ky, coef);
-          F::sub(neg, z, rr[1]); ent(b, j, 6 + 6 * m + 2, neg, offM + 2 * WP);
-          // rho3: t_z g + t_rz h + c Cz - A_z
-          F::mul(t0, rr[2], ts[2]); F::add(gW, gW, t0);
-          F::mul(t0, rr[2], ts[5]); F::add(hW, hW, t0);
-          F::mul(coef, rr[2], cm); ZK_ADD_TERM(kz, coef);
-          F::sub(neg, z, rr[2]); ent(b, j, 6 + 6 * m + 3, neg, offM + 3 * WP);
-          // rho4: t_z g + t_r4 h + c C_4 - A_4_1
-          F::mul(t0, rr[3], ts[2]); F::add(gW, gW, t0);
-          F::mul(t0, rr[3], ts[6]); F::add(hW, hW, t0);
-          F::add(coef, rr[3], rr[4]); F::mul(coef, coef, cm);     // C_4: (rho4 + rho5) c
-          ent(b, j, 6 + 6 * m + 0, coef, offM);
-          F::sub(neg, z, rr[3]); ent(b, j, 6 + 6 * m + 4, neg, offM + 4 * WP);
-          F::sub(neg, z, rr[4]); ent(b, j, 6 + 6 * m + 5, neg, offM + 5 * WP);
-        } else {
-          const int e = step == 3 ? 0 : 1;
-          ld<3>(c3, c.item_chal + ((size_t)t * HASHES_PER_ITEM + 4 + e) * 3);
-          challenge_to_limbs(cc, c3);
-          F::to_mont(cm, cc);
-          const uint8_t* ep = pa + 4 * WP + 4 * MULT_LEN + e * EQ_LEN;
-          const uint32_t offE = offPa + 4 * WP + 4 * MULT_LEN + e * EQ_LEN;
-          uint32_t tx[8], tr1[8], tr2[8], ra[8], rb[8], coef[8], neg[8], z[8];
-          zero_n<8>(z);
-          wscalar_parse(tx, ep + 2 * WP); F::to_mont(tx, tx);
-          wscalar_parse(tr1, ep + 2 * WP + WS); F::to_mont(tr1, tr1);
-          wscalar_parse(tr2, ep + 2 * WP + 2 * WS); F::to_mont(tr2, tr2);
-          tape_ok = vdraw(rho, dr + 32 * d, false) && tape_ok; F::to_mont(ra, rho);
-          tape_ok = vdraw(rho, dr + 32 * (d + 1), false) && tape_ok; F::to_mont(rb, rho);
-          d += 2;
-          F::add(t1, ra, rb); F::mul(t0, t1, tx); F::add(gW, gW, t0);
-          F::mul(t0, ra, tr1); F::add(hW, hW, t0);
-          F::mul(t0, rb, tr2); F::add(hW, hW, t0);
-          F::mul(coef, ra, cm); ZK_ADD_TERM(e == 0 ? 5 : 7, coef);     // C1 = C11 | C13
-          F::mul(coef, rb, cm); ZK_ADD_TERM(e == 0 ? 8 : 9, coef);     // C2 = Cint | Cint2
-          F::sub(neg, z, ra); ent(b, j, 30 + 2 * e, neg, offE);
-          F::sub(neg, z, rb); ent(b, j, 30 + 2 * e + 1, neg, offE + WP);
-        }
-      }
-#undef ZK_ADD_TERM
-      ent(b, j, 0, cTx, offTx);
-      ent(b, j, 1, cTy, offTy);
-      ent(b, j, 2, cC8, offPa);
-      ent(b, j, 3, cC10, offPa + WP);
-      ent(b, j, 4, cC11, offPa + 2 * WP);
-      ent(b, j, 5, cC13, offPa + 3 * WP);
+      uint32_t a[PA_NCOM][8], in[6][8], r1[8], r2[8];
+      fold_point_add(f, a, c.item_chal + (size_t)t * HASHES_PER_ITEM * 3, pa, dr + 32, out, e0 + 2, roff + REP_HEAD + 2 * NS);
+      point_add_expand(in, a);
+      // C1 = T1x = sx g + r1 h, C4 = T1y = sy g + r2 h (exp.ts:326-329) are folded onto g and h
+      ld<8>(sx, c.sp_T_aff + (size_t)t * 16);
+      ld<8>(sy, c.sp_T_aff + (size_t)t * 16 + 8);
+      wscalar_parse(r1, pa + PA_LEN); F::to_mont(r1, r1);
+      wscalar_parse(r2, pa + PA_LEN + WS); F::to_mont(r2, r2);
+      F::mul(t0, in[0], sx); F::add(f.gW, f.gW, t0);
+      F::mul(t0, in[0], r1); F::add(f.hW, f.hW, t0);
+      F::mul(t0, in[3], sy); F::add(f.gW, f.gW, t0);
+      F::mul(t0, in[3], r2); F::add(f.hW, f.hW, t0);
+      copy_n<8>(pX, in[1]);
+      copy_n<8>(pY, in[4]);
+      out.put_m(e0 + 0, in[2], offTx);
+      out.put_m(e0 + 1, in[5], offTy);
       c.ent_cnt[t] = V_ENT_PER_SAMPLE;
     }
-    if (!tape_ok) ZK_SET_STATUS(c.status + b, ZKA_ERR_TAPE_RANGE);
-    st<8>(part, gW); st<8>(part + 8, hW); st<8>(part + 16, pX); st<8>(part + 24, pY);
+    if (!f.tape_ok) ZK_SET_STATUS(c.status + b, ZKA_ERR_TAPE_RANGE);
+    st<8>(part, f.gW); st<8>(part + 8, f.hW); st<8>(part + 16, pX); st<8>(part + 24, pY);
     st<8>(part + 32, sR); st<8>(part + 40, sH); st<8>(part + 48, sC);
     // multiN variable point A_i
     P256Aff A;
@@ -1273,11 +1084,8 @@ struct VGkOnlyLayoutTask {
     c.gk_off[b] = bad ? 0 : HEAD_LEN;
     bool okp = true;
     if (!bad) {
-      uint32_t x[PGL], y[PGL], r[8];
-      okp = tom_parse(x, y, pr + 2 * NP);
-      const uint8_t* g = pr + HEAD_LEN;
-      for (int i = 0; i < 4 * ngk; i++) okp = tom_parse(x, y, g + 1 + (size_t)i * WP) && okp;
-      for (int i = 0; i < 3 * ngk + 1; i++) okp = wscalar_parse(r, g + 1 + (size_t)4 * ngk * WP + (size_t)i * WS) && okp;
+      okp = valid_points(pr + 2 * NP, 1);
+      okp = valid_gk(pr + HEAD_LEN, ngk) && okp;
     }
     if (bad || !okp) ZK_SET_STATUS(c.status + b, ZKA_ERR_MALFORMED);
     c.gk_ok_len[b] = (!bad && okp && ngk == c.n) ? 1 : 0;
@@ -1296,9 +1104,9 @@ struct VGkOnlyFinalTask {
 // (233 / 633 / 3266 bytes).  One thread per statement folds all relations under the tape's randomizers into
 //   * scalars of the variable points (inputs and proof points)  -> entries of ONE Pippenger instance,
 //   * the coefficients of g and h                                -> one fixed-base commitment,
-// exactly like the batched verifier does for a sampled repetition; derived commitments (C7, C9, C12, Cint) are
-// expanded onto the inputs they are sums of.
-enum : int { SUB_EQ = 0, SUB_MULT = 1, SUB_PADD = 2, SUB_ENT_MAX = 38 };
+// with the same folds as the batched verifier's sampled repetitions (zk_sigma.cuh); the derived commitments (C7, C9,
+// C12, Cint, Cint2) are expanded onto the inputs they are sums of.
+enum : int { SUB_EQ = 0, SUB_MULT = 1, SUB_PADD = 2, SUB_ENT_MAX = 6 + PA_ENTRIES };   // 38: PX..RY, PointAddProof
 ZK_LAYOUT_FN int sub_points(int kind) { return kind == SUB_EQ ? 2 : kind == SUB_MULT ? 3 : 6; }
 ZK_LAYOUT_FN int sub_proof_len(int kind) { return kind == SUB_EQ ? EQ_LEN : kind == SUB_MULT ? MULT_LEN : PA_LEN; }
 ZK_LAYOUT_FN int sub_draws(int kind) { return kind == SUB_EQ ? 2 : kind == SUB_MULT ? 5 : 24; }
@@ -1342,86 +1150,10 @@ struct VSubProofTask {
   int32_t* status;         // [B]
   uint8_t* ok;             // [B]
 
-  struct Fold {            // running state of one statement
-    uint32_t gW[8], hW[8];
-    bool tape_ok;
+  struct DerivedBytes {    // encodings of the derived points, BSTRIDE apart in DER_* order
+    uint8_t* out;
+    ZK_HD void operator()(int d, const TomPt& p) const { tom_encode_proj(out + (size_t)d * BSTRIDE, p); }
   };
-  ZK_HD static void acc_add(uint32_t* a, const uint32_t* v) { Tomq::add(a, a, v); }
-  // aggregateMult (mult.ts:148-175).  bx/by/bz: 67-byte encodings; mp: MultProof bytes; dr: 5 drains.
-  // cx/cy/cz: Montgomery coefficient accumulators of Cx, Cy, Cz; es: canonical scalars of C4 Ax Ay Az A41 A42.
-  ZK_HD static void mult(Fold& f, const uint8_t* bx, const uint8_t* by, const uint8_t* bz, const uint8_t* mp, const uint8_t* dr,
-                         uint32_t* cx, uint32_t* cy, uint32_t* cz, uint32_t (*es)[8]) {
-    using F = Tomq;
-    Sha256 h;
-    h.init();
-    h.update(bx, WP); h.update(by, WP); h.update(bz, WP); h.update(mp, 6 * WP);
-    uint32_t c3[3], cc[8], cm[8];
-    h.final80(c3);
-    challenge_to_limbs(cc, c3);
-    F::to_mont(cm, cc);
-    uint32_t ts[7][8], rr[5][8], rho[8], t0[8], coef[8], neg[8], z[8];
-    zero_n<8>(z);
-    for (int q = 0; q < 7; q++) { wscalar_parse(ts[q], mp + 6 * WP + q * WS); F::to_mont(ts[q], ts[q]); }
-    for (int q = 0; q < 5; q++) { f.tape_ok = vdraw(rho, dr + 32 * q, false) && f.tape_ok; F::to_mont(rr[q], rho); }
-    // rho1: t_x g + t_rx h + c Cx - A_x
-    F::mul(t0, rr[0], ts[0]); acc_add(f.gW, t0);
-    F::mul(t0, rr[0], ts[3]); acc_add(f.hW, t0);
-    F::mul(coef, rr[0], cm); acc_add(cx, coef);
-    F::sub(neg, z, rr[0]); F::from_mont(es[1], neg);
-    // rho2: t_y g + t_ry h + c Cy - A_y ; rho5: t_x Cy + c C_4 - A_4_2
-    F::mul(t0, rr[1], ts[1]); acc_add(f.gW, t0);
-    F::mul(t0, rr[1], ts[4]); acc_add(f.hW, t0);
-    F::mul(coef, rr[1], cm);
-    F::mul(t0, rr[4], ts[0]); F::add(coef, coef, t0);
-    acc_add(cy, coef);
-    F::sub(neg, z, rr[1]); F::from_mont(es[2], neg);
-    // rho3: t_z g + t_rz h + c Cz - A_z
-    F::mul(t0, rr[2], ts[2]); acc_add(f.gW, t0);
-    F::mul(t0, rr[2], ts[5]); acc_add(f.hW, t0);
-    F::mul(coef, rr[2], cm); acc_add(cz, coef);
-    F::sub(neg, z, rr[2]); F::from_mont(es[3], neg);
-    // rho4: t_z g + t_r4 h + c C_4 - A_4_1
-    F::mul(t0, rr[3], ts[2]); acc_add(f.gW, t0);
-    F::mul(t0, rr[3], ts[6]); acc_add(f.hW, t0);
-    F::add(coef, rr[3], rr[4]); F::mul(coef, coef, cm); F::from_mont(es[0], coef);   // C_4: (rho4 + rho5) c
-    F::sub(neg, z, rr[3]); F::from_mont(es[4], neg);
-    F::sub(neg, z, rr[4]); F::from_mont(es[5], neg);
-  }
-  // aggregateEquality (equality.ts:94-116): es = canonical scalars of A1, A2
-  ZK_HD static void equality(Fold& f, const uint8_t* b1, const uint8_t* b2, const uint8_t* ep, const uint8_t* dr, uint32_t* c1,
-                             uint32_t* c2, uint32_t (*es)[8]) {
-    using F = Tomq;
-    Sha256 h;
-    h.init();
-    h.update(b1, WP); h.update(b2, WP); h.update(ep, 2 * WP);
-    uint32_t c3[3], cc[8], cm[8];
-    h.final80(c3);
-    challenge_to_limbs(cc, c3);
-    F::to_mont(cm, cc);
-    uint32_t tx[8], tr1[8], tr2[8], ra[8], rb[8], rho[8], t0[8], t1[8], coef[8], neg[8], z[8];
-    zero_n<8>(z);
-    wscalar_parse(tx, ep + 2 * WP); F::to_mont(tx, tx);
-    wscalar_parse(tr1, ep + 2 * WP + WS); F::to_mont(tr1, tr1);
-    wscalar_parse(tr2, ep + 2 * WP + 2 * WS); F::to_mont(tr2, tr2);
-    f.tape_ok = vdraw(rho, dr, false) && f.tape_ok; F::to_mont(ra, rho);
-    f.tape_ok = vdraw(rho, dr + 32, false) && f.tape_ok; F::to_mont(rb, rho);
-    F::add(t1, ra, rb); F::mul(t0, t1, tx); acc_add(f.gW, t0);
-    F::mul(t0, ra, tr1); acc_add(f.hW, t0);
-    F::mul(t0, rb, tr2); acc_add(f.hW, t0);
-    F::mul(coef, ra, cm); acc_add(c1, coef);
-    F::mul(coef, rb, cm); acc_add(c2, coef);
-    F::sub(neg, z, ra); F::from_mont(es[0], neg);
-    F::sub(neg, z, rb); F::from_mont(es[1], neg);
-  }
-  ZK_HD void emit(int b, int e, const uint32_t* canon, uint32_t off) const {
-    st<8>(ent_scalar + ((size_t)b * SUB_ENT_MAX + e) * 8, canon);
-    ent_off[(size_t)b * SUB_ENT_MAX + e] = off;
-  }
-  ZK_HD void emit_m(int b, int e, const uint32_t* mont, uint32_t off) const {
-    uint32_t v[8];
-    Tomq::from_mont(v, mont);
-    emit(b, e, v, off);
-  }
   ZK_HD void operator()(int b) const {
     using F = Tomq;
     const uint8_t* row = rows + (size_t)b * stride;
@@ -1429,101 +1161,51 @@ struct VSubProofTask {
     const int np = sub_points(kind);
     const uint8_t* proof = row + (size_t)np * WP;
     const uint32_t poff = (uint32_t)(np * WP);
+    const Entries out{ent_scalar, ent_off};
+    const size_t e0 = (size_t)b * SUB_ENT_MAX;
     status[b] = ZKA_OK;
     ok[b] = 0;
     // deserialisation checks of every point and scalar (deserializePoint / deserializeScalar would throw)
-    bool good = true;
-    {
-      uint32_t x[PGL], y[PGL], r[8];
-      for (int i = 0; i < np; i++) good = tom_parse(x, y, row + (size_t)i * WP) && good;
-      if (kind == SUB_EQ) {
-        for (int i = 0; i < 2; i++) good = tom_parse(x, y, proof + (size_t)i * WP) && good;
-        for (int i = 0; i < 3; i++) good = wscalar_parse(r, proof + 2 * WP + (size_t)i * WS) && good;
-      } else {
-        const int nm = kind == SUB_MULT ? 1 : 4;
-        const uint8_t* m0 = kind == SUB_MULT ? proof : proof + 4 * WP;
-        if (kind == SUB_PADD) for (int i = 0; i < 4; i++) good = tom_parse(x, y, proof + (size_t)i * WP) && good;
-        for (int m = 0; m < nm; m++) {
-          for (int i = 0; i < 6; i++) good = tom_parse(x, y, m0 + (size_t)m * MULT_LEN + (size_t)i * WP) && good;
-          for (int i = 0; i < 7; i++) good = wscalar_parse(r, m0 + (size_t)m * MULT_LEN + 6 * WP + (size_t)i * WS) && good;
-        }
-        if (kind == SUB_PADD)
-          for (int e = 0; e < 2; e++) {
-            const uint8_t* ep = proof + 4 * WP + 4 * MULT_LEN + (size_t)e * EQ_LEN;
-            for (int i = 0; i < 2; i++) good = tom_parse(x, y, ep + (size_t)i * WP) && good;
-            for (int i = 0; i < 3; i++) good = wscalar_parse(r, ep + 2 * WP + (size_t)i * WS) && good;
-          }
-      }
-    }
-    Fold f;
+    bool good = valid_points(row, np);
+    good = (kind == SUB_EQ ? valid_equality(proof) : kind == SUB_MULT ? valid_mult(proof) : valid_point_add(proof)) && good;
+    SigmaFold f;
     zero_n<8>(f.gW); zero_n<8>(f.hW);
     f.tape_ok = true;
     uint32_t zero[8];
     zero_n<8>(zero);
-    for (int e = 0; e < SUB_ENT_MAX; e++) emit(b, e, zero, 0);   // unused entries: scalar 0 on the first input point
+    for (int e = 0; e < SUB_ENT_MAX; e++) out.put(e0 + e, zero, 0);   // unused entries: scalar 0 on the first input point
     if (!good) {
       ZK_SET_STATUS(status + b, ZKA_ERR_MALFORMED);
     } else if (kind == SUB_EQ) {
-      uint32_t c1[8], c2[8], es[2][8];
-      zero_n<8>(c1); zero_n<8>(c2);
-      equality(f, row, row + WP, proof, dr, c1, c2, es);
-      emit_m(b, 0, c1, 0); emit_m(b, 1, c2, WP);
-      emit(b, 2, es[0], poff); emit(b, 3, es[1], poff + WP);
+      uint32_t c3[3], a[2][8], es[2][8];
+      zero_n<8>(a[0]); zero_n<8>(a[1]);
+      sigma_challenge(c3, row, row + WP, nullptr, proof, 2);
+      fold_equality(f, c3, proof, dr, a[0], a[1], es);
+      for (int i = 0; i < 2; i++) { out.put_m(e0 + i, a[i], (uint32_t)i * WP); out.put(e0 + 2 + i, es[i], poff + (uint32_t)i * WP); }
     } else if (kind == SUB_MULT) {
-      uint32_t cx[8], cy[8], cz[8], es[6][8];
-      zero_n<8>(cx); zero_n<8>(cy); zero_n<8>(cz);
-      mult(f, row, row + WP, row + 2 * WP, proof, dr, cx, cy, cz, es);
-      emit_m(b, 0, cx, 0); emit_m(b, 1, cy, WP); emit_m(b, 2, cz, 2 * WP);
-      for (int i = 0; i < 6; i++) emit(b, 3 + i, es[i], poff + (uint32_t)i * WP);
+      uint32_t c3[3], a[3][8], es[6][8];
+      zero_n<8>(a[0]); zero_n<8>(a[1]); zero_n<8>(a[2]);
+      sigma_challenge(c3, row, row + WP, row + 2 * WP, proof, 6);
+      fold_mult(f, c3, proof, dr, a[0], a[1], a[2], es);
+      for (int i = 0; i < 3; i++) out.put_m(e0 + i, a[i], (uint32_t)i * WP);
+      for (int i = 0; i < 6; i++) out.put(e0 + 3 + i, es[i], poff + (uint32_t)i * WP);
     } else {
-      // aggregatePointAdd (pointAdd.ts:199-259): C1..C6 = PX QX RX PY QY RY
-      const uint8_t *PX = row, *PY = row + WP, *QX = row + 2 * WP, *QY = row + 3 * WP, *RX = row + 4 * WP, *RY = row + 5 * WP;
-      TomPt p1, p2, p3, p4, p5, p6, n, r;
+      // aggregatePointAdd (pointAdd.ts:199-259): C1..C6 = PX QX RX PY QY RY, at row slot (k % 3) * 2 + k / 3
+      TomPt p[6];
       uint32_t x[PGL], y[PGL];
-      tom_parse(x, y, PX); tom_from_affine(p1, x, y);
-      tom_parse(x, y, QX); tom_from_affine(p2, x, y);
-      tom_parse(x, y, RX); tom_from_affine(p3, x, y);
-      tom_parse(x, y, PY); tom_from_affine(p4, x, y);
-      tom_parse(x, y, QY); tom_from_affine(p5, x, y);
-      tom_parse(x, y, RY); tom_from_affine(p6, x, y);
-      uint8_t d7[BSTRIDE], d9[BSTRIDE], d12[BSTRIDE], dix[BSTRIDE], diy[BSTRIDE];
-      tom_neg(n, p1); tom_add(r, p2, n); tom_encode_proj(d7, r);        // C7 = C2 - C1
-      tom_neg(n, p4); tom_add(r, p5, n); tom_encode_proj(d9, r);        // C9 = C5 - C4
-      tom_neg(n, p3); tom_add(r, p1, n); tom_encode_proj(d12, r);       // C12 = C1 - C3
-      tom_add(r, p3, p1); tom_add(r, r, p2); tom_encode_proj(dix, r);   // Cint = C3 + C1 + C2
-      tom_add(r, p4, p6); tom_encode_proj(diy, r);                      // Cint = C4 + C6
-      const uint8_t *C8 = proof, *C10 = proof + WP, *C11 = proof + 2 * WP, *C13 = proof + 3 * WP;
-      const uint8_t* mp = proof + 4 * WP;
-      const uint8_t* ep = mp + 4 * MULT_LEN;
-      uint32_t a7[8], a8[8], a9[8], a10[8], a11[8], a12[8], a13[8], aix[8], aiy[8], ag[8];
-      zero_n<8>(a7); zero_n<8>(a8); zero_n<8>(a9); zero_n<8>(a10); zero_n<8>(a11); zero_n<8>(a12); zero_n<8>(a13);
-      zero_n<8>(aix); zero_n<8>(aiy); zero_n<8>(ag);
-      uint32_t es[6][8], ee[2][8];
-      const uint32_t om = poff + 4 * WP, oe = om + 4 * MULT_LEN;
-      mult(f, d7, C8, tg_bytes, mp, dr, a7, a8, ag, es);                                  // pi_8
-      for (int i = 0; i < 6; i++) emit(b, 10 + i, es[i], om + (uint32_t)i * WP);
-      mult(f, C8, d9, C10, mp + MULT_LEN, dr + 32 * 5, a8, a9, a10, es);                  // pi_10
-      for (int i = 0; i < 6; i++) emit(b, 16 + i, es[i], om + MULT_LEN + (uint32_t)i * WP);
-      mult(f, C10, C10, C11, mp + 2 * MULT_LEN, dr + 32 * 10, a10, a10, a11, es);         // pi_11
-      for (int i = 0; i < 6; i++) emit(b, 22 + i, es[i], om + 2 * MULT_LEN + (uint32_t)i * WP);
-      equality(f, C11, dix, ep, dr + 32 * 15, a11, aix, ee);                              // pi_x
-      emit(b, 34, ee[0], oe); emit(b, 35, ee[1], oe + WP);
-      mult(f, C10, d12, C13, mp + 3 * MULT_LEN, dr + 32 * 17, a10, a12, a13, es);         // pi_13
-      for (int i = 0; i < 6; i++) emit(b, 28 + i, es[i], om + 3 * MULT_LEN + (uint32_t)i * WP);
-      equality(f, C13, diy, ep + EQ_LEN, dr + 32 * 22, a13, aiy, ee);                     // pi_y
-      emit(b, 36, ee[0], oe + EQ_LEN); emit(b, 37, ee[1], oe + EQ_LEN + WP);
-      acc_add(f.gW, ag);                                                                  // C_14 = g
-      // derived commitments expanded onto the inputs
-      uint32_t cPX[8], cPY[8], cQX[8], cQY[8], cRX[8], cRY[8];
-      F::sub(cPX, a12, a7); F::add(cPX, cPX, aix);       // -C7 +C12 +Cint
-      F::add(cQX, a7, aix);
-      F::sub(cRX, aix, a12);
-      F::sub(cPY, aiy, a9);
-      copy_n<8>(cQY, a9);
-      copy_n<8>(cRY, aiy);
-      emit_m(b, 0, cPX, 0); emit_m(b, 1, cPY, WP); emit_m(b, 2, cQX, 2 * WP); emit_m(b, 3, cQY, 3 * WP);
-      emit_m(b, 4, cRX, 4 * WP); emit_m(b, 5, cRY, 5 * WP);
-      emit_m(b, 6, a8, poff); emit_m(b, 7, a10, poff + WP); emit_m(b, 8, a11, poff + 2 * WP); emit_m(b, 9, a13, poff + 3 * WP);
+#pragma unroll
+      for (int k = 0; k < 6; k++) { tom_parse(x, y, row + (size_t)((k % 3) * 2 + k / 3) * WP); tom_from_affine(p[k], x, y); }
+      uint8_t der[DERS_PER_ITEM * BSTRIDE];
+      point_add_derived(DerivedBytes{der}, p[0], p[1], p[2], p[3], p[4], p[5]);
+      uint32_t chal[HASHES_PER_ITEM][3], a[PA_NCOM][8], in[6][8];
+      for (int h = 0; h < HASHES_PER_ITEM; h++) pa_challenge(chal[h], h, der, tg_bytes, proof);
+      fold_point_add(f, a, chal[0], proof, dr, out, e0 + 6, poff);
+      point_add_expand(in, a);
+#pragma unroll
+      for (int k = 0; k < 6; k++) {
+        const int slot = (k % 3) * 2 + k / 3;
+        out.put_m(e0 + slot, in[k], (uint32_t)slot * WP);
+      }
     }
     if (good && !f.tape_ok) ZK_SET_STATUS(status + b, ZKA_ERR_TAPE_RANGE);
     uint32_t v[8];
