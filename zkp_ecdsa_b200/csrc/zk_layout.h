@@ -39,7 +39,9 @@ enum : int {
   REP0_LEN = REP_HEAD + 2 * NS + PA_LEN + 2 * WS, // 3596 (exp.ts:36-40)
   HEAD_LEN = 2 * NP + 2 * WP,                     // 264  R comS1 keyXcom keyYcom
   MAX_REPS = 80,
-  BSTRIDE = 68,                                   // stride of one encoded point in the byte stores
+  // stride of one encoded point (65 or 67 bytes) in the byte stores: a multiple of 16, so that every staged encoding
+  // starts on a 16-byte boundary and moves in five 16-byte transactions (a staging layout, not part of the proof format)
+  BSTRIDE = 80,
 };
 
 ZK_LAYOUT_FN int gk_len(int n) { return 1 + 4 * n * WP + (3 * n + 1) * WS; }

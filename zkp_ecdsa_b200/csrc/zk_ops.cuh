@@ -139,9 +139,32 @@ ZK_HD void tom_ld_pre(TomPre& q, const uint32_t* m) {
 
 #endif
 
-// Encoded point (tag || x || y, big-endian coordinates of CB bytes) written as 32-bit words into a
-// 4-byte aligned BSTRIDE slot: 17 word stores instead of 65/67 byte stores (the byte index of
-// every output position is a compile-time constant after unrolling).
+// 16-byte vector loads and stores of the device build; the host simulator moves the same words one at a time
+ZK_HD void ld4(uint32_t* w, const void* p) {
+#if defined(__CUDA_ARCH__)
+  const uint4 u = *reinterpret_cast<const uint4*>(p);
+  w[0] = u.x; w[1] = u.y; w[2] = u.z; w[3] = u.w;
+#else
+  const uint32_t* q = reinterpret_cast<const uint32_t*>(p);
+  for (int i = 0; i < 4; i++) w[i] = q[i];
+#endif
+}
+ZK_HD void st4(void* p, const uint32_t* w) {
+#if defined(__CUDA_ARCH__)
+  *reinterpret_cast<uint4*>(p) = make_uint4(w[0], w[1], w[2], w[3]);
+#else
+  uint32_t* q = reinterpret_cast<uint32_t*>(p);
+  for (int i = 0; i < 4; i++) q[i] = w[i];
+#endif
+}
+// a 32-byte row of 8 words (scalar rows, affine coordinates; every such buffer is 16-byte aligned): two 16-byte transactions
+ZK_HD void ld8v(uint32_t* r, const uint32_t* p) { ld4(r, p); ld4(r + 4, p + 4); }
+ZK_HD void st8v(uint32_t* p, const uint32_t* r) { st4(p, r); st4(p + 4, r + 4); }
+ZK_HD bool aligned16(const void* p) { return ((size_t)p & 15) == 0; }
+
+// Encoded point (tag || x || y, big-endian coordinates of CB bytes) written into a BSTRIDE slot: five 16-byte stores
+// into a 16-byte aligned slot (every staging slot), 20 word stores into any other 4-byte aligned one.  The byte index
+// of every output position is a compile-time constant after unrolling; bytes past the encoding are written as 0.
 template <int N, int CB>
 ZK_HD uint32_t enc_byte(int i, uint32_t tag, const uint32_t* x, const uint32_t* y) {
   if (i == 0) return tag;
@@ -152,12 +175,18 @@ ZK_HD uint32_t enc_byte(int i, uint32_t tag, const uint32_t* x, const uint32_t* 
 }
 template <int N, int CB>
 ZK_HD void store_point_words(uint8_t* o, uint32_t tag, const uint32_t* x, const uint32_t* y) {
-  uint32_t* ow = reinterpret_cast<uint32_t*>(o);
+  uint32_t w[BSTRIDE / 4];
 #pragma unroll
-  for (int j = 0; j < BSTRIDE / 4; j++) {
-    const uint32_t w = enc_byte<N, CB>(4 * j, tag, x, y) | (enc_byte<N, CB>(4 * j + 1, tag, x, y) << 8) |
-                       (enc_byte<N, CB>(4 * j + 2, tag, x, y) << 16) | (enc_byte<N, CB>(4 * j + 3, tag, x, y) << 24);
-    ow[j] = w;
+  for (int j = 0; j < BSTRIDE / 4; j++)
+    w[j] = enc_byte<N, CB>(4 * j, tag, x, y) | (enc_byte<N, CB>(4 * j + 1, tag, x, y) << 8) |
+           (enc_byte<N, CB>(4 * j + 2, tag, x, y) << 16) | (enc_byte<N, CB>(4 * j + 3, tag, x, y) << 24);
+  if (aligned16(o)) {
+#pragma unroll
+    for (int j = 0; j < BSTRIDE / 16; j++) st4(o + 16 * j, w + 4 * j);
+  } else {
+    uint32_t* ow = reinterpret_cast<uint32_t*>(o);
+#pragma unroll
+    for (int j = 0; j < BSTRIDE / 4; j++) ow[j] = w[j];
   }
 }
 
@@ -189,9 +218,28 @@ ZK_HD uint32_t signed_digit(const uint32_t* k, int j, int w, uint32_t& carry, bo
   return neg ? (1u << w) - d : d;
 }
 
-// read a 32-byte big-endian tape draw into 8 limbs
+// read a 32-byte big-endian tape draw into 8 limbs.  A 16-byte aligned draw (every row of the library's own tape
+// buffers, and device tapes whose base and stride are multiples of 16) is two read-only 16-byte loads and eight
+// byte swaps; any other address takes 32 single-byte loads, so every caller pointer and stride stays legal.  The
+// buffer must not be written by the same kernel (the 16-byte loads go through the non-coherent read-only path).
+ZK_HD uint32_t bswap32(uint32_t x) {
+#if defined(__CUDA_ARCH__)
+  return __byte_perm(x, 0u, 0x0123);
+#else
+  return (x >> 24) | ((x >> 8) & 0xff00u) | ((x << 8) & 0xff0000u) | (x << 24);
+#endif
+}
 ZK_HD void tape_draw(uint32_t* r, const uint8_t* tape, int draw) {
   const uint8_t* p = tape + 32 * (size_t)draw;
+#if defined(__CUDA_ARCH__)
+  if (aligned16(p)) {
+    const uint4 a = __ldg(reinterpret_cast<const uint4*>(p)), b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
+    // stream word w (bytes 4w..4w+3, most significant first) is limb 7 - w
+    r[7] = bswap32(a.x); r[6] = bswap32(a.y); r[5] = bswap32(a.z); r[4] = bswap32(a.w);
+    r[3] = bswap32(b.x); r[2] = bswap32(b.y); r[1] = bswap32(b.z); r[0] = bswap32(b.w);
+    return;
+  }
+#endif
 #pragma unroll
   for (int i = 0; i < 8; i++) {
     const uint8_t* q = p + 28 - 4 * i;
@@ -659,9 +707,17 @@ ZK_HD void gk_block_sum(uint32_t* acc, const uint32_t* ring_m, const uint32_t (*
 
 // ================================================================================== hashing
 // Streams `npts` encoded points (given as (pointer, length) by a functor) through SHA-256.
-// Encodings in 4-byte aligned slots are fetched one point ahead (17 independent word loads).
+// Encodings are fetched one point ahead: five 16-byte loads from a 16-byte aligned address (every staging slot; the
+// last block also holds the encoding's final bytes, so the load stays inside memory the encoding occupies), 17
+// word loads from another 4-byte aligned one (proof rows), bytes otherwise.
 ZK_HD bool hash_pt_fetch(uint32_t* t, const uint8_t* p, int len) {
   if (((size_t)p & 3) || len < 64 || len > 68) return false;
+  if (aligned16(p)) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) ld4(t + 4 * j, p + 16 * j);
+    t[16] = len > 64 ? *reinterpret_cast<const uint32_t*>(p + 64) : 0u;
+    return true;
+  }
   const uint32_t* q = reinterpret_cast<const uint32_t*>(p);
 #pragma unroll
   for (int j = 0; j < 17; j++) t[j] = (4 * j < len) ? q[j] : 0u;
@@ -697,55 +753,139 @@ ZK_HD void challenge_to_limbs(uint32_t* r, const uint32_t* c3) {
   r[0] = c3[0]; r[1] = c3[1]; r[2] = c3[2];
 }
 
-// Store the first n bytes of a little-endian byte stream held in words w[0..NW) to an arbitrarily
-// aligned destination: <= 3 head bytes, aligned 32-bit stores built with 64-bit funnel shifts,
-// <= 3 tail bytes.  All register indices are static (the proof layout has odd field offsets, so
-// byte-wise copies were 65/67 single-byte stores per point).
-template <int NW>
-ZK_HD void store_stream(uint8_t* dst, const uint32_t* w, int n) {
-  const int head = (int)((4 - ((size_t)dst & 3)) & 3);
+// the encoded point (N = 65 or 67 bytes) at src as little-endian stream words w[0, 20): five 16-byte loads from a
+// 16-byte aligned address (every BSTRIDE slot), word loads from another 4-byte aligned one, bytes otherwise
+template <int N>
+ZK_HD void load_point(uint32_t* w, const uint8_t* src) {
+  if (aligned16(src)) {
 #pragma unroll
-  for (int i = 0; i < 3; i++)
-    if (i < head && i < n) dst[i] = (uint8_t)(w[0] >> (8 * i));
-  uint32_t* dw = reinterpret_cast<uint32_t*>(dst + head);
-  const int nw = (n - head) >> 2;
+    for (int j = 0; j < BSTRIDE / 16; j++) ld4(w + 4 * j, src + 16 * j);
+  } else if (((size_t)src & 3) == 0) {
+    const uint32_t* sw = reinterpret_cast<const uint32_t*>(src);
 #pragma unroll
-  for (int j = 0; j < NW; j++) {
-    const uint64_t pair = ((uint64_t)(j + 1 < NW ? w[j + 1] : 0u) << 32) | w[j];
-    const uint32_t v = (uint32_t)(pair >> (8 * head));
-    if (j < nw) {
-      dw[j] = v;
-    } else if (j == nw) {
+    for (int j = 0; j < BSTRIDE / 4; j++) w[j] = 4 * j < N ? sw[j] : 0u;
+  } else {
 #pragma unroll
-      for (int t = 0; t < 3; t++)
-        if (head + 4 * nw + t < n) dst[head + 4 * nw + t] = (uint8_t)(v >> (8 * t));
+    for (int j = 0; j < BSTRIDE / 4; j++) {
+      uint32_t v = 0;
+#pragma unroll
+      for (int t = 0; t < 4; t++)
+        if (4 * j + t < N) v |= (uint32_t)src[4 * j + t] << (8 * t);
+      w[j] = v;
     }
   }
 }
-// copy an encoded point (n = 65 or 67 bytes) from a 4-byte aligned BSTRIDE slot
-ZK_HD void copy_point(uint8_t* dst, const uint8_t* src, int n) {
-  const uint32_t* sw = reinterpret_cast<const uint32_t*>(src);
-  uint32_t w[BSTRIDE / 4];
-#pragma unroll
-  for (int i = 0; i < BSTRIDE / 4; i++) w[i] = sw[i];
-  store_stream<BSTRIDE / 4>(dst, w, n);
-}
-// write a canonical 8-limb scalar as a big-endian field of LEN bytes (32 or 33)
-template <int LEN>
-ZK_HD void put_scalar(uint8_t* o, const uint32_t* c) {
-  uint32_t w[9];
-#pragma unroll
-  for (int j = 0; j < 9; j++) {
-    uint32_t v = 0;
-#pragma unroll
-    for (int t = 0; t < 4; t++) {
-      const int k = 4 * j + t;               // stream position
-      const int pos = LEN - 1 - k;           // byte significance
-      if (k < LEN && pos >= 0 && pos < 32) v |= ((c[pos >> 2] >> (8 * (pos & 3))) & 0xffu) << (8 * t);
-    }
-    w[j] = v;
+
+// Writes one contiguous output region of any alignment as a byte stream.  Pieces (encoded points, scalars, single
+// bytes) are appended in order as little-endian stream words; every whole 16-byte block of the region is one 16-byte
+// store, assembled in registers with a run-time byte shift.  The region's first and last blocks may be shared with
+// neighbouring regions written by other threads (MultProof m and m + 1, a repetition head and its body): only the
+// region's own bytes of them are stored, with 4- and 1-byte stores.  All register indices are static.
+struct ByteWriter {
+  uint8_t* blk;   // the 16-byte block being assembled
+  uint32_t q[4];  // its bytes below `fill`, little-endian; zero above
+  int fill;       // bytes of the block decided so far
+  int lead;       // bytes [0, lead) of the block belong to whatever precedes the region (first block only)
+  ZK_HD explicit ByteWriter(uint8_t* dst) : blk(dst - ((size_t)dst & 15)), fill((int)((size_t)dst & 15)), lead(fill) {
+    q[0] = q[1] = q[2] = q[3] = 0;
   }
-  store_stream<9>(o, w, LEN);
-}
+  ZK_HD static uint32_t funnel(uint32_t lo, uint32_t hi, int sh) {   // high word of (hi:lo) << sh, sh in [0, 32)
+#if defined(__CUDA_ARCH__)
+    return __funnelshift_l(lo, hi, sh);
+#else
+    return (uint32_t)((((uint64_t)hi << 32) | lo) >> (32 - sh));
+#endif
+  }
+  ZK_HD void store_part(int lo, int hi) const {   // bytes [lo, hi) of the current block
+#pragma unroll
+    for (int w = 0; w < 4; w++) {
+      if (lo <= 4 * w && 4 * w + 4 <= hi) {
+        *reinterpret_cast<uint32_t*>(blk + 4 * w) = q[w];
+      } else {
+#pragma unroll
+        for (int t = 0; t < 4; t++)
+          if (lo <= 4 * w + t && 4 * w + t < hi) blk[4 * w + t] = (uint8_t)(q[w] >> (8 * t));
+      }
+    }
+  }
+  // append nb (1..16) bytes held in c[0, 4)
+  ZK_HD void chunk(const uint32_t* c, int nb) {
+    uint32_t m[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const int k = nb - 4 * i;   // bytes of word i that belong to the chunk
+      m[i] = k >= 4 ? c[i] : k <= 0 ? 0u : c[i] & ((1u << (8 * k)) - 1u);
+    }
+    const int sh = 8 * (fill & 3), ws = fill >> 2;
+    uint32_t d[5];
+    d[0] = sh ? m[0] << sh : m[0];
+#pragma unroll
+    for (int i = 1; i < 4; i++) d[i] = funnel(m[i - 1], m[i], sh);
+    d[4] = sh ? m[3] >> (32 - sh) : 0u;
+    uint32_t e[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+      uint32_t v = 0;
+#pragma unroll
+      for (int s = 0; s < 4; s++)
+        if (k - s >= 0 && k - s <= 4) v = ws == s ? d[k - s] : v;
+      e[k] = v;
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++) q[k] |= e[k];
+    fill += nb;
+    if (fill >= 16) {
+      if (lead == 0) st4(blk, q); else store_part(lead, 16);
+      blk += 16;
+      lead = 0;
+      fill -= 16;
+#pragma unroll
+      for (int k = 0; k < 4; k++) q[k] = e[4 + k];
+    }
+  }
+  // append the first NB bytes of the stream words w[0, ceil(NB / 4))
+  template <int NB>
+  ZK_HD void put(const uint32_t* w) {
+#pragma unroll
+    for (int c = 0; c < (NB + 15) / 16; c++) {
+      uint32_t v[4];
+#pragma unroll
+      for (int i = 0; i < 4; i++) v[i] = 16 * c + 4 * i < NB ? w[4 * c + i] : 0u;
+      chunk(v, NB - 16 * c < 16 ? NB - 16 * c : 16);
+    }
+  }
+  ZK_HD void put_byte(uint32_t b) {
+    const uint32_t v[4] = {b, 0u, 0u, 0u};
+    chunk(v, 1);
+  }
+  // an encoded point of N bytes (65 or 67) from a BSTRIDE slot
+  template <int N>
+  ZK_HD void put_point(const uint8_t* src) {
+    uint32_t w[BSTRIDE / 4];
+    load_point<N>(w, src);
+    put<N>(w);
+  }
+  // a canonical 8-limb scalar as a big-endian field of LEN bytes (32 or 33)
+  template <int LEN>
+  ZK_HD void put_scalar(const uint32_t* c) {
+    uint32_t w[9];
+#pragma unroll
+    for (int j = 0; j < 9; j++) {
+      uint32_t v = 0;
+#pragma unroll
+      for (int t = 0; t < 4; t++) {
+        const int k = 4 * j + t;               // stream position
+        const int pos = LEN - 1 - k;           // byte significance
+        if (k < LEN && pos >= 0 && pos < 32) v |= ((c[pos >> 2] >> (8 * (pos & 3))) & 0xffu) << (8 * t);
+      }
+      w[j] = v;
+    }
+    put<LEN>(w);
+  }
+  // store the bytes of the last, partly filled block; the writer is done
+  ZK_HD void finish() {
+    if (fill > lead) store_part(lead, fill);
+  }
+};
 
 }  // namespace zk

@@ -425,19 +425,19 @@ struct JobsATask {
     const int b = t / per, j = t % per;
     uint32_t v[8], r[8], m[8];
     if (j < 2) {
-      ld<8>(m, c.pk_aff + (size_t)b * 16 + 8 * j);
+      ld8v(m, c.pk_aff + (size_t)b * 16 + 8 * j);
       draw_checked<FpP256>(r, c, b, DRAW_PKX_R + j);
     } else {
       const int i = (j - 2) >> 1, xy = (j - 2) & 1;
       const size_t slot = (size_t)b * (c.S + 1) + i;
       if (c.pa_T_inf[slot]) ZK_SET_STATUS(c.status + b, ZKA_ERR_T_INFINITY);   // exp.ts:150-152
       if (c.pa_A_inf[slot]) ZK_SET_STATUS(c.status + b, ZKA_ERR_IDENTITY_ENC);
-      ld<8>(m, c.pa_T_aff + slot * 16 + 8 * xy);
+      ld8v(m, c.pa_T_aff + slot * 16 + 8 * xy);
       draw_checked<FpP256>(r, c, b, DRAW_REP0 + DRAWS_PER_REP * i + 2 + xy);
     }
     Fp::from_mont(v, m);  // coordinate as an integer: a scalar of the proof group
-    st<8>(c.s1_jv + (size_t)t * 8, v);
-    st<8>(c.s1_jr + (size_t)t * 8, r);
+    st8v(c.s1_jv + (size_t)t * 8, v);
+    st8v(c.s1_jr + (size_t)t * 8, r);
   }
 };
 
@@ -582,8 +582,12 @@ struct ItemScalarsTask {
   ZK_HD void job(size_t item, int j, const uint32_t* v_mont, const uint32_t* r_canon) const {
     uint32_t v[8];
     Tomq::from_mont(v, v_mont);
-    st<8>(c.s2_jv + c.s2_job(item, j) * 8, v);
-    st<8>(c.s2_jr + c.s2_job(item, j) * 8, r_canon);
+    st8v(c.s2_jv + c.s2_job(item, j) * 8, v);
+    st8v(c.s2_jr + c.s2_job(item, j) * 8, r_canon);
+  }
+  ZK_HD void job_raw(size_t item, int j, const uint32_t* v, const uint32_t* r) const {
+    st8v(c.s2_jv + c.s2_job(item, j) * 8, v);
+    st8v(c.s2_jr + c.s2_job(item, j) * 8, r);
   }
   ZK_HD void operator()(int it) const {
     using F = Tomq;
@@ -592,11 +596,11 @@ struct ItemScalarsTask {
     const int d0 = draws_before_items(c.S) + DRAWS_PER_ITEM * k;
     // coordinates (Montgomery residues mod p256.p double as F_q elements)
     uint32_t x1[8], y1[8], x2[8], y2[8], x3[8];
-    ld<8>(x1, c.pb_T1_aff + (size_t)it * 16);
-    ld<8>(y1, c.pb_T1_aff + (size_t)it * 16 + 8);
-    ld<8>(x2, c.pk_aff + (size_t)b * 16);
-    ld<8>(y2, c.pk_aff + (size_t)b * 16 + 8);
-    ld<8>(x3, c.pa_T_aff + ((size_t)b * (c.S + 1) + i) * 16);
+    ld8v(x1, c.pb_T1_aff + (size_t)it * 16);
+    ld8v(y1, c.pb_T1_aff + (size_t)it * 16 + 8);
+    ld8v(x2, c.pk_aff + (size_t)b * 16);
+    ld8v(y2, c.pk_aff + (size_t)b * 16 + 8);
+    ld8v(x3, c.pa_T_aff + ((size_t)b * (c.S + 1) + i) * 16);
     // blinders (canonical) and their Montgomery forms
     uint32_t rT1x[8], rT1y[8], rPkx[8], rPky[8], rTx[8], rTy[8];
     draw_checked<FpP256>(rT1x, c, b, d0 + IT_T1X_R);
@@ -612,7 +616,7 @@ struct ItemScalarsTask {
     // pointAdd.ts:130-136
     uint32_t i7[8], i8[8], i9[8], i10[8], i11[8], i12[8], i13[8];
     F::sub(i7, x2, x1);
-    ld<8>(i8, c.item_inv + (size_t)it * 8);   // 1 / i7 (ItemInvTask)
+    ld8v(i8, c.item_inv + (size_t)it * 8);    // 1 / i7 (ItemInvTask)
     F::sub(i9, y2, y1);
     F::mul(i10, i8, i9);
     F::sqr(i11, i10);
@@ -662,21 +666,21 @@ struct ItemScalarsTask {
       job(it, j0 + 0, t, u);
       // Ax, Ay, Az, A4_1 = commit(k_x), commit(k_y), commit(k_z), commit(k_z) (mult.ts:110-113)
       draw_checked<FpP256>(ra, c, b, dm + 3);
-      st<8>(c.s2_jv + c.s2_job(it, j0 + 1) * 8, kx); st<8>(c.s2_jr + c.s2_job(it, j0 + 1) * 8, ra);
+      job_raw(it, j0 + 1, kx, ra);
       draw_checked<FpP256>(ra, c, b, dm + 4);
-      st<8>(c.s2_jv + c.s2_job(it, j0 + 2) * 8, ky); st<8>(c.s2_jr + c.s2_job(it, j0 + 2) * 8, ra);
+      job_raw(it, j0 + 2, ky, ra);
       draw_checked<FpP256>(ra, c, b, dm + 5);
-      st<8>(c.s2_jv + c.s2_job(it, j0 + 3) * 8, kz); st<8>(c.s2_jr + c.s2_job(it, j0 + 3) * 8, ra);
+      job_raw(it, j0 + 3, kz, ra);
       draw_checked<FpP256>(ra, c, b, dm + 6);
-      st<8>(c.s2_jv + c.s2_job(it, j0 + 4) * 8, kz); st<8>(c.s2_jr + c.s2_job(it, j0 + 4) * 8, ra);
+      job_raw(it, j0 + 4, kz, ra);
       // A4_2 = Cy*k_x = (k_x y) g + (k_x ry) h   (mult.ts:114)
       F::mul(t, mkx, y);
       F::mul(u, mkx, ry);
       F::from_mont(u, u);
       job(it, j0 + 5, t, u);
       uint32_t* sm = sec + (size_t)m * 7 * 8;
-      st<8>(sm, x); st<8>(sm + 8, y); st<8>(sm + 16, z);
-      st<8>(sm + 24, rx); st<8>(sm + 32, ry); st<8>(sm + 40, rz); st<8>(sm + 48, r4);
+      st8v(sm, x); st8v(sm + 8, y); st8v(sm + 16, z);
+      st8v(sm + 24, rx); st8v(sm + 32, ry); st8v(sm + 40, rz); st8v(sm + 48, r4);
     }
     // the two EqualityProofs (pointAdd.ts:151-160): (x, r1, r2)
     for (int e = 0; e < 2; e++) {
@@ -684,13 +688,13 @@ struct ItemScalarsTask {
       uint32_t kk[8], ra[8];
       draw_checked<FpP256>(kk, c, b, de + 0);
       draw_checked<FpP256>(ra, c, b, de + 1);
-      st<8>(c.s2_jv + c.s2_job(it, JOB_EQ0 + 2 * e) * 8, kk); st<8>(c.s2_jr + c.s2_job(it, JOB_EQ0 + 2 * e) * 8, ra);
+      job_raw(it, JOB_EQ0 + 2 * e, kk, ra);
       draw_checked<FpP256>(ra, c, b, de + 2);
-      st<8>(c.s2_jv + c.s2_job(it, JOB_EQ0 + 2 * e + 1) * 8, kk); st<8>(c.s2_jr + c.s2_job(it, JOB_EQ0 + 2 * e + 1) * 8, ra);
+      job_raw(it, JOB_EQ0 + 2 * e + 1, kk, ra);
       uint32_t* se = sec + (size_t)(28 + 3 * e) * 8;
-      st<8>(se, e == 0 ? i11 : i13);
-      st<8>(se + 8, e == 0 ? m11 : m13);
-      st<8>(se + 16, e == 0 ? rcx : rcy);
+      st8v(se, e == 0 ? i11 : i13);
+      st8v(se + 8, e == 0 ? m11 : m13);
+      st8v(se + 16, e == 0 ? rcx : rcy);
     }
   }
 };
@@ -754,20 +758,20 @@ struct ItemHashTask {
 };
 
 // response t = k - c*w  (mod q): k canonical, w Montgomery, c canonical 80-bit
-ZK_HD void response(uint8_t* out, const uint32_t* k_canon, const uint32_t* cc, const uint32_t* w_mont) {
+ZK_HD void response(uint32_t* t, const uint32_t* k_canon, const uint32_t* cc, const uint32_t* w_mont) {
   using F = Tomq;
-  uint32_t cw[8], t[8];
+  uint32_t cw[8];
   F::mul(cw, cc, w_mont);   // c * (w R) / R = c*w, canonical
   F::sub(t, k_canon, cw);
-  put_scalar<WS>(out, t);
 }
 
 // Stage 8 — responses + byte assembly of one 0-bit repetition (exp.ts:212-225,
 // pointAdd.ts:162, mult.ts:122-130, equality.ts:73-77).  One thread per (item, part):
-// part 0..3 MultProof m, 4..5 EqualityProof e, 6 repetition header/tail.
+// part 0..3 MultProof m, 4..5 EqualityProof e, 6 repetition header/tail.  Each part writes its
+// contiguous byte regions through one ByteWriter each (a MultProof, an EqualityProof, z z2 C8 C10 C11 C13,
+// r1 r2), so neighbouring parts only share the edge blocks of their regions.
 struct ItemEmitTask {
   ProveCtx c;
-  ZK_HD void cp(uint8_t* dst, const uint8_t* src, int n) const { copy_point(dst, src, n); }
   ZK_HD void operator()(int t) const {
     const size_t it = (size_t)t / 7;
     const int part = t % 7;
@@ -779,38 +783,43 @@ struct ItemEmitTask {
     const uint32_t* sec = c.secrets + it * SECRETS_PER_ITEM * 8;
     if (part < 4) {
       const int m = part;
-      uint8_t* o = pa + 4 * WP + m * MULT_LEN;
-      for (int p = 0; p < 6; p++) cp(o + p * WP, c.s2_bytes + c.s2_job(it, JOB_MULT0 + 6 * m + p) * BSTRIDE, WP);
-      o += 6 * WP;
-      uint32_t cc[8], c3[3], kk[8], w[8];
+      ByteWriter o(pa + 4 * WP + m * MULT_LEN);
+#pragma unroll
+      for (int p = 0; p < 6; p++) o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_MULT0 + 6 * m + p) * BSTRIDE);
+      uint32_t cc[8], c3[3], kk[8], w[8], r[8];
       ld<3>(c3, c.item_chal + (it * HASHES_PER_ITEM + m) * 3);
       challenge_to_limbs(cc, c3);
       const int dm = d0 + item_mult_draw(m);
       const uint32_t* sm = sec + (size_t)m * 7 * 8;
       // t_x t_y t_z t_rx t_ry t_rz t_r4 ; k's: kx ky kz Ax.r Ay.r Az.r A4_1.r ; w: x y z rx ry rz r4
+#pragma unroll
       for (int q = 0; q < 7; q++) {
         tape_draw(kk, c.tape_of(b), dm + q);
         reduce_once<FpP256>(kk);
-        ld<8>(w, sm + q * 8);
-        response(o + q * WS, kk, cc, w);
+        ld8v(w, sm + q * 8);
+        response(r, kk, cc, w);
+        o.put_scalar<WS>(r);
       }
+      o.finish();
     } else if (part < 6) {
       const int e = part - 4;
-      uint8_t* o = pa + 4 * WP + 4 * MULT_LEN + e * EQ_LEN;
-      cp(o, c.s2_bytes + c.s2_job(it, JOB_EQ0 + 2 * e) * BSTRIDE, WP);
-      cp(o + WP, c.s2_bytes + c.s2_job(it, JOB_EQ0 + 2 * e + 1) * BSTRIDE, WP);
-      o += 2 * WP;
-      uint32_t cc[8], c3[3], kk[8], w[8];
+      ByteWriter o(pa + 4 * WP + 4 * MULT_LEN + e * EQ_LEN);
+      o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_EQ0 + 2 * e) * BSTRIDE);
+      o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_EQ0 + 2 * e + 1) * BSTRIDE);
+      uint32_t cc[8], c3[3], kk[8], w[8], r[8];
       ld<3>(c3, c.item_chal + (it * HASHES_PER_ITEM + 4 + e) * 3);
       challenge_to_limbs(cc, c3);
       const int de = d0 + (e == 0 ? IT_EQ0 : IT_EQ1);
       const uint32_t* se = sec + (size_t)(28 + 3 * e) * 8;
+#pragma unroll
       for (int q = 0; q < 3; q++) {   // t_x = k - c x ; t_r1 = A1.r - c C1.r ; t_r2 = A2.r - c C2.r
         tape_draw(kk, c.tape_of(b), de + q);
         reduce_once<FpP256>(kk);
-        ld<8>(w, se + q * 8);
-        response(o + q * WS, kk, cc, w);
+        ld8v(w, se + q * 8);
+        response(r, kk, cc, w);
+        o.put_scalar<WS>(r);
       }
+      o.finish();
     } else {
       // z = alpha - s1, z2 = r_i - comS1.r  (mod n)  (exp.ts:186,221); r1 = T1x.r, r2 = T1y.r
       using Fn = P256n;
@@ -819,56 +828,64 @@ struct ItemEmitTask {
       tape_draw(ri, c.tape_of(b), DRAW_REP0 + DRAWS_PER_REP * i + 1); reduce_once<FnP256>(ri);
       tape_draw(r0, c.tape_of(b), DRAW_COMS1_R); reduce_once<FnP256>(r0);
       ld<8>(s1, c.s1 + (size_t)b * 8);
+      ByteWriter o(body);                      // z z2 C8 C10 C11 C13
       Fn::sub(z, alpha, s1);
-      put_scalar<NS>(body, z);
+      o.put_scalar<NS>(z);
       Fn::sub(z, ri, r0);
-      put_scalar<NS>(body + NS, z);
-      cp(pa, c.s2_bytes + c.s2_job(it, JOB_C8) * BSTRIDE, WP);
-      cp(pa + WP, c.s2_bytes + c.s2_job(it, JOB_C10) * BSTRIDE, WP);
-      cp(pa + 2 * WP, c.s2_bytes + c.s2_job(it, JOB_C11) * BSTRIDE, WP);
-      cp(pa + 3 * WP, c.s2_bytes + c.s2_job(it, JOB_C13) * BSTRIDE, WP);
+      o.put_scalar<NS>(z);
+      o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_C8) * BSTRIDE);
+      o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_C10) * BSTRIDE);
+      o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_C11) * BSTRIDE);
+      o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_C13) * BSTRIDE);
+      o.finish();
+      ByteWriter ot(pa + PA_LEN);              // r1 r2
       uint32_t r[8];
       tape_draw(r, c.tape_of(b), d0 + IT_T1X_R); reduce_once<FpP256>(r);
-      put_scalar<WS>(pa + PA_LEN, r);
+      ot.put_scalar<WS>(r);
       tape_draw(r, c.tape_of(b), d0 + IT_T1Y_R); reduce_once<FpP256>(r);
-      put_scalar<WS>(pa + PA_LEN + WS, r);
+      ot.put_scalar<WS>(r);
+      ot.finish();
     }
   }
 };
 
 // Stage 8b — proof header and per-repetition heads/1-bit bodies.  One thread per (proof, slot),
-// slot in [0, S] (slot S writes the 264-byte header R comS1 keyXcom keyYcom).
+// slot in [0, S] (slot S writes the 264-byte header R comS1 keyXcom keyYcom).  A 0-bit repetition's
+// head is one byte region (its body is ItemEmitTask's), a 1-bit repetition is one region as a whole.
 struct RepEmitTask {
   ProveCtx c;
-  ZK_HD void cp(uint8_t* dst, const uint8_t* src, int n) const { copy_point(dst, src, n); }
   ZK_HD void operator()(int t) const {
     const int S1 = c.S + 1;
     const int b = t / S1, i = t % S1;
     uint8_t* proof = c.proofs + (size_t)b * c.proof_stride;
     if (i == c.S) {
       if (c.mode == 1) return;   // proveExp alone: the row holds the repetitions only
-      cp(proof, c.r_bytes + (size_t)b * BSTRIDE, NP);
-      cp(proof + NP, c.pa_A_bytes + ((size_t)b * S1 + c.S) * BSTRIDE, NP);
-      cp(proof + 2 * NP, c.s1_bytes + c.s1_pt(b, 0) * BSTRIDE, WP);
-      cp(proof + 2 * NP + WP, c.s1_bytes + c.s1_pt(b, 1) * BSTRIDE, WP);
+      ByteWriter o(proof);
+      o.put_point<NP>(c.r_bytes + (size_t)b * BSTRIDE);
+      o.put_point<NP>(c.pa_A_bytes + ((size_t)b * S1 + c.S) * BSTRIDE);
+      o.put_point<WP>(c.s1_bytes + c.s1_pt(b, 0) * BSTRIDE);
+      o.put_point<WP>(c.s1_bytes + c.s1_pt(b, 1) * BSTRIDE);
+      o.finish();
       if (c.pa_A_inf[(size_t)b * S1 + c.S]) ZK_SET_STATUS(c.status + b, ZKA_ERR_IDENTITY_ENC);
       return;
     }
     uint8_t* rep = proof + c.rep_off[(size_t)b * c.S + i];
     const uint32_t bit = (c.chal[(size_t)b * 3 + (i >> 5)] >> (i & 31)) & 1u;
-    rep[0] = (uint8_t)bit;
-    cp(rep + 1, c.pa_A_bytes + ((size_t)b * S1 + i) * BSTRIDE, NP);
-    cp(rep + 1 + NP, c.s1_bytes + c.s1_pt(b, 2 + 2 * i) * BSTRIDE, WP);
-    cp(rep + 1 + NP + WP, c.s1_bytes + c.s1_pt(b, 3 + 2 * i) * BSTRIDE, WP);
+    ByteWriter o(rep);
+    o.put_byte(bit);
+    o.put_point<NP>(c.pa_A_bytes + ((size_t)b * S1 + i) * BSTRIDE);
+    o.put_point<WP>(c.s1_bytes + c.s1_pt(b, 2 + 2 * i) * BSTRIDE);
+    o.put_point<WP>(c.s1_bytes + c.s1_pt(b, 3 + 2 * i) * BSTRIDE);
     if (bit) {   // exp.ts:170-183: alpha, r, Tx.r, Ty.r
-      uint8_t* o = rep + REP_HEAD;
       uint32_t r[8];
+#pragma unroll
       for (int q = 0; q < 4; q++) {
         tape_draw(r, c.tape_of(b), DRAW_REP0 + DRAWS_PER_REP * i + q);
-        if (q < 2) { reduce_once<FnP256>(r); put_scalar<NS>(o, r); o += NS; }
-        else       { reduce_once<FpP256>(r); put_scalar<WS>(o, r); o += WS; }
+        if (q < 2) { reduce_once<FnP256>(r); o.put_scalar<NS>(r); }
+        else       { reduce_once<FpP256>(r); o.put_scalar<WS>(r); }
       }
     }
+    o.finish();
   }
 };
 
@@ -893,12 +910,12 @@ struct GkJobsTask {
     zero_n<8>(v);
     v[0] = bit;
     size_t j = c.s2_gk(b, i);                        // cl_i
-    st<8>(c.s2_jv + j * 8, v); st<8>(c.s2_jr + j * 8, ri);
+    st8v(c.s2_jv + j * 8, v); st8v(c.s2_jr + j * 8, ri);
     j = c.s2_gk(b, c.n + i);                         // ca_i
-    st<8>(c.s2_jv + j * 8, ai); st<8>(c.s2_jr + j * 8, si);
+    st8v(c.s2_jv + j * 8, ai); st8v(c.s2_jr + j * 8, si);
     j = c.s2_gk(b, 2 * c.n + i);                     // cb_i
     if (bit) copy_n<8>(v, ai); else zero_n<8>(v);
-    st<8>(c.s2_jv + j * 8, v); st<8>(c.s2_jr + j * 8, ti);
+    st8v(c.s2_jv + j * 8, v); st8v(c.s2_jr + j * 8, ti);
   }
 };
 
@@ -1051,16 +1068,16 @@ struct GkEmitTask {
     st<3>(c.gk_x + (size_t)b * 3, c3);
     challenge_to_limbs(xc, c3);
     F::to_mont(xm, xc);
+    // byte regions: n and the 4n points, then the f, za and zb arrays (zd follows zb)
     uint8_t* o = c.proofs + (size_t)b * c.proof_stride + c.gk_off[b];
-    *o++ = (uint8_t)n;
-    for (int k = 0; k < 4 * n; k++) {
-      copy_point(o, c.s2_bytes + c.s2_gk(b, k) * BSTRIDE, WP);
-      o += WP;
+    {
+      ByteWriter op(o);
+      op.put_byte((uint32_t)n);
+      for (int k = 0; k < 4 * n; k++) op.put_point<WP>(c.s2_bytes + c.s2_gk(b, k) * BSTRIDE);
+      op.finish();
     }
-    uint8_t* of = o;
-    uint8_t* oza = o + (size_t)n * WS;
-    uint8_t* ozb = o + (size_t)2 * n * WS;
-    uint8_t* ozd = o + (size_t)3 * n * WS;
+    o += 1 + (size_t)4 * n * WP;
+    ByteWriter of(o), oza(o + (size_t)n * WS), ozb(o + (size_t)2 * n * WS);
     const int d0 = gk_draw0(c, b);
     uint32_t zd[8], xp[8], t[8], u[8];
     // zd = pkX.r * x^n - sum rho_i x^i
@@ -1077,17 +1094,17 @@ struct GkEmitTask {
       // f_i = l_i x + a_i
       uint32_t f[8];
       if (bit) F::add(f, xc, ai); else copy_n<8>(f, ai);
-      put_scalar<WS>(of + (size_t)i * WS, f);
+      of.put_scalar<WS>(f);
       // za_i = r_i x + s_i
       F::mul(t, ri, xm);          // canonical r_i * x
       F::add(u, t, si);
-      put_scalar<WS>(oza + (size_t)i * WS, u);
+      oza.put_scalar<WS>(u);
       // zb_i = r_i (x - f_i) + t_i
       F::sub(u, xc, f);
       F::to_mont(u, u);
       F::mul(t, ri, u);
       F::add(u, t, ti);
-      put_scalar<WS>(ozb + (size_t)i * WS, u);
+      ozb.put_scalar<WS>(u);
       // zd -= rho_i x^i   (xp = x^i in Montgomery form)
       F::mul(t, rho, xp);
       F::sub(zd, zd, t);
@@ -1097,7 +1114,10 @@ struct GkEmitTask {
     tape_draw(rpk, c.tape_of(b), DRAW_PKX_R); reduce_once<FpP256>(rpk);
     F::mul(t, rpk, xp);           // pkX.r * x^n
     F::add(zd, zd, t);
-    put_scalar<WS>(ozd, zd);
+    ozb.put_scalar<WS>(zd);
+    of.finish();
+    oza.finish();
+    ozb.finish();
   }
 };
 
@@ -1132,7 +1152,7 @@ struct GkAloneSetupTask {
   const uint8_t* com_r;    // [B][32]
   const uint8_t* tape;     // [B][tape_stride]
   size_t tape_stride;
-  uint8_t* itape;          // [B][96 + tape_stride]
+  uint8_t* itape;          // [B][c.tape_stride]: 96 + tape_stride rounded up to a multiple of 16
   ZK_HD void operator()(int b) const {
     c.status[b] = ZKA_OK;
     c.zcount[b] = 0;
@@ -1146,7 +1166,7 @@ struct GkAloneSetupTask {
     const size_t need = (size_t)32 * 5 * c.n;
     for (size_t i = 0; i < need; i++) row[96 + i] = tape[(size_t)b * tape_stride + i];
     uint32_t r[8];
-    tape_draw(r, row, DRAW_PKX_R);
+    tape_draw(r, com_r + (size_t)b * 32, 0);   // = draw DRAW_PKX_R of the row (not read back: the row is written here)
     if (!lt_p<FpP256>(r)) ZK_SET_STATUS(c.status + b, ZKA_ERR_TAPE_RANGE);
   }
 };
@@ -1164,8 +1184,8 @@ struct SubProveJobsTask {
   size_t tape_stride;
   uint32_t *jv, *jr;        // [B][4|9][8]
   int32_t* status;
-  ZK_HD bool rd(uint32_t* r, const uint8_t* p) const {
-    limbs_from_be<8>(r, p, 32);
+  ZK_HD static bool rd(uint32_t* r, const uint8_t* p, int draw = 0) {   // draw `draw` of the row at p
+    tape_draw(r, p, draw);
     if (lt_p<FpP256>(r)) return true;
     sub_p<FpP256>(r, r);
     return false;
@@ -1182,14 +1202,14 @@ struct SubProveJobsTask {
     if (kind == 0) {
       uint32_t x[8], r1[8], r2[8], k[8], ra[8], rb[8];
       rd(x, sc); rd(r1, sc + 32); rd(r2, sc + 64);      // newScalar reduces the statement's values
-      ok = rd(k, dr) && ok; ok = rd(ra, dr + 32) && ok; ok = rd(rb, dr + 64) && ok;
+      ok = rd(k, dr, 0) && ok; ok = rd(ra, dr, 1) && ok; ok = rd(rb, dr, 2) && ok;
       st<8>(v, x); st<8>(r, r1); st<8>(v + 8, x); st<8>(r + 8, r2);
       st<8>(v + 16, k); st<8>(r + 16, ra); st<8>(v + 24, k); st<8>(r + 24, rb);
     } else {
       uint32_t x[8], y[8], z[8], rx[8], ry[8], rz[8], kx[8], ky[8], kz[8], a1[8], a2[8], a3[8], a4[8];
       rd(x, sc); rd(y, sc + 32); rd(z, sc + 64); rd(rx, sc + 96); rd(ry, sc + 128); rd(rz, sc + 160);
-      ok = rd(kx, dr) && ok; ok = rd(ky, dr + 32) && ok; ok = rd(kz, dr + 64) && ok;
-      ok = rd(a1, dr + 96) && ok; ok = rd(a2, dr + 128) && ok; ok = rd(a3, dr + 160) && ok; ok = rd(a4, dr + 192) && ok;
+      ok = rd(kx, dr, 0) && ok; ok = rd(ky, dr, 1) && ok; ok = rd(kz, dr, 2) && ok;
+      ok = rd(a1, dr, 3) && ok; ok = rd(a2, dr, 4) && ok; ok = rd(a3, dr, 5) && ok; ok = rd(a4, dr, 6) && ok;
       uint32_t xm[8], kxm[8], t[8], u[8];
       F::to_mont(xm, x);
       F::to_mont(kxm, kx);
@@ -1233,24 +1253,27 @@ struct SubProveEmitTask {
     uint32_t c3[3], cc[8];
     h.final80(c3);
     challenge_to_limbs(cc, c3);
-    for (int j = 0; j < nc; j++) copy_point(com + (size_t)j * WP, pb + (size_t)j * BSTRIDE, WP);
-    for (int j = nc; j < J; j++) copy_point(out + (size_t)(j - nc) * WP, pb + (size_t)j * BSTRIDE, WP);
-    uint8_t* o = out + (size_t)(J - nc) * WP;
-    auto resp = [&](int q, const uint8_t* kbytes, const uint32_t* w_canon) {
-      uint32_t k[8], wm[8];
-      limbs_from_be<8>(k, kbytes, 32);
+    ByteWriter oc(com), o(out);
+    for (int j = 0; j < nc; j++) oc.put_point<WP>(pb + (size_t)j * BSTRIDE);
+    oc.finish();
+    for (int j = nc; j < J; j++) o.put_point<WP>(pb + (size_t)j * BSTRIDE);
+    auto resp = [&](int q, const uint32_t* w_canon) {   // response q, with draw q of the row
+      uint32_t k[8], wm[8], t[8];
+      tape_draw(k, dr, q);
       reduce_once<FpP256>(k);
       F::to_mont(wm, w_canon);
-      response(o + (size_t)q * WS, k, cc, wm);
+      response(t, k, cc, wm);
+      o.put_scalar<WS>(t);
     };
     uint32_t w[8];
     if (kind == 0) {   // t_x = k - c x, t_r1 = A1.r - c r1, t_r2 = A2.r - c r2
-      for (int q = 0; q < 3; q++) { limbs_from_be<8>(w, sc + 32 * q, 32); reduce_once<FpP256>(w); resp(q, dr + 32 * q, w); }
+      for (int q = 0; q < 3; q++) { limbs_from_be<8>(w, sc + 32 * q, 32); reduce_once<FpP256>(w); resp(q, w); }
     } else {           // t_x t_y t_z t_rx t_ry t_rz t_r4
-      for (int q = 0; q < 6; q++) { limbs_from_be<8>(w, sc + 32 * q, 32); reduce_once<FpP256>(w); resp(q, dr + 32 * q, w); }
+      for (int q = 0; q < 6; q++) { limbs_from_be<8>(w, sc + 32 * q, 32); reduce_once<FpP256>(w); resp(q, w); }
       ld<8>(w, jr + ((size_t)b * J + 3) * 8);
-      resp(6, dr + 32 * 6, w);
+      resp(6, w);
     }
+    o.finish();
   }
 };
 
@@ -1327,9 +1350,11 @@ struct PaddExtractTask {
     }
     const uint8_t* pa = c.proofs + (size_t)b * c.proof_stride + REP_HEAD + 2 * NS;
     for (int i = 0; i < PA_LEN; i++) out[i] = pa[i];
-    copy_point(com, c.s2_bytes + c.s2_job(b, JOB_T1X) * BSTRIDE, WP);
-    copy_point(com + WP, c.s2_bytes + c.s2_job(b, JOB_T1Y) * BSTRIDE, WP);
-    for (int j = 0; j < 4; j++) copy_point(com + (size_t)(2 + j) * WP, c.s1_bytes + c.s1_pt(b, j) * BSTRIDE, WP);
+    ByteWriter o(com);
+    o.put_point<WP>(c.s2_bytes + c.s2_job(b, JOB_T1X) * BSTRIDE);
+    o.put_point<WP>(c.s2_bytes + c.s2_job(b, JOB_T1Y) * BSTRIDE);
+    for (int j = 0; j < 4; j++) o.put_point<WP>(c.s1_bytes + c.s1_pt(b, j) * BSTRIDE);
+    o.finish();
   }
 };
 

@@ -1112,7 +1112,7 @@ ZK_LAYOUT_FN int sub_proof_len(int kind) { return kind == SUB_EQ ? EQ_LEN : kind
 ZK_LAYOUT_FN int sub_draws(int kind) { return kind == SUB_EQ ? 2 : kind == SUB_MULT ? 5 : 24; }
 ZK_LAYOUT_FN int sub_entries(int kind) { return kind == SUB_EQ ? 4 : kind == SUB_MULT ? 9 : SUB_ENT_MAX; }
 
-// encoding (67 bytes in a 68-byte slot) of an E1 affine point given as Montgomery (x', y)
+// encoding (67 bytes in a BSTRIDE slot) of an E1 affine point given as Montgomery (x', y)
 #if defined(ZKA_PG_WAR256)
 ZK_HD void tom_encode_affine(uint8_t* out, const uint32_t* xm, const uint32_t* ym) {
   uint32_t cx[8], cy[8];

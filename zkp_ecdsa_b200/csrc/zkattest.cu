@@ -1172,6 +1172,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
     const Output<uint32_t> lo(proof_len_out, 1);
     const Output<int32_t> so(status, 1);
     const int lanes = ctx->nlanes;
+    const size_t dev_tape_stride = (tape_stride + 15) & ~(size_t)15;   // row pitch of a host tape staged on the device
     const bool all_dev = po.dev && is_device_ptr(tape);
     const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)(all_dev ? ctx->chunk : std::min(ctx->chunk, ctx->host_chunk)), lanes, !all_dev);
     const uint32_t nchunks = (uint32_t)off.size() - 1;
@@ -1205,14 +1206,16 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         ev_record(ln.ev_small[slot], ci);
         if (is_device_ptr(tape)) {
           cin[slot].tape = tape + (size_t)b0 * tape_stride;
-        } else if (!ctx->tape_split) {
+        } else if (!ctx->tape_split && dev_tape_stride == tape_stride) {
           cin[slot].tape = stage_in(ci, tape_buf, tape + (size_t)b0 * tape_stride, Bc * tape_stride);
         } else {
-          // host tape: only the draws used before the challenge (3 + 4S of up to 3 + 44S + 5n) travel now; the
-          // item and GK draws of each proof follow after the challenge, when their number is known
-          uint8_t* dt = tape_buf.get<uint8_t>(Bc * tape_stride);
-          const size_t pre = std::min(tape_stride, (size_t)32 * draws_before_items(S));
-          copy_d2h_2d(ci, dt, tape_stride, tape + (size_t)b0 * tape_stride, tape_stride, pre, Bc);
+          // host tape: staged at a row pitch of a multiple of 16 (dev_tape_stride), so that every draw is read with
+          // 16-byte loads whatever the caller's stride.  With tape_split only the draws used before the challenge
+          // (3 + 4S of up to 3 + 44S + 5n) travel now; the item and GK draws of each proof follow after the challenge,
+          // when their number is known
+          uint8_t* dt = tape_buf.get<uint8_t>(Bc * dev_tape_stride);
+          const size_t width = ctx->tape_split ? std::min(tape_stride, (size_t)32 * draws_before_items(S)) : tape_stride;
+          copy_d2h_2d(ci, dt, dev_tape_stride, tape + (size_t)b0 * tape_stride, tape_stride, width, Bc);
           cin[slot].tape = dt;
         }
         ev_record(ln.ev_tape[slot], ci);
@@ -1239,7 +1242,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         c.pk = cin[slot].pk;
         c.which = cin[slot].which;
         c.tape = cin[slot].tape;
-        c.tape_stride = tape_stride;
+        c.tape_stride = is_device_ptr(tape) ? tape_stride : dev_tape_stride;
         c.tape_draws = (uint32_t)(tape_stride / 32);
         c.ring_m = ring_m;
         const size_t S1 = (size_t)S + 1;
@@ -1336,7 +1339,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
           const size_t o0 = (size_t)32 * draws_before_items(S);
           const size_t o1 = std::min(tape_stride, (size_t)32 * prove_draws((int)tot2[1], n, S));
           if (o1 > o0)
-            copy_d2h_2d(st, const_cast<uint8_t*>(c.tape) + o0, tape_stride, tape + (size_t)b0 * tape_stride + o0, tape_stride, o1 - o0, Bc);
+            copy_d2h_2d(st, const_cast<uint8_t*>(c.tape) + o0, c.tape_stride, tape + (size_t)b0 * tape_stride + o0, tape_stride, o1 - o0, Bc);
         }
         const double t_mid = ms_now();
         {
@@ -1441,7 +1444,9 @@ int zka_prove_membership_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, co
     const Output<uint8_t> po(proofs, proof_stride);
     const Output<uint32_t> lo(proof_len, 1);
     const Output<int32_t> so(status, 1);
-    const size_t it_stride = 96 + tape_stride;   // internal tape: [pad, com.r, pad] then the caller's draws (S = 0: GK draws start at 3)
+    // internal tape: [pad, com.r, pad] then the caller's draws (S = 0: GK draws start at 3); the row pitch is rounded up
+    // to a multiple of 16 so that every draw is read with 16-byte loads
+    const size_t it_len = 96 + tape_stride, it_stride = (it_len + 15) & ~(size_t)15;
     const uint32_t chunk = 8192;
     for (uint32_t b0 = 0; b0 < B; b0 += chunk) {
       const int Bc = (int)std::min<uint32_t>(chunk, B - b0);
@@ -1453,7 +1458,7 @@ int zka_prove_membership_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, co
       c.which = d_idx;
       c.ring_m = ring_m;
       uint8_t* itape = w.take<uint8_t>((size_t)Bc * it_stride);
-      c.tape = itape; c.tape_stride = it_stride; c.tape_draws = (uint32_t)(it_stride / 32);
+      c.tape = itape; c.tape_stride = it_stride; c.tape_draws = (uint32_t)(it_len / 32);
       c.which_s = w.take<uint32_t>(Bc);
       c.zcount = w.take<uint32_t>(Bc);
       c.gk_off = w.take<uint32_t>(Bc);
@@ -1537,7 +1542,7 @@ int zka_prove_pointadd_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, cons
   if (tape_stride < (size_t)32 * 38) return fail(ctx, ZKA_E_ARG, "tape_stride < 32 * 38");
   return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    const size_t it_stride = (size_t)32 * (9 + 38);
+    const size_t it_stride = (size_t)32 * (9 + 38);   // a multiple of 16: every draw is read with 16-byte loads
     const size_t row_stride = REP0_LEN;
     const Output<uint8_t> co(commitments, 6 * WP), po(proofs, PA_LEN);
     const Output<int32_t> so(status, 1);
