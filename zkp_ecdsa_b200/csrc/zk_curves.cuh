@@ -2,7 +2,12 @@
 //
 // P-256: homogeneous projective (X:Y:Z), complete a=-3 formulas of Renes-Costello-Batina
 //   2015 (Alg. 4 add, Alg. 5 mixed add, Alg. 6 double) — the same formulas the reference
-//   uses (/root/reference/src/curves/weier.ts:133-230), on Montgomery residues.
+//   uses (/root/reference/src/curves/weier.ts:133-230), on Montgomery residues — wherever
+//   arbitrary points meet.  The positional fixed-base walks (accum_fixed) accumulate in
+//   Jacobian coordinates with the incomplete mixed addition madd-2007-bl (7M + 4S), whose
+//   three exceptional inputs (identity accumulator, P + P, P + (-P)) are tested for and
+//   handled exactly; the doubling chains use Jacobian dbl-2001-b.  The device squaring of
+//   p256.p is a 36-product multiplier of its own.
 // tomEdwards256: the reference works on  a x^2 + y^2 = 1 + d x^2 y^2  with Hisil et al.
 //   extended coordinates (/root/reference/src/curves/edwards.ts:141-183).  Here every point
 //   is moved once to the isomorphic curve  x'^2 + y^2 = 1 + d' x'^2 y'^2  (x' = sqrt(a) x,

@@ -16,6 +16,7 @@
 //  * p256.p (8 limbs, strict): p = 2^256 - 2^224 + 2^192 + 2^96 - 1 and -1/p = 1 mod 2^32, so
 //    m_i = column word and m_i*p is five signed word additions: column k gets
 //    -m_k + m_{k-3} + m_{k-6} - m_{k-7} + m_{k-8}.  64 products instead of 136, no quotient mults.
+//    Its squaring (p256_sqr_body) forms each cross product once: 36 products.
 #pragma once
 // included from zk_field.cuh after the field descriptors and multi-word helpers
 
@@ -269,6 +270,53 @@ __device__ __forceinline__ void p256_mul_body(uint32_t* r, const uint32_t* a, co
   for (int i = 0; i < N; i++) r[i] = ge ? u[i] : t[i];
 }
 
+// r = a^2/2^256 mod p256.p, strict: input < p, output < p.  The columns of p256_mul_body with b = a: the cross
+// products a_i a_j (i < j) of a column go into a triple of their own, which is doubled (three ALU additions) and
+// added to the column accumulator with the square a_{k/2}^2 — the accumulator's carry-in must not be doubled.
+// 28 + 8 = 36 products instead of 64; the reduction is the same additions-only one.
+__device__ __forceinline__ void p256_sqr_body(uint32_t* r, const uint32_t* a) {
+  constexpr int N = 8;
+  uint32_t m[N], t[N + 1];
+  uint32_t a0 = 0, a1 = 0, a2 = 0;   // signed 96-bit column accumulator (two's complement)
+#pragma unroll
+  for (int k = 0; k < 2 * N; k++) {
+    if (k >= 1 && k <= 2 * N - 3) {  // columns with at least one cross product: 4 a_i a_j < 2^66, doubled < 2^67
+      uint32_t c0 = 0, c1 = 0, c2 = 0;
+#pragma unroll
+      for (int i = 0; i < N; i++) {
+        const int j = k - i;
+        if (i < j && j < N) mac3(c0, c1, c2, a[i], a[j]);
+      }
+      asm("add.cc.u32 %0, %0, %0;\n\t"
+          "addc.cc.u32 %1, %1, %1;\n\t"
+          "addc.u32 %2, %2, %2;\n\t"
+          "add.cc.u32 %3, %3, %0;\n\t"
+          "addc.cc.u32 %4, %4, %1;\n\t"
+          "addc.u32 %5, %5, %2;"
+          : "+r"(c0), "+r"(c1), "+r"(c2), "+r"(a0), "+r"(a1), "+r"(a2));
+    }
+    if ((k & 1) == 0 && k / 2 < N) mac3(a0, a1, a2, a[k / 2], a[k / 2]);
+    // + m_{k-3} + m_{k-6} - m_{k-7} + m_{k-8}
+    if (k - 3 >= 0 && k - 3 < N) addw(a0, a1, a2, m[k - 3 < 0 ? 0 : (k - 3 >= N ? 0 : k - 3)]);
+    if (k - 6 >= 0 && k - 6 < N) addw(a0, a1, a2, m[k - 6 < 0 ? 0 : (k - 6 >= N ? 0 : k - 6)]);
+    if (k - 7 >= 0 && k - 7 < N) subw(a0, a1, a2, m[k - 7 < 0 ? 0 : (k - 7 >= N ? 0 : k - 7)]);
+    if (k - 8 >= 0 && k - 8 < N) addw(a0, a1, a2, m[k - 8 < 0 ? 0 : (k - 8 >= N ? 0 : k - 8)]);
+    if (k < N) {
+      m[k] = a0;
+      a0 = 0;
+    } else {
+      t[k - N] = a0;
+    }
+    a0 = a1; a1 = a2; a2 = (uint32_t)((int32_t)a2 >> 31);
+  }
+  t[N] = a0;   // 0 or 1
+  uint32_t u[N];
+  uint32_t br = sub_p<FpP256>(u, t);
+  const bool ge = (t[N] != 0) || (br == 0);
+#pragma unroll
+  for (int i = 0; i < N; i++) r[i] = ge ? u[i] : t[i];
+}
+
 // ---------------------------------------------------------------------------------------------
 // p256.p, operand scanning with even/odd accumulator arrays (see tom_row).  -1/p = 1 mod 2^32, so the
 // quotient digit of row i is the limb at position i itself, and m*p = m*(2^256 - 2^224 + 2^192 + 2^96 - 1)
@@ -380,6 +428,11 @@ static __device__ __noinline__ V8 p256_mul_fn(V8 a, V8 b) {
   p256_mul_body(r.v, a.v, b.v);
   return r;
 }
+static __device__ __noinline__ V8 p256_sqr_fn(V8 a) {
+  V8 r;
+  p256_sqr_body(r.v, a.v);
+  return r;
+}
 __device__ __forceinline__ void tom_mul(uint32_t* r, const uint32_t* a, const uint32_t* b) {
 #if defined(ZKA_INLINE_MUL)
   tom_mul_body(r, a, b);
@@ -400,6 +453,18 @@ __device__ __forceinline__ void p256_mul(uint32_t* r, const uint32_t* a, const u
 #pragma unroll
   for (int i = 0; i < 8; i++) { x.v[i] = a[i]; y.v[i] = b[i]; }
   V8 z = p256_mul_fn(x, y);
+#pragma unroll
+  for (int i = 0; i < 8; i++) r[i] = z.v[i];
+#endif
+}
+__device__ __forceinline__ void p256_sqr(uint32_t* r, const uint32_t* a) {
+#if defined(ZKA_INLINE_MUL)
+  p256_sqr_body(r, a);
+#else
+  V8 x;
+#pragma unroll
+  for (int i = 0; i < 8; i++) x.v[i] = a[i];
+  V8 z = p256_sqr_fn(x);
 #pragma unroll
   for (int i = 0; i < 8; i++) r[i] = z.v[i];
 #endif

@@ -328,11 +328,13 @@ struct RPointTask {
     uint32_t m[8], u1[8], u2[8];
     ld<8>(m, c.u12 + (size_t)b * 16);     Fn::from_mont(u1, m);
     ld<8>(m, c.u12 + (size_t)b * 16 + 8); Fn::from_mont(u2, m);
-    P256Pt R;
-    p256_set_identity(R);
-    p256_accum_fixed(R, c.g_tabw, u1, c.g_w);
+    P256Jac acc;
+    p256_set_identity_jac(acc);
+    p256_accum_fixed_jac(acc, c.g_tabw, u1, c.g_w);
     const int kw = (int)c.tab_count[1];
-    p256_accum_fixed(R, c.rtab + (size_t)c.tab_of[b] * key_table_words(kw), u2, kw);
+    p256_accum_fixed_jac(acc, c.rtab + (size_t)c.tab_of[b] * key_table_words(kw), u2, kw);
+    P256Pt R;
+    p256_jac_to_hom(R, acc);
     uint32_t zi[8];
     P256Aff Ra;
     if (p256_is_identity(R)) {
@@ -382,13 +384,17 @@ struct PhaseAP256Task {
     Fn::to_mont(am, alpha);
     ld<8>(um, c.u12 + (size_t)b * 16);     Fn::mul(pm, am, um); Fn::from_mont(a1, pm);
     ld<8>(um, c.u12 + (size_t)b * 16 + 8); Fn::mul(pm, am, um); Fn::from_mont(a2, pm);
-    P256Pt T, A;
-    p256_set_identity(T);
-    p256_accum_fixed(T, c.g_tabw, a1, c.g_w);
+    // one Jacobian accumulator through G -> key -> h; only T and A are converted (jac_to_hom keeps Z = 0 for the
+    // identity, so P256NormTask's infinity flags are unchanged)
+    P256Jac acc;
+    p256_set_identity_jac(acc);
+    p256_accum_fixed_jac(acc, c.g_tabw, a1, c.g_w);
     const int kw = (int)c.tab_count[1];
-    p256_accum_fixed(T, c.rtab + (size_t)c.tab_of[b] * key_table_words(kw), a2, kw);
-    A = T;
-    p256_accum_fixed(A, c.h_tab8, r, c.h_w);
+    p256_accum_fixed_jac(acc, c.rtab + (size_t)c.tab_of[b] * key_table_words(kw), a2, kw);
+    P256Pt T, A;
+    p256_jac_to_hom(T, acc);
+    p256_accum_fixed_jac(acc, c.h_tab8, r, c.h_w);
+    p256_jac_to_hom(A, acc);
     p256_st_proj(c.pa_T + (size_t)t * P256_PROJ_WORDS, T);
     p256_st_proj(c.pa_A + (size_t)t * P256_PROJ_WORDS, A);
   }
