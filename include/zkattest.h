@@ -37,6 +37,23 @@
  *   Every draw must already be below its modulus (rnd()'s rejection loop is done by the host:
  *   the modulus of draw k depends only on k); otherwise status = ZKA_ERR_TAPE_RANGE.
  *
+ * Seeded randomness (zka_prove_batch_seeded, zka_verify_batch_seeded, zka_seed_tape).  Instead of a tape the caller
+ * gives 32 seed bytes per proof and the library expands the tape on the GPU.  The expansion is a ChaCha20 keystream
+ * (RFC 8439 2.3: 20 rounds, little-endian words, 32-bit block counter from 0) keyed by the seed, with the 96-bit nonce
+ * le32(domain) || le64(index); stream(seed, domain, index) = its blocks 0, 1, 2, ... concatenated.
+ *   prover draw k (tape order above, k < 3 + 44S + 5n): rnd(modulus of draw k) on stream(seed, 1, k) — 32 bytes at a
+ *     time read as a big-endian integer, the first one below the modulus kept — gives tape bytes [32k, 32k + 32).
+ *   verifier 32-byte slot t (the 2n + 1 GK drains, then the 25 * samples packed exp drains, in layout order): the first
+ *     32-byte candidate of stream(seed, 2, t) below p256.n.  p256.n is the smaller modulus; one bound serves every slot,
+ *     as the modulus of a packed drain depends on challenge bits (a 2^-32 relaxation of rnd() that does not affect the
+ *     soundness of the random linear combination).
+ *   verifier index byte i (i < S - 2): rnd(S - i) on stream(seed, 3, i), one byte per candidate; the pad bytes are zero.
+ * A seeded call is byte-identical to the tape call on zka_seed_tape's expansion of the same seeds.
+ * A SEED IS AS SECRET AS THE WITNESS AND MUST BE FRESH FOR EVERY PROOF: two proofs of different statements made from one
+ * seed share every alpha_i; a repetition that reveals alpha_i in one and z = alpha_i - s1 in the other gives s1, and then
+ * pk = s1 * R - Q: the signer is deanonymised.  The domains keep a seed's prover and verifier streams apart; they do not
+ * make reuse safe.  Draw seeds from the OS CSPRNG.
+ *
  * Pointers may be host or CUDA device pointers (detected per argument); host buffers are
  * staged through the library's stream.  The caller owns every buffer.
  * Return value: 0 on success, negative on a fatal (argument/CUDA) error — see zka_last_error.
@@ -141,6 +158,22 @@ int zka_verify_batch_ex(zka_ctx* ctx, const zka_params* params, uint32_t B,
                         const uint8_t* msg_hash, const uint8_t* ring, uint32_t N,
                         const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                         const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples);
+
+/* ---- seeded randomness (rule under "Seeded randomness" above): 32 bytes per proof instead of a tape ----
+ * zka_prove_batch_seeded / zka_verify_batch_seeded: zka_prove_batch / zka_verify_batch_ex with the tape expanded on the
+ * GPU from `seeds` (B x 32, host or device); every other argument, check and status is theirs.  Seeds count as the tape
+ * does for the chunk schedule (host or device buffers) and the progress flags. */
+int zka_prove_batch_seeded(zka_ctx* ctx, const zka_params* params, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
+                           const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N,
+                           const uint8_t* seeds /* B x 32 */, uint8_t* proofs, size_t proof_stride,
+                           uint32_t* proof_len, int32_t* status);
+int zka_verify_batch_seeded(zka_ctx* ctx, const zka_params* params, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
+                            uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                            const uint8_t* seeds /* B x 32 */, uint32_t samples, uint8_t* ok, int32_t* status);
+/* the tape a seed stands for: kind 0 = prover, all 3 + 44S + 5n draws (zka_prove_tape_len bytes); kind 1 = the verify
+ * layout for `samples` (zka_verify_tape_len_ex bytes).  tape: B x tape_stride, host or device. */
+int zka_seed_tape(zka_ctx* ctx, int kind, uint32_t B, const uint8_t* seeds, uint32_t ring_size, uint32_t sec_level,
+                  uint32_t samples, uint8_t* tape, size_t tape_stride);
 
 /* ---- stand-alone sub-proof verifiers: the surface of the reference's own unit tests and benches ----
  * verifyExp(paramsNIST, paramsWario, Clambda, Px, Py, pi, secparam, Q?)   /root/reference/src/exp/exp.ts:233-349

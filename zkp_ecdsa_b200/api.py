@@ -132,9 +132,20 @@ class Engine:
 
     def prove_signature_list(self, params: SystemParametersList, msg_hash: bytes, sig_bytes: bytes,
                              public_key: bytes, which: int, keys: Sequence[int],
-                             tape: Optional[bytes] = None) -> SignatureProofList:
-        """proveSignatureList (zkpAttestList.ts:104-145); `tape` replaces crypto.getRandomValues."""
+                             tape: Optional[bytes] = None, seed: Optional[bytes] = None) -> SignatureProofList:
+        """proveSignatureList (zkpAttestList.ts:104-145); `tape` replaces crypto.getRandomValues, or `seed` (32 secret,
+        never reused bytes, include/zkattest.h) has the GPU expand it.  Default: an OS-CSPRNG tape."""
         ring = _keys_to_ring(keys)
+        if seed is not None:
+            if tape is not None:
+                raise ValueError('give either tape or seed')
+            res = self.prove_batch_seeded(params, np.frombuffer(msg_hash, np.uint8).reshape(1, 32).copy(),
+                                          np.frombuffer(sig_bytes, np.uint8).reshape(1, 64).copy(),
+                                          np.frombuffer(public_key, np.uint8).reshape(1, 65).copy(),
+                                          np.array([which], np.uint32), ring, _seed_rows(seed, 1))
+            if res.status[0]:
+                raise ZkaProofError(res.status[0])
+            return SignatureProofList(res.proof_bytes(0))
         ts = self.lib.prove_tape_len(len(keys), params.sec_level)
         if tape is None:
             t = synth_os_tape(1, ts, params.sec_level)
@@ -150,19 +161,26 @@ class Engine:
         return SignatureProofList(res.proof_bytes(0))
 
     def verify_signature_list(self, params: SystemParametersList, msg_hash: bytes, keys: Sequence[int],
-                              proof: SignatureProofList, tape: Optional[bytes] = None) -> bool:
-        """verifySignatureList (zkpAttestList.ts:147-184): True/False, raises on malformed input."""
+                              proof: SignatureProofList, tape: Optional[bytes] = None, seed: Optional[bytes] = None) -> bool:
+        """verifySignatureList (zkpAttestList.ts:147-184): True/False, raises on malformed input.  `tape` or `seed` (32
+        bytes the GPU expands into the verifier's randomness) replace the default OS-CSPRNG tape."""
+        if seed is not None and tape is not None:
+            raise ValueError('give either tape or seed')
         ring = _keys_to_ring(keys)
-        ts = self.lib.verify_tape_len(len(keys), params.sec_level)
-        if tape is None:
-            t = synth_os_verify_tape(1, ts, len(keys), params.sec_level)
-        else:
-            t = np.zeros((1, ts), np.uint8)
-            t[0, :min(ts, len(tape))] = np.frombuffer(tape[:ts], np.uint8)
         stride = max(len(proof.data), 1)
         pr = np.frombuffer(proof.data, np.uint8).reshape(1, stride).copy()
-        ok, st = self.verify_batch(params, np.frombuffer(msg_hash, np.uint8).reshape(1, 32).copy(), ring, pr,
-                                   np.array([len(proof.data)], np.uint32), t)
+        msg = np.frombuffer(msg_hash, np.uint8).reshape(1, 32).copy()
+        plen = np.array([len(proof.data)], np.uint32)
+        if seed is not None:
+            ok, st = self.verify_batch_seeded(params, msg, ring, pr, plen, _seed_rows(seed, 1))
+        else:
+            ts = self.lib.verify_tape_len(len(keys), params.sec_level)
+            if tape is None:
+                t = synth_os_verify_tape(1, ts, len(keys), params.sec_level)
+            else:
+                t = np.zeros((1, ts), np.uint8)
+                t[0, :min(ts, len(tape))] = np.frombuffer(tape[:ts], np.uint8)
+            ok, st = self.verify_batch(params, msg, ring, pr, plen, t)
         if st[0]:
             raise ZkaProofError(st[0])
         return bool(ok[0])
@@ -187,6 +205,38 @@ class Engine:
         self.lib.verify_batch(params.handle, B, msg_hash, ring, ring.shape[0], proofs, proofs.shape[1], proof_len,
                               tape, tape.shape[1], ok, status)
         return ok, status
+
+    def prove_batch_seeded(self, params, msg_hash, sig, pk, which, ring, seeds=None, proofs=None) -> ProveResult:
+        """prove_batch with the randomness expanded on the GPU from `seeds` (B x 32 uint8, secret, one fresh seed per
+        proof; include/zkattest.h).  Default: os.urandom(32 * B)."""
+        B = msg_hash.shape[0]
+        N = ring.shape[0]
+        seeds = _seed_rows(os.urandom(32 * B), B) if seeds is None else seeds
+        stride = self.lib.proof_max_len(N, params.sec_level)
+        if proofs is None:
+            proofs = np.zeros((B, stride), np.uint8)
+        plen = np.zeros(B, np.uint32)
+        status = np.zeros(B, np.int32)
+        self.lib.prove_batch_seeded(params.handle, B, msg_hash, sig, pk, which, ring, N, seeds, proofs, proofs.shape[1], plen,
+                                    status)
+        return ProveResult(proofs, plen, status)
+
+    def verify_batch_seeded(self, params, msg_hash, ring, proofs, proof_len, seeds=None, samples: int = 20):
+        """verify_batch (`samples` sampled repetitions, 20 in verifySignatureList) with the randomness expanded on the
+        GPU from `seeds` (B x 32 uint8).  Default: os.urandom(32 * B)."""
+        B = msg_hash.shape[0]
+        seeds = _seed_rows(os.urandom(32 * B), B) if seeds is None else seeds
+        ok = np.zeros(B, np.uint8)
+        status = np.zeros(B, np.int32)
+        self.lib.verify_batch_seeded(params.handle, B, msg_hash, ring, ring.shape[0], proofs, proofs.shape[1], proof_len, seeds,
+                                     samples, ok, status)
+        return ok, status
+
+
+def _seed_rows(seed: bytes, rows: int) -> np.ndarray:
+    if len(seed) != 32 * rows:
+        raise ValueError(f'a seed is 32 bytes per proof ({32 * rows} expected, {len(seed)} given)')
+    return np.frombuffer(bytes(seed), np.uint8).reshape(rows, 32).copy()
 
 
 def _rnd_below(m: int) -> bytes:

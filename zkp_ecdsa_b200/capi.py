@@ -29,6 +29,7 @@ SYMBOLS = [
     'zka_verify_exp_batch', 'zka_verify_membership_batch', 'zka_verify_equality_batch', 'zka_verify_mult_batch',
     'zka_verify_pointadd_batch', 'zka_prove_exp_batch', 'zka_prove_membership_batch',
     'zka_prove_equality_batch', 'zka_prove_mult_batch', 'zka_prove_pointadd_batch', 'zka_stat', 'zka_proof_group', 'zka_set_progress', 'zka_chunk_schedule',
+    'zka_prove_batch_seeded', 'zka_verify_batch_seeded', 'zka_seed_tape',
 ]
 
 STATUS_MESSAGES = {
@@ -151,6 +152,13 @@ class ZkaLib:
                                           C.c_void_p, C.c_void_p]
             L.zka_proofs_unpack.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
                                             C.c_void_p, C.c_void_p]
+        if hasattr(L, 'zka_seed_tape'):
+            L.zka_prove_batch_seeded.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 5 + [C.c_uint32, C.c_void_p,
+                                                 C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+            L.zka_verify_batch_seeded.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                                  C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+            L.zka_seed_tape.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
+                                        C.c_size_t]
         ctx = C.c_void_p()
         rc = L.zka_init(device, C.byref(ctx))
         if rc != 0 or not ctx:
@@ -268,6 +276,26 @@ class ZkaLib:
         self._check(self.lib.zka_verify_batch_ex(self.ctx, params, B, _ptr(msg_hash), _ptr(ring), N, _ptr(proofs), proof_stride,
                                                  _ptr(proof_len), _ptr(tape), tape_stride, _ptr(ok), _ptr(status), samples),
                     'zka_verify_batch_ex')
+
+    # ------------------------------------------------------------------ seeded randomness
+    def prove_batch_seeded(self, params, B, msg_hash, sig, pk, which, ring, N, seeds, proofs, proof_stride, proof_len, status):
+        self._check(self.lib.zka_prove_batch_seeded(self.ctx, params, B, _ptr(msg_hash), _ptr(sig), _ptr(pk), _ptr(which), _ptr(ring),
+                                                    N, _ptr(seeds), _ptr(proofs), proof_stride, _ptr(proof_len), _ptr(status)),
+                    'zka_prove_batch_seeded')
+
+    def verify_batch_seeded(self, params, B, msg_hash, ring, N, proofs, proof_stride, proof_len, seeds, samples, ok, status):
+        self._check(self.lib.zka_verify_batch_seeded(self.ctx, params, B, _ptr(msg_hash), _ptr(ring), N, _ptr(proofs), proof_stride,
+                                                     _ptr(proof_len), _ptr(seeds), samples, _ptr(ok), _ptr(status)),
+                    'zka_verify_batch_seeded')
+
+    def seed_tape(self, kind, seeds, ring_size, sec_level=80, samples=20) -> np.ndarray:
+        """The tape `seeds` (B x 32) stand for: kind 0 the prover's (zka_prove_tape_len), 1 the verifier's for `samples`."""
+        B = seeds.shape[0]
+        ln = self.prove_tape_len(ring_size, sec_level) if kind == 0 else self.verify_tape_len_ex(ring_size, sec_level, samples)
+        out = np.zeros((B, ln), np.uint8)
+        self._check(self.lib.zka_seed_tape(self.ctx, kind, B, _ptr(seeds), ring_size, sec_level, samples, _ptr(out), ln),
+                    'zka_seed_tape')
+        return out
 
     # ------------------------------------------------------------------ stand-alone sub-proof verifiers
     def verify_exp_batch(self, params, base, com, px, py, q, proofs, proof_len, tape, samples):

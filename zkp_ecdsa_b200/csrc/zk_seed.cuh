@@ -1,0 +1,167 @@
+// zk_seed.cuh — the randomness of a seeded call: every tape draw expanded on the device from the proof's 32-byte seed.
+//
+// The rule (normative statement in include/zkattest.h, restated in oracle/seed_tape.py):
+//   stream(seed, domain, index) = ChaCha20 (RFC 8439 2.3, 20 rounds) keyed by the seed, nonce le32(domain) || le64(index),
+//                                 blocks 0, 1, 2, ... concatenated
+//   prover draw k            rnd(draw_modulus(k)) on stream(seed, 1, k): the first 32-byte big-endian candidate below
+//                            the modulus (p256.n or p256.p = tom.order, a function of k alone)
+//   verifier 32-byte slot t  the first 32-byte candidate of stream(seed, 2, t) below p256.n (GK drains, then exp drains)
+//   verifier index byte i    rnd(S - i) on stream(seed, 3, i): one byte per candidate
+// The tasks below write exactly the tape layouts of include/zkattest.h into library-owned, 16-byte aligned rows, so the
+// pipeline behind them is the tape-mode pipeline unchanged.  Pure ALU work (add, xor, rotate): no multiplier.
+#pragma once
+#include "zk_verify.cuh"
+
+namespace zk {
+
+enum : uint32_t { SEED_DOM_PROVE = 1, SEED_DOM_VERIFY = 2, SEED_DOM_INDEX = 3 };
+
+ZK_HD uint32_t chacha_rotl(uint32_t x, int n) {
+#if defined(__CUDA_ARCH__)
+  return __funnelshift_l(x, x, n);
+#else
+  return (x << n) | (x >> (32 - n));
+#endif
+}
+ZK_HD void chacha_qr(uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d) {
+  a += b; d ^= a; d = chacha_rotl(d, 16);
+  c += d; b ^= c; b = chacha_rotl(b, 12);
+  a += b; d ^= a; d = chacha_rotl(d, 8);
+  c += d; b ^= c; b = chacha_rotl(b, 7);
+}
+// One ChaCha20 block (RFC 8439 2.3): ks[i] = keystream word i, i.e. keystream bytes 4i .. 4i+3 little-endian.
+ZK_HD void chacha20_block(uint32_t* ks, const uint32_t* key, uint32_t counter, uint32_t n0, uint32_t n1, uint32_t n2) {
+  uint32_t s[16] = {0x61707865u, 0x3320646eu, 0x79622d32u, 0x6b206574u, key[0], key[1], key[2], key[3],
+                    key[4], key[5], key[6], key[7], counter, n0, n1, n2};
+  uint32_t x[16];
+#pragma unroll
+  for (int i = 0; i < 16; i++) x[i] = s[i];
+#pragma unroll
+  for (int r = 0; r < 10; r++) {
+    chacha_qr(x[0], x[4], x[8], x[12]);
+    chacha_qr(x[1], x[5], x[9], x[13]);
+    chacha_qr(x[2], x[6], x[10], x[14]);
+    chacha_qr(x[3], x[7], x[11], x[15]);
+    chacha_qr(x[0], x[5], x[10], x[15]);
+    chacha_qr(x[1], x[6], x[11], x[12]);
+    chacha_qr(x[2], x[7], x[8], x[13]);
+    chacha_qr(x[3], x[4], x[9], x[14]);
+  }
+#pragma unroll
+  for (int i = 0; i < 16; i++) ks[i] = x[i] + s[i];
+}
+
+// the seed as the ChaCha20 key: word i = le32(seed[4i .. 4i+3])
+ZK_HD void seed_key(uint32_t* key, const uint8_t* seed) {
+  if (aligned16(seed)) {
+    ld8v(key, reinterpret_cast<const uint32_t*>(seed));
+    return;
+  }
+#pragma unroll
+  for (int i = 0; i < 8; i++)
+    key[i] = (uint32_t)seed[4 * i] | ((uint32_t)seed[4 * i + 1] << 8) | ((uint32_t)seed[4 * i + 2] << 16) |
+             ((uint32_t)seed[4 * i + 3] << 24);
+}
+
+// rnd(m) for a 32-byte modulus m (8 little-endian limbs, m >= 2^255 so that a candidate passes with probability > 1/2) on
+// stream(key, domain, index): out = the kept candidate as 8 words in memory order (bytes 4w .. 4w+3 of the draw, i.e.
+// the keystream words themselves), ready to be stored as the 32 tape bytes.
+ZK_HD void seed_draw32(uint32_t* out, const uint32_t* key, uint32_t domain, uint64_t index, const uint32_t* m) {
+  for (uint32_t blk = 0;; blk++) {
+    uint32_t ks[16];
+    chacha20_block(ks, key, blk, domain, (uint32_t)index, (uint32_t)(index >> 32));
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      uint32_t v[8];   // the candidate as limbs: limb 7 - w is big-endian bytes 4w .. 4w+3
+#pragma unroll
+      for (int w = 0; w < 8; w++) v[7 - w] = bswap32(ks[8 * h + w]);
+      if (lt_n<8>(v, m)) {
+#pragma unroll
+        for (int w = 0; w < 8; w++) out[w] = ks[8 * h + w];
+        return;
+      }
+    }
+  }
+}
+
+// rnd(limit) for 1 < limit <= 256 on stream(key, SEED_DOM_INDEX, i): one byte per candidate
+ZK_HD uint32_t seed_index_byte(const uint32_t* key, uint32_t i, uint32_t limit) {
+  for (uint32_t blk = 0;; blk++) {
+    uint32_t ks[16];
+    chacha20_block(ks, key, blk, SEED_DOM_INDEX, i, 0u);
+    for (int j = 0; j < 64; j++) {
+      const uint32_t v = (ks[j >> 2] >> (8 * (j & 3))) & 0xffu;
+      if (v < limit) return v;
+    }
+  }
+}
+
+// p256.n (order_n) or p256.p = tom.order as 8 little-endian limbs
+ZK_HD void seed_modulus(uint32_t* m, bool order_n) {
+  m[0] = order_n ? 0xfc632551u : 0xffffffffu;
+  m[1] = order_n ? 0xf3b9cac2u : 0xffffffffu;
+  m[2] = order_n ? 0xa7179e84u : 0xffffffffu;
+  m[3] = order_n ? 0xbce6faadu : 0u;
+  m[4] = order_n ? 0xffffffffu : 0u;
+  m[5] = order_n ? 0xffffffffu : 0u;
+  m[6] = order_n ? 0u : 1u;
+  m[7] = 0xffffffffu;
+}
+// modulus of prover draw k (include/zkattest.h tape order): comS1.r and alpha_i, r_i mod p256.n, the rest mod tom.order
+ZK_HD bool prove_draw_mod_n(int k, int S) {
+  return k == DRAW_COMS1_R || (k >= DRAW_REP0 && k < draws_before_items(S) && ((k - DRAW_REP0) % DRAWS_PER_REP) < 2);
+}
+
+// Prover draws [d0, d0 + span) of every row: thread t = (row t / span, draw d0 + t % span), one 32-byte draw in two
+// 16-byte stores.  With zcount set, row b stops at prove_draws(zcount[b], n, S), the last draw its proof reads.
+struct SeedProveTapeTask {
+  const uint8_t* seeds;   // [B][32]
+  uint8_t* tape;          // [B][tape_stride], 16-byte aligned rows
+  size_t tape_stride;
+  int S, n, d0, span;
+  const uint32_t* zcount; // [B] or null
+  ZK_HD void operator()(int t) const {
+    const int b = t / span, k = d0 + t % span;
+    if (zcount && k >= prove_draws((int)zcount[b], n, S)) return;
+    uint32_t key[8], m[8], w[8];
+    seed_key(key, seeds + (size_t)b * 32);
+    seed_modulus(m, prove_draw_mod_n(k, S));
+    seed_draw32(w, key, SEED_DOM_PROVE, (uint64_t)k, m);
+    st8v(reinterpret_cast<uint32_t*>(tape + (size_t)b * tape_stride + (size_t)32 * k), w);
+  }
+};
+
+// The verifier layout of every row (zk_verify.cuh): thread t = (row, slot).  Slots [0, 2n + 1 + 25K) are the 32-byte
+// draws in order (GK drains, then the packed exp drains behind the index area); the V_IDX_PAD / 16 slots after them
+// write the index area 16 bytes at a time (index bytes i < S - 2, zero padding behind).
+struct SeedVerifyTapeTask {
+  const uint8_t* seeds;   // [B][32]
+  uint8_t* tape;          // [B][tape_stride], 16-byte aligned rows
+  size_t tape_stride;
+  int n, S, K;
+  ZK_HD int draws() const { return 2 * n + 1 + 25 * K; }
+  ZK_HD int slots() const { return draws() + V_IDX_PAD / 16; }
+  ZK_HD void operator()(int t) const {
+    const int b = t / slots(), s = t % slots(), g = 2 * n + 1;
+    uint32_t key[8], w[8];
+    seed_key(key, seeds + (size_t)b * 32);
+    uint8_t* row = tape + (size_t)b * tape_stride;
+    if (s < draws()) {
+      uint32_t m[8];
+      seed_modulus(m, true);
+      seed_draw32(w, key, SEED_DOM_VERIFY, (uint64_t)s, m);
+      st8v(reinterpret_cast<uint32_t*>(row + (s < g ? (size_t)32 * s : (size_t)32 * s + V_IDX_PAD)), w);
+      return;
+    }
+    const int j = s - draws();
+#pragma unroll
+    for (int q = 0; q < 4; q++) w[q] = 0;
+    for (int q = 0; q < 16; q++) {
+      const int i = 16 * j + q;
+      if (i < S - 2) w[q >> 2] |= seed_index_byte(key, (uint32_t)i, (uint32_t)(S - i)) << (8 * (q & 3));
+    }
+    st4(row + (size_t)32 * g + 16 * j, w);
+  }
+};
+
+}  // namespace zk

@@ -21,6 +21,7 @@
 
 #include "zk_launch.cuh"
 #include "zk_prove.cuh"
+#include "zk_seed.cuh"
 #include "zk_verify_agg.cuh"
 
 namespace zk {
@@ -293,7 +294,7 @@ struct Lane {
   // verifier's chunk-wide aggregate check (zk_verify_agg.cuh: its fixed parts, and one pool per MSM as the two MSMs
   // run side by side)
   DevBuf w[51];
-  DevBuf in[2][8], out[2][3];
+  DevBuf in[2][9], out[2][3];
   DevBuf agg[8], agg_tom[5 + 2 * AGG_MAX_LEVELS], agg_nist[5 + 2 * AGG_MAX_LEVELS];
   std::string err;
   ~Lane() {
@@ -1147,11 +1148,14 @@ int zka_key_to_int(zka_ctx* ctx, uint32_t count, const uint8_t* pk, uint8_t* x_o
 // ------------------------------------------------------------------------------- prove
 // mode 0: proveSignatureList.  mode 1: proveExp alone (exp.ts:126-231) — base / s_in / q_in are the statement,
 // msg_hash / sig / which / ring are unused, the rows hold the repetitions only.
+// seeds (B x 32, mode 0 only) instead of a tape: every lane expands its chunk's draws into its own tape buffer
+// (SeedProveTapeTask), the draws before the challenge first, the item and GK draws after the scan.
 static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
                       const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* tape,
                       size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out,
-                      int32_t* status, int mode, const uint8_t* base, const uint8_t* s_in, const uint8_t* q_in) {
-  if (!ctx || !P || !pk || !tape || !proofs || !proof_len_out || !status) return ZKA_E_ARG;
+                      int32_t* status, int mode, const uint8_t* base, const uint8_t* s_in, const uint8_t* q_in,
+                      const uint8_t* seeds = nullptr) {
+  if (!ctx || !P || !pk || (!tape && !seeds) || !proofs || !proof_len_out || !status) return ZKA_E_ARG;
   if (mode == 0 && (!msg_hash || !sig || !which || !ring)) return ZKA_E_ARG;
   if (mode == 1 && (!base || !s_in)) return ZKA_E_ARG;
   if (B == 0) return 0;
@@ -1160,7 +1164,10 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
   const int S = (int)P->sec_level;
   const int n = mode == 0 ? ceil_log2(N) : 0;
   if (proof_stride < (mode == 0 ? zka_proof_max_len(N, S) : (size_t)S * REP0_LEN)) return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len");
-  if (tape_stride < (size_t)32 * (mode == 0 ? prove_draws(0, n, S) : draws_before_items(S))) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
+  const bool seeded = seeds != nullptr;
+  if (!seeded && tape_stride < (size_t)32 * (mode == 0 ? prove_draws(0, n, S) : draws_before_items(S))) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
+  // seeded: the library's tape rows hold every draw a proof can read (a multiple of 32 bytes, so 16-byte aligned rows)
+  const int seed_draws = prove_draws(S, n, S);
   return guarded(ctx, [&] {
     // ring + Lagrange matrix: once per call, on lane 0, finished before the lanes start
     const uint32_t* ring_m = nullptr;
@@ -1173,7 +1180,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
     const Output<int32_t> so(status, 1);
     const int lanes = ctx->nlanes;
     const size_t dev_tape_stride = (tape_stride + 15) & ~(size_t)15;   // row pitch of a host tape staged on the device
-    const bool all_dev = po.dev && is_device_ptr(tape);
+    const bool all_dev = po.dev && is_device_ptr(seeded ? seeds : tape);
     const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)(all_dev ? ctx->chunk : std::min(ctx->chunk, ctx->host_chunk)), lanes, !all_dev);
     const uint32_t nchunks = (uint32_t)off.size() - 1;
     const int used = (int)std::min<uint32_t>((uint32_t)lanes, nchunks);
@@ -1187,7 +1194,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
     auto run_lane = [&](int li) {
       Lane& ln = ctx->lane(li);
       Stream& st = ln.st;
-      struct ChunkIn { const uint8_t *msg_hash, *sig, *pk, *tape, *base, *s_in, *q_in; const uint32_t* which; } cin[2];
+      struct ChunkIn { const uint8_t *msg_hash, *sig, *pk, *tape, *base, *s_in, *q_in, *seeds; const uint32_t* which; } cin[2];
       auto issue_inputs = [&](uint32_t k, int slot) {
         const uint32_t b0 = off[k];
         const size_t Bc = off[k + 1] - b0;
@@ -1203,8 +1210,12 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         cin[slot].base = rows(base, 65);
         cin[slot].s_in = rows(s_in, 32);
         cin[slot].q_in = rows(q_in, 65);
+        cin[slot].seeds = rows(seeds, 32);
         ev_record(ln.ev_small[slot], ci);
-        if (is_device_ptr(tape)) {
+        if (seeded) {
+          // filled on the lane's stream by SeedProveTapeTask; nothing crosses PCIe
+          cin[slot].tape = tape_buf.get<uint8_t>(Bc * (size_t)32 * seed_draws);
+        } else if (is_device_ptr(tape)) {
           cin[slot].tape = tape + (size_t)b0 * tape_stride;
         } else if (!ctx->tape_split && dev_tape_stride == tape_stride) {
           cin[slot].tape = stage_in(ci, tape_buf, tape + (size_t)b0 * tape_stride, Bc * tape_stride);
@@ -1242,8 +1253,8 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         c.pk = cin[slot].pk;
         c.which = cin[slot].which;
         c.tape = cin[slot].tape;
-        c.tape_stride = is_device_ptr(tape) ? tape_stride : dev_tape_stride;
-        c.tape_draws = (uint32_t)(tape_stride / 32);
+        c.tape_stride = seeded ? (size_t)32 * seed_draws : is_device_ptr(tape) ? tape_stride : dev_tape_stride;
+        c.tape_draws = seeded ? (uint32_t)seed_draws : (uint32_t)(tape_stride / 32);
         c.ring_m = ring_m;
         const size_t S1 = (size_t)S + 1;
         const size_t nA = (size_t)Bc * S1;
@@ -1318,6 +1329,10 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         }
         // --- phase A (first consumer of the tape) and R = u1*G + u2*pk side by side
         ev_wait(st, ln.ev_tape[slot]);
+        if (seeded) {
+          const int d1 = draws_before_items(S);
+          launch(st, (long long)Bc * d1, SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, 0, d1, nullptr});
+        }
         {
           const int nAp = (int)((nA + 31) & ~(size_t)31);
           launch(st, (long long)nAp + Bc, PhaseAAndRPointTask{PhaseAP256Task{c}, RPointTask{c}, (int)nA, nAp});
@@ -1331,9 +1346,13 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         launch(st, 1, ScanTask{c});
         uint32_t tot2[2] = {0, 0};
         copy_d2h(st, tot2, c.item_total, 8);
-        const bool tape_host = ctx->tape_split && !is_device_ptr(tape);
+        const bool tape_host = !seeded && ctx->tape_split && !is_device_ptr(tape);
         sync(st);
-        if (tape_host) {
+        if (seeded) {
+          // the item and GK draws of each proof, up to the longest proof of the chunk (zmax = tot2[1])
+          const int d1 = draws_before_items(S), span = prove_draws((int)tot2[1], n, S) - d1;
+          launch(st, (long long)Bc * span, SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, d1, span, c.zcount});
+        } else if (tape_host) {
           // second part of the tape: draws [3 + 4S, 3 + 4S + 40 zmax + 5n) of every row in one strided copy
           // (zmax = the largest zero-bit count of the chunk)
           const size_t o0 = (size_t)32 * draws_before_items(S);
@@ -1414,6 +1433,48 @@ int zka_prove_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t
                     int32_t* status) {
   return prove_impl(ctx, P, B, msg_hash, sig, pk, which, ring, N, tape, tape_stride, proofs, proof_stride, proof_len_out, status, 0,
                     nullptr, nullptr, nullptr);
+}
+
+int zka_prove_batch_seeded(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
+                           const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* seeds,
+                           uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status) {
+  if (!seeds) return ZKA_E_ARG;
+  return prove_impl(ctx, P, B, msg_hash, sig, pk, which, ring, N, nullptr, 0, proofs, proof_stride, proof_len_out, status, 0,
+                    nullptr, nullptr, nullptr, seeds);
+}
+
+// The tape a seed stands for (the rule of zk_seed.cuh): kind 0 all prove_draws(S, n, S) prover draws, kind 1 the verify
+// layout for `samples`.  Rows are expanded into a 16-byte aligned staging buffer and copied out at the caller's stride.
+int zka_seed_tape(zka_ctx* ctx, int kind, uint32_t B, const uint8_t* seeds, uint32_t ring_size, uint32_t sec_level,
+                  uint32_t samples, uint8_t* tape, size_t tape_stride) {
+  if (!ctx || !seeds || !tape || (kind != 0 && kind != 1)) return ZKA_E_ARG;
+  if (B == 0) return 0;
+  if (ring_size < 2 || ring_size > (1u << 20)) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
+  if (sec_level < 1 || sec_level > MAX_REPS) return fail(ctx, ZKA_E_ARG, "sec_level must be in [1,80]");
+  const int S = (int)sec_level, n = ceil_log2(ring_size), K = (int)samples;
+  if (kind == 1 && K < 1) return fail(ctx, ZKA_E_ARG, "samples must be >= 1");
+  if (kind == 1 && S < K) return fail(ctx, ZKA_E_ARG, "security level not achieved");
+  const size_t len = kind == 0 ? (size_t)32 * prove_draws(S, n, S) : verify_tape_len(n, S, K);   // both multiples of 16
+  if (tape_stride < len) return fail(ctx, ZKA_E_ARG, kind == 0 ? "tape_stride < zka_prove_tape_len" : "tape_stride < zka_verify_tape_len");
+  return guarded(ctx, [&] {
+    Stream& st = ctx->st;
+    const uint32_t rows = 1024;
+    for (uint32_t b0 = 0; b0 < B; b0 += rows) {
+      const uint32_t Bc = std::min(rows, B - b0);
+      Cursor in(ctx->in[0]), w(ctx->w);
+      const uint8_t* ds = stage_in(st, in.next(), seeds + (size_t)b0 * 32, (size_t)Bc * 32);
+      uint8_t* dt = w.take<uint8_t>((size_t)Bc * len);
+      if (kind == 0) {
+        launch(st, (long long)Bc * prove_draws(S, n, S), SeedProveTapeTask{ds, dt, len, S, n, 0, prove_draws(S, n, S), nullptr});
+      } else {
+        const SeedVerifyTapeTask vt{ds, dt, len, n, S, K};
+        launch(st, (long long)Bc * vt.slots(), vt);
+      }
+      copy_d2h_2d(st, tape + (size_t)b0 * tape_stride, tape_stride, dt, len, len, Bc);
+      sync(st);
+    }
+    return 0;
+  });
 }
 
 // proveExp(paramsNIST = (p256, base, NistGroup.h), paramsWario = ProofGroup, s, Cs, P = pk, Px, Py, secparam = sec_level, Q?)
@@ -1619,7 +1680,7 @@ int zka_verify_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_
 static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                        uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                        const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples, int mode,
-                       const uint8_t* q_ext);
+                       const uint8_t* q_ext, const uint8_t* seeds = nullptr);
 
 int zka_verify_batch_ex(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                         uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
@@ -1628,12 +1689,20 @@ int zka_verify_batch_ex(zka_ctx* ctx, const zka_params* P, uint32_t B, const uin
   return verify_impl(ctx, P, B, msg_hash, ring, N, proofs, proof_stride, proof_len, tape, tape_stride, ok, status, samples, 0, nullptr);
 }
 
+int zka_verify_batch_seeded(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
+                            uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                            const uint8_t* seeds, uint32_t samples, uint8_t* ok, int32_t* status) {
+  if (!msg_hash || !ring || !seeds) return ZKA_E_ARG;
+  return verify_impl(ctx, P, B, msg_hash, ring, N, proofs, proof_stride, proof_len, nullptr, 0, ok, status, samples, 0, nullptr, seeds);
+}
+
 // mode 0: verifySignatureList; mode 1: verifyExp alone on assembled rows (msg_hash / ring unused, Q from q_ext)
+// seeds (B x 32, mode 0 only) instead of a tape: SeedVerifyTapeTask expands each chunk's verify layout on the lane's stream
 static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                        uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                        const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples, int mode,
-                       const uint8_t* q_ext) {
-  if (!ctx || !P || !proofs || !proof_len || !tape || !ok || !status) return ZKA_E_ARG;
+                       const uint8_t* q_ext, const uint8_t* seeds) {
+  if (!ctx || !P || !proofs || !proof_len || (!tape && !seeds) || !ok || !status) return ZKA_E_ARG;
   if (B == 0) return 0;
   if (N < 2 || N > (1u << 20)) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
   const int S = (int)P->sec_level;
@@ -1642,8 +1711,10 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
   // verifyExp throws 'security level not achieved' when secparam > pi.length (exp.ts:243-245)
   if (S < K) return fail(ctx, ZKA_E_ARG, "security level not achieved");
   const int n = ceil_log2(N);
-  if (tape_stride < (mode == 1 ? (size_t)V_IDX_PAD + (size_t)32 * 25 * K : verify_tape_len(n, S, K)))
+  const bool seeded = seeds != nullptr;
+  if (!seeded && tape_stride < (mode == 1 ? (size_t)V_IDX_PAD + (size_t)32 * 25 * K : verify_tape_len(n, S, K)))
     return fail(ctx, ZKA_E_ARG, "tape_stride < zka_verify_tape_len");
+  const size_t seed_stride = verify_tape_len(n, S, K);   // a multiple of 16
   return guarded(ctx, [&] {
     const uint32_t* ring_m = nullptr;
     if (mode == 0) {
@@ -1653,7 +1724,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
     const Output<uint8_t> oo(ok, 1);
     const Output<int32_t> so(status, 1);
     const int lanes = ctx->nlanes;
-    const bool all_dev = is_device_ptr(proofs) && is_device_ptr(tape);
+    const bool all_dev = is_device_ptr(proofs) && is_device_ptr(seeded ? seeds : tape);
     // (two equal chunks per lane instead of the tapered host schedule: no gain at batch 8192, slower at batch 1024)
     const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)std::min(ctx->chunk, all_dev ? 4096 : std::min(4096, ctx->host_chunk)), lanes, !all_dev);
     const uint32_t nchunks = (uint32_t)off.size() - 1;
@@ -1666,7 +1737,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
     // lane's stream; the copies of one lane overlap the kernels of the others
     // the inputs of a lane's NEXT chunk travel on the copy-in stream (second set of staging buffers) while the current
     // chunk computes; a chunk's kernels wait for its event only
-    struct VIn { const uint8_t* msg; const uint8_t* proofs; const uint32_t* plen; const uint8_t* tape; };
+    struct VIn { const uint8_t* msg; const uint8_t* proofs; const uint32_t* plen; const uint8_t* tape; const uint8_t* seeds; };
     auto stage_chunk = [&](Lane& ln, int slot, uint32_t kk) {
       // ONE copy-in stream for all lanes of the call: the chunks' inputs cross PCIe in the order they were queued, each at
       // full bandwidth (with a copy stream per lane the first chunks and the prefetched ones were all in flight at once).
@@ -1691,7 +1762,9 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
         v.proofs = dp;
       }
       v.plen = stage_in(ci, in.next(), proof_len + b0, Bc);
-      v.tape = stage_in(ci, in.next(), tape + (size_t)b0 * tape_stride, Bc * tape_stride);
+      if (seeded) v.tape = in.next().get<uint8_t>(Bc * seed_stride);   // filled by SeedVerifyTapeTask
+      else v.tape = stage_in(ci, in.next(), tape + (size_t)b0 * tape_stride, Bc * tape_stride);
+      v.seeds = stage_in(ci, in.next(), seeded ? seeds + (size_t)b0 * 32 : nullptr, Bc * 32);
       ev_record(ln.ev_small[slot], ci);
       return v;
     };
@@ -1723,8 +1796,12 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       c.proof_stride = proof_stride;
       c.proof_len = cur.plen;
       c.tape = cur.tape;
-      c.tape_stride = tape_stride;
+      c.tape_stride = seeded ? seed_stride : tape_stride;
       c.ring_m = ring_m;
+      if (seeded) {
+        const SeedVerifyTapeTask vt{cur.seeds, const_cast<uint8_t*>(cur.tape), seed_stride, n, S, K};
+        launch(st, (long long)Bc * vt.slots(), vt);
+      }
       double t_in = 0.0;
       if (trace) { sync(st); t_in = ms_now(); }
       const size_t ns = (size_t)Bc * K;
