@@ -71,6 +71,7 @@ extern "C" {
 
 typedef struct zka_ctx zka_ctx;
 typedef struct zka_params zka_params;
+typedef struct zka_rings zka_rings;
 
 enum {
   ZKA_OK = 0,
@@ -174,6 +175,44 @@ int zka_verify_batch_seeded(zka_ctx* ctx, const zka_params* params, uint32_t B, 
  * layout for `samples` (zka_verify_tape_len_ex bytes).  tape: B x tape_stride, host or device. */
 int zka_seed_tape(zka_ctx* ctx, int kind, uint32_t B, const uint8_t* seeds, uint32_t ring_size, uint32_t sec_level,
                   uint32_t samples, uint8_t* tape, size_t tape_stride);
+
+/* ---- ring sets: one batch against many key rings ----
+ * The reference takes its own `keys` in every proveSignatureList / verifySignatureList call (zkpAttestList.ts:104-111,
+ * 147-152); a ring set lets one batch do the same.  zka_rings_create: R >= 1 rings, ring r of sizes[r] entries in
+ * [2, 2^20] (sizes: host memory); keys = the rings' 32-byte entries concatenated in ring order (host or device).  Each ring
+ * is reduced mod the proof-group order and padded to 2^ceil(log2 sizes[r]) entries with ITS OWN first entry, exactly as
+ * the ring of one zka_prove_batch call is (gk.ts:75-86).  ZKA_E_ARG when R = 0, a size is outside [2, 2^20] or the padded
+ * rings hold more than 2^24 entries (512 MB).  The handle belongs to its context (like zka_params): destroy it first.
+ *
+ * zka_prove_batch_rings[_seeded] / zka_verify_batch_rings[_seeded] are zka_prove_batch[_seeded] / zka_verify_batch_ex /
+ * zka_verify_batch_seeded with (ring, N) replaced by (rings, ring_of[B]): row i is proved / verified against ring
+ * ring_of[i] (host or device), and its proof bytes, verdict and status are those of the one-ring call with that ring.
+ *   - Per-row layout: each row's tape, seeded expansion, proof layout and status use its own ring size N_r and depth
+ *     n_r = ceil(log2 N_r): 3 + 4S + 40Z + 5 n_r prover draws; the verify tape starts with 2 n_r + 1 GK drains.  Strides
+ *     must cover the largest ring the call uses (zka_prove_tape_len, zka_verify_tape_len_ex, zka_proof_max_len of it).
+ *   - which[i] >= N_r gives the row status ZKA_ERR_BAD_INDEX, also inside the padding (N_r = 5, which = 6).
+ *   - Any ring_of[i] >= R: the call returns ZKA_E_ARG before any work.
+ *   - The call runs each maximal run of consecutive rows whose rings share a depth as one pass of the batched pipeline.
+ *     Rows in any order give the same bytes; rows grouped by depth are fast (interleaved depths make many small passes).
+ *   - zka_set_progress flags are not written by these calls. */
+int zka_rings_create(zka_ctx* ctx, uint32_t R, const uint32_t* sizes /* R */, const uint8_t* keys /* sum(sizes) x 32 */,
+                     zka_rings** out);
+void zka_rings_destroy(zka_rings* rings);
+int zka_prove_batch_rings(zka_ctx* ctx, const zka_params* params, const zka_rings* rings, const uint32_t* ring_of /* B */,
+                          uint32_t B, const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which,
+                          const uint8_t* tape, size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len,
+                          int32_t* status);
+int zka_prove_batch_rings_seeded(zka_ctx* ctx, const zka_params* params, const zka_rings* rings, const uint32_t* ring_of,
+                                 uint32_t B, const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which,
+                                 const uint8_t* seeds /* B x 32 */, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len,
+                                 int32_t* status);
+int zka_verify_batch_rings(zka_ctx* ctx, const zka_params* params, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
+                           const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                           const uint8_t* tape, size_t tape_stride, uint32_t samples, uint8_t* ok, int32_t* status);
+int zka_verify_batch_rings_seeded(zka_ctx* ctx, const zka_params* params, const zka_rings* rings, const uint32_t* ring_of,
+                                  uint32_t B, const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride,
+                                  const uint32_t* proof_len, const uint8_t* seeds /* B x 32 */, uint32_t samples, uint8_t* ok,
+                                  int32_t* status);
 
 /* ---- stand-alone sub-proof verifiers: the surface of the reference's own unit tests and benches ----
  * verifyExp(paramsNIST, paramsWario, Clambda, Px, Py, pi, secparam, Q?)   /root/reference/src/exp/exp.ts:233-349

@@ -82,6 +82,35 @@ class ProveResult:
         return self.proofs[b, :int(self.proof_len[b])].tobytes()
 
 
+class RingSet:
+    """R key rings on the device (zka_rings*): a batch call proves / verifies row i against ring ring_of[i]."""
+
+    def __init__(self, handle, lib, sizes: List[int]):
+        self.handle = handle
+        self._lib = lib
+        self.sizes = list(sizes)
+        self.depths = [max(1, (s - 1).bit_length()) for s in self.sizes]   # ceil(log2 N_r), N_r >= 2
+
+    def close(self) -> None:
+        """Free the device rings (zka_rings_destroy); idempotent."""
+        if self.handle is not None and self._lib is not None and getattr(self._lib, 'ctx', None):
+            self._lib.rings_destroy(self.handle)
+        self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def largest(self, ring_of) -> int:
+        """Size of the largest ring `ring_of` uses (strides are taken from it)."""
+        used = np.unique(np.asarray(ring_of, np.uint32))
+        if used.size and int(used[-1]) >= len(self.sizes):
+            raise ValueError(f'ring index {int(used[-1])} outside a set of {len(self.sizes)} rings')
+        return max((self.sizes[int(r)] for r in used), default=2)
+
+
 def _keys_to_ring(keys: Sequence[int]) -> np.ndarray:
     out = np.zeros((len(keys), 32), np.uint8)
     for i, k in enumerate(keys):
@@ -230,6 +259,67 @@ class Engine:
         status = np.zeros(B, np.int32)
         self.lib.verify_batch_seeded(params.handle, B, msg_hash, ring, ring.shape[0], proofs, proofs.shape[1], proof_len, seeds,
                                      samples, ok, status)
+        return ok, status
+
+    # ------------------------------------------------------------------ ring sets: one batch, many rings
+    def load_rings(self, rings: Sequence) -> RingSet:
+        """Upload R rings (each a sequence of ints, like `keys`, or an N x 32 uint8 array of entries) as one device set.
+        Integer entries are reduced mod the proof-group order like _keys_to_ring; array entries are taken as given (the
+        library reduces them the same way)."""
+        parts = [np.ascontiguousarray(r, np.uint8).reshape(-1, 32) if isinstance(r, np.ndarray) else _keys_to_ring(r)
+                 for r in rings]
+        sizes = np.array([p.shape[0] for p in parts], np.uint32)
+        keys = np.concatenate(parts, axis=0) if parts else np.zeros((0, 32), np.uint8)
+        return RingSet(self.lib.rings_create(sizes, keys), self.lib, [int(s) for s in sizes])
+
+    def prove_batch_rings(self, params, rings: RingSet, ring_of, msg_hash, sig, pk, which, tape, proofs=None) -> ProveResult:
+        """prove_batch with row i against ring ring_of[i] of `rings`; tape rows as wide as the largest ring used needs."""
+        B = msg_hash.shape[0]
+        ring_of = np.ascontiguousarray(ring_of, np.uint32)
+        stride = self.lib.proof_max_len(rings.largest(ring_of), params.sec_level)
+        if proofs is None:
+            proofs = np.zeros((B, stride), np.uint8)
+        plen = np.zeros(B, np.uint32)
+        status = np.zeros(B, np.int32)
+        self.lib.prove_batch_rings(params.handle, rings.handle, ring_of, B, msg_hash, sig, pk, which, tape, tape.shape[1], proofs,
+                                   proofs.shape[1], plen, status)
+        return ProveResult(proofs, plen, status)
+
+    def prove_batch_rings_seeded(self, params, rings: RingSet, ring_of, msg_hash, sig, pk, which, seeds=None,
+                                 proofs=None) -> ProveResult:
+        """prove_batch_rings with the randomness expanded on the GPU from `seeds` (B x 32).  Default: os.urandom(32 * B)."""
+        B = msg_hash.shape[0]
+        ring_of = np.ascontiguousarray(ring_of, np.uint32)
+        seeds = _seed_rows(os.urandom(32 * B), B) if seeds is None else seeds
+        stride = self.lib.proof_max_len(rings.largest(ring_of), params.sec_level)
+        if proofs is None:
+            proofs = np.zeros((B, stride), np.uint8)
+        plen = np.zeros(B, np.uint32)
+        status = np.zeros(B, np.int32)
+        self.lib.prove_batch_rings_seeded(params.handle, rings.handle, ring_of, B, msg_hash, sig, pk, which, seeds, proofs,
+                                          proofs.shape[1], plen, status)
+        return ProveResult(proofs, plen, status)
+
+    def verify_batch_rings(self, params, rings: RingSet, ring_of, msg_hash, proofs, proof_len, tape, samples: int = 20):
+        """verify_batch_ex with row i against ring ring_of[i]; tape rows cover the largest ring used."""
+        B = msg_hash.shape[0]
+        ring_of = np.ascontiguousarray(ring_of, np.uint32)
+        ok = np.zeros(B, np.uint8)
+        status = np.zeros(B, np.int32)
+        self.lib.verify_batch_rings(params.handle, rings.handle, ring_of, B, msg_hash, proofs, proofs.shape[1], proof_len, tape,
+                                    tape.shape[1], samples, ok, status)
+        return ok, status
+
+    def verify_batch_rings_seeded(self, params, rings: RingSet, ring_of, msg_hash, proofs, proof_len, seeds=None,
+                                  samples: int = 20):
+        """verify_batch_rings with the randomness expanded on the GPU from `seeds` (B x 32).  Default: os.urandom(32 * B)."""
+        B = msg_hash.shape[0]
+        ring_of = np.ascontiguousarray(ring_of, np.uint32)
+        seeds = _seed_rows(os.urandom(32 * B), B) if seeds is None else seeds
+        ok = np.zeros(B, np.uint8)
+        status = np.zeros(B, np.int32)
+        self.lib.verify_batch_rings_seeded(params.handle, rings.handle, ring_of, B, msg_hash, proofs, proofs.shape[1], proof_len, seeds,
+                                           samples, ok, status)
         return ok, status
 
 

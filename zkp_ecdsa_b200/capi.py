@@ -30,6 +30,8 @@ SYMBOLS = [
     'zka_verify_pointadd_batch', 'zka_prove_exp_batch', 'zka_prove_membership_batch',
     'zka_prove_equality_batch', 'zka_prove_mult_batch', 'zka_prove_pointadd_batch', 'zka_stat', 'zka_proof_group', 'zka_set_progress', 'zka_chunk_schedule',
     'zka_prove_batch_seeded', 'zka_verify_batch_seeded', 'zka_seed_tape',
+    'zka_rings_create', 'zka_rings_destroy', 'zka_prove_batch_rings', 'zka_prove_batch_rings_seeded', 'zka_verify_batch_rings',
+    'zka_verify_batch_rings_seeded',
 ]
 
 STATUS_MESSAGES = {
@@ -159,6 +161,18 @@ class ZkaLib:
                                                   C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
             L.zka_seed_tape.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
                                         C.c_size_t]
+        if hasattr(L, 'zka_rings_create'):
+            L.zka_rings_create.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]
+            L.zka_rings_destroy.argtypes = [C.c_void_p]
+            L.zka_prove_batch_rings.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 5 + [
+                C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+            L.zka_prove_batch_rings_seeded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 6 + [
+                C.c_size_t, C.c_void_p, C.c_void_p]
+            L.zka_verify_batch_rings.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                 C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_void_p]
+            L.zka_verify_batch_rings_seeded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                                        C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                                        C.c_void_p]
         ctx = C.c_void_p()
         rc = L.zka_init(device, C.byref(ctx))
         if rc != 0 or not ctx:
@@ -296,6 +310,40 @@ class ZkaLib:
         self._check(self.lib.zka_seed_tape(self.ctx, kind, B, _ptr(seeds), ring_size, sec_level, samples, _ptr(out), ln),
                     'zka_seed_tape')
         return out
+
+    # ------------------------------------------------------------------ ring sets (row i against ring ring_of[i])
+    def rings_create(self, sizes: np.ndarray, keys):
+        """sizes: R uint32 (host); keys: sum(sizes) x 32 bytes, host array or device pointer -> zka_rings* handle."""
+        h = C.c_void_p()
+        self._check(self.lib.zka_rings_create(self.ctx, sizes.size, _ptr(sizes), _ptr(keys), C.byref(h)), 'zka_rings_create')
+        return h
+
+    def rings_destroy(self, h):
+        self.lib.zka_rings_destroy(h)
+
+    def prove_batch_rings(self, params, rings, ring_of, B, msg_hash, sig, pk, which, tape, tape_stride, proofs, proof_stride,
+                          proof_len, status):
+        self._check(self.lib.zka_prove_batch_rings(self.ctx, params, rings, _ptr(ring_of), B, _ptr(msg_hash), _ptr(sig), _ptr(pk),
+                                                   _ptr(which), _ptr(tape), tape_stride, _ptr(proofs), proof_stride, _ptr(proof_len),
+                                                   _ptr(status)), 'zka_prove_batch_rings')
+
+    def prove_batch_rings_seeded(self, params, rings, ring_of, B, msg_hash, sig, pk, which, seeds, proofs, proof_stride, proof_len,
+                                 status):
+        self._check(self.lib.zka_prove_batch_rings_seeded(self.ctx, params, rings, _ptr(ring_of), B, _ptr(msg_hash), _ptr(sig), _ptr(pk),
+                                                          _ptr(which), _ptr(seeds), _ptr(proofs), proof_stride, _ptr(proof_len),
+                                                          _ptr(status)), 'zka_prove_batch_rings_seeded')
+
+    def verify_batch_rings(self, params, rings, ring_of, B, msg_hash, proofs, proof_stride, proof_len, tape, tape_stride, samples, ok,
+                           status):
+        self._check(self.lib.zka_verify_batch_rings(self.ctx, params, rings, _ptr(ring_of), B, _ptr(msg_hash), _ptr(proofs), proof_stride,
+                                                    _ptr(proof_len), _ptr(tape), tape_stride, samples, _ptr(ok), _ptr(status)),
+                    'zka_verify_batch_rings')
+
+    def verify_batch_rings_seeded(self, params, rings, ring_of, B, msg_hash, proofs, proof_stride, proof_len, seeds, samples, ok,
+                                  status):
+        self._check(self.lib.zka_verify_batch_rings_seeded(self.ctx, params, rings, _ptr(ring_of), B, _ptr(msg_hash), _ptr(proofs),
+                                                           proof_stride, _ptr(proof_len), _ptr(seeds), samples, _ptr(ok), _ptr(status)),
+                    'zka_verify_batch_rings_seeded')
 
     # ------------------------------------------------------------------ stand-alone sub-proof verifiers
     def verify_exp_batch(self, params, base, com, px, py, q, proofs, proof_len, tape, samples):

@@ -46,7 +46,11 @@ struct ProveCtx {
   const uint8_t* tape;       // [B][tape_stride]
   size_t tape_stride;
   uint32_t tape_draws;       // draws available per proof
-  const uint32_t* ring_m;    // [2^n] ring values mod tom.order, Montgomery, padded with ring[0]
+  const uint32_t* ring_m;    // [2^n] ring values mod tom.order, Montgomery, padded with ring[0]; with a ring set, every
+                             //    ring of the set (zka_rings), ring r at entry ring_base[r]
+  const uint32_t* ring_of;   // [B] ring-set calls: the ring of each row (null: every row uses ring_m, N entries)
+  const uint32_t* ring_base; // [R] entry offset of each padded ring of the set
+  const uint32_t* ring_size; // [R] N_r (every ring of one pass has depth n)
   // parameters / tables
   const uint32_t* g_tab8;    // P-256 generator, w=8 affine table [32][256][16]
   const uint32_t* h_tab8;    // NistGroup.h, fixed-base affine table with h_w-bit windows
@@ -118,6 +122,9 @@ struct ProveCtx {
   ZK_HD size_t s2_count() const { return (size_t)M * (JOBS_PER_ITEM + DERS_PER_ITEM) + (size_t)B * 4 * n; }
   ZK_HD size_t s1_pt(size_t b, int j) const { return b * (2 + 2 * S) + j; }  // 0 pkX, 1 pkY, 2+2i Tx_i, 3+2i Ty_i
   ZK_HD const uint8_t* tape_of(int b) const { return tape + (size_t)b * tape_stride; }
+  // the ring of row b (its 2^n padded entries) and its size
+  ZK_HD const uint32_t* ring_of_row(int b) const { return ring_of ? ring_m + (size_t)8 * ring_base[ring_of[b]] : ring_m; }
+  ZK_HD uint32_t ring_size_row(int b) const { return ring_of ? ring_size[ring_of[b]] : (uint32_t)N; }
 };
 
 // draw a scalar and check it is below the modulus (the host pre-filters, see include/zkattest.h)
@@ -187,7 +194,7 @@ struct PreKeyTask {   // validate and store the public key (everything the key t
     // an index outside the ring is flagged by RPointTask (ZKA_ERR_BAD_INDEX); the Groth-Kohlweiss tasks
     // must still stay inside ring_m[2^n], so they read this clamped copy
     const uint32_t w = c.which[b];
-    c.which_s[b] = w < (uint32_t)c.N ? w : 0u;
+    c.which_s[b] = w < c.ring_size_row(b) ? w : 0u;
   }
 };
 struct PreTask {      // the scalars of the statement and Q = z1*G
@@ -262,9 +269,9 @@ struct PreTask {      // the scalars of the statement and Q = z1*G
   }
 };
 
-// Stage 0a — equal public keys share one table.  All proofs of a call prove membership in ONE ring, so a
-// batch holds at most N distinct keys; tables (a 255-doubling chain, 780 additions and 832
-// normalisations each) are built per distinct key.  Thread b looks for the first proof with the same
+// Stage 0a — equal public keys share one table.  A chunk of Bc proofs holds up to Bc distinct keys (at most N when
+// every proof of a one-ring call is made by a ring member, up to Bc with a ring set); tables (a 255-doubling chain,
+// 780 additions and 832 normalisations each) are built per distinct key.  Thread b looks for the first proof with the same
 // (validated, Montgomery-form) key; KeyRankTask turns first occurrences into dense table indices.
 struct KeyDedupTask {
   ProveCtx c;
@@ -357,7 +364,7 @@ struct RPointTask {
     rb[0] = 0x04;
     Fp::from_mont(cv, Ra.x); limbs_to_be<8>(rb + 1, cv, 32);
     Fp::from_mont(cv, Ra.y); limbs_to_be<8>(rb + 33, cv, 32);
-    if (c.mode == 0 && c.which[b] >= (uint32_t)c.N) ZK_SET_STATUS_OVER(c.status + b, ZKA_ERR_BAD_INDEX, ZKA_ERR_TAPE_RANGE);
+    if (c.mode == 0 && c.which[b] >= c.ring_size_row(b)) ZK_SET_STATUS_OVER(c.status + b, ZKA_ERR_BAD_INDEX, ZKA_ERR_TAPE_RANGE);
   }
 };
 
@@ -955,8 +962,9 @@ struct GkPolyTask {     // one thread per (proof, w, ring block)
     }
     uint32_t dval[8], vw[8];
     zero_n<8>(dval);
-    ld<8>(vw, c.ring_m + (size_t)c.which_s[b] * 8);
-    if (!degenerate) gk_block_sum(dval, c.ring_m, f0, f1, n, k, (uint32_t)blk, vw);
+    const uint32_t* ring = c.ring_of_row(b);
+    ld<8>(vw, ring + (size_t)c.which_s[b] * 8);
+    if (!degenerate) gk_block_sum(dval, ring, f0, f1, n, k, (uint32_t)blk, vw);
     uint32_t* out = nblk == 1 ? c.gk_dv + (size_t)bw * 8 : c.gk_part + (size_t)t * 8;
     st<8>(out, dval);
   }
@@ -1165,8 +1173,9 @@ struct GkAloneSetupTask {
     c.gk_off[b] = 0;
     c.proof_len[b] = (uint32_t)gk_len(c.n);
     const uint32_t w = c.which[b];
-    c.which_s[b] = w < (uint32_t)c.N ? w : 0u;
-    if (w >= (uint32_t)c.N) ZK_SET_STATUS(c.status + b, ZKA_ERR_BAD_INDEX);
+    const uint32_t nr = c.ring_size_row(b);
+    c.which_s[b] = w < nr ? w : 0u;
+    if (w >= nr) ZK_SET_STATUS(c.status + b, ZKA_ERR_BAD_INDEX);
     uint8_t* row = itape + (size_t)b * c.tape_stride;
     for (int i = 0; i < 96; i++) row[i] = (i >= 32 && i < 64) ? com_r[(size_t)b * 32 + (i - 32)] : 0;
     const size_t need = (size_t)32 * 5 * c.n;
@@ -1391,6 +1400,31 @@ struct RingPrepTask {
     const int src = i < N ? i : 0;
     uint32_t v[8], m[8];
     limbs_from_be<8>(v, ring + (size_t)src * 32, 32);
+    reduce_once<FpP256>(v);
+    Tomq::to_mont(m, v);
+    st<8>(ring_m + (size_t)i * 8, m);
+  }
+};
+
+// every ring of a ring set at once: one thread per padded entry i finds its ring r (the last with ring_base[r] <= i) by
+// binary search, then converts and pads like RingPrepTask, ring r with its own first entry
+struct RingSetPrepTask {
+  const uint8_t* keys;         // the rings' 32-byte entries concatenated in ring order
+  const uint32_t* key_off;     // [R] first entry of ring r in `keys`
+  const uint32_t* ring_base;   // [R] first entry of ring r in ring_m (ring_base[r + 1] - ring_base[r] = 2^n_r)
+  const uint32_t* ring_size;   // [R]
+  uint32_t* ring_m;            // [total][8]
+  int R;
+  ZK_HD void operator()(int i) const {
+    int lo = 0, hi = R - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (ring_base[mid] <= (uint32_t)i) lo = mid; else hi = mid - 1;
+    }
+    const uint32_t j = (uint32_t)i - ring_base[lo];
+    const uint32_t src = key_off[lo] + (j < ring_size[lo] ? j : 0u);
+    uint32_t v[8], m[8];
+    limbs_from_be<8>(v, keys + (size_t)src * 32, 32);
     reduce_once<FpP256>(v);
     Tomq::to_mont(m, v);
     st<8>(ring_m + (size_t)i * 8, m);

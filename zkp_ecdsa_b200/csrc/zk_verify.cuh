@@ -67,7 +67,9 @@ struct VerifyCtx {
   const uint32_t* proof_len;   // [B]
   const uint8_t* tape;         // [B][tape_stride]
   size_t tape_stride;
-  const uint32_t* ring_m;      // [2^n][8] Montgomery mod q
+  const uint32_t* ring_m;      // [2^n][8] Montgomery mod q (a ring set: all its rings, see ProveCtx)
+  const uint32_t* ring_of;     // [B] ring-set calls: the ring of each row (null: ring_m for every row)
+  const uint32_t* ring_base;   // [R] entry offset of each padded ring of the set
   const uint32_t* g_tab8;
   const uint32_t* h_tab8;
   int h_w;
@@ -130,6 +132,7 @@ struct VerifyCtx {
   ZK_HD int segs() const { return (K + V_SEG - 1) / V_SEG; }
   ZK_HD const uint8_t* proof_of(int b) const { return proofs + (size_t)b * proof_stride; }
   ZK_HD const uint8_t* tape_of(int b) const { return tape + (size_t)b * tape_stride; }
+  ZK_HD const uint32_t* ring_of_row(int b) const { return ring_of ? ring_m + (size_t)8 * ring_base[ring_of[b]] : ring_m; }
   ZK_HD size_t gk_tape_bytes() const { return mode == 1 ? 0 : (size_t)32 * (2 * n + 1); }
   ZK_HD const uint8_t* exp_tape(int b) const { return tape_of(b) + gk_tape_bytes() + V_IDX_PAD; }
   ZK_HD size_t ta_pt(size_t sample, int j) const { return sample * 2 + j; }   // 0 T1x, 1 T1y
@@ -623,7 +626,7 @@ struct VGkSumTask {
         F::to_mont(fm[i], f);
         F::sub(omf[i], xm, fm[i]);
       }
-      gk_block_sum(acc, c.ring_m, omf, fm, n, k, (uint32_t)blk, nullptr);
+      gk_block_sum(acc, c.ring_of_row(b), omf, fm, n, k, (uint32_t)blk, nullptr);
     }
     st<8>(c.gk_part + (size_t)t * 8, acc);
   }
@@ -685,7 +688,7 @@ struct VGkTask {
     {
       const int k = gk_block_bits(n), nblk = 1 << (n - k);
       if (nblk == 1) {
-        gk_block_sum(total, c.ring_m, omf, fm, n, k, 0u, nullptr);
+        gk_block_sum(total, c.ring_of_row(b), omf, fm, n, k, 0u, nullptr);
       } else {               // block sums from VGkSumTask
         uint32_t v[8];
         zero_n<8>(total);

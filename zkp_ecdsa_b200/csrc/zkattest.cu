@@ -294,7 +294,7 @@ struct Lane {
   // verifier's chunk-wide aggregate check (zk_verify_agg.cuh: its fixed parts, and one pool per MSM as the two MSMs
   // run side by side)
   DevBuf w[51];
-  DevBuf in[2][9], out[2][3];
+  DevBuf in[2][10], out[2][3];
   DevBuf agg[8], agg_tom[5 + 2 * AGG_MAX_LEVELS], agg_nist[5 + 2 * AGG_MAX_LEVELS];
   std::string err;
   ~Lane() {
@@ -347,6 +347,16 @@ struct zka_params {
   FixedTable th;          // ProofGroup.h table
   uint8_t h_nist[65];
   uint8_t h_proof[WP];
+};
+
+// R rings on the device (zka_rings_create): ring r is reduced mod the proof-group order and padded to 2^n_r entries with
+// its own first entry, at entry ring_base[r] of ring_m
+struct zka_rings {
+  zka_ctx* ctx = nullptr;
+  uint32_t R = 0;
+  std::vector<uint32_t> size;              // N_r
+  std::vector<int> depth;                  // n_r = ceil(log2 N_r)
+  DevBuf ring_m, ring_base, ring_size;     // [total][8], [R], [R]
 };
 
 namespace {
@@ -617,17 +627,54 @@ void run_lanes(zka_ctx* ctx, int used, Fn fn) {
 }
 
 // ---- stage chains shared by the batched pipelines and the stand-alone sub-proof paths
-// The ring of a call on the device (RingPrepTask) and, for the prover, the GK Lagrange matrix (it depends only on n and
-// is cached per context).
+// The GK Lagrange matrix of the prover: it depends only on n and is cached per context
+void prep_lagrange(zka_ctx* ctx, Stream& st, int n) {
+  if (ctx->lag_n != n) {
+    launch(st, 1, GkLagrangeTask{ctx->lag.get<uint32_t>((size_t)n * n * 8), n});
+    ctx->lag_n = n;
+  }
+}
+// The ring of a call on the device (RingPrepTask) and, for the prover, the Lagrange matrix.
 const uint32_t* prep_ring(zka_ctx* ctx, Stream& st, const uint8_t* ring, uint32_t N, int n, bool lagrange) {
   const uint8_t* d_ring = stage_in(st, ctx->ring_in, ring, (size_t)N * 32);
   uint32_t* ring_m = ctx->ring_m.get<uint32_t>(((size_t)1 << n) * 8);
   launch(st, 1ll << n, RingPrepTask{d_ring, ring_m, (int)N});
-  if (lagrange && ctx->lag_n != n) {
-    launch(st, 1, GkLagrangeTask{ctx->lag.get<uint32_t>((size_t)n * n * 8), n});
-    ctx->lag_n = n;
-  }
+  if (lagrange) prep_lagrange(ctx, st, n);
   return ring_m;
+}
+
+// One pass of a ring-set call: consecutive rows whose rings share the depth n.  A chunk's launch geometry (B n GK threads,
+// 4n + 1 GK scalars per proof, the verify tape layout, the seeded spans) assumes one n, so prove_impl / verify_impl run
+// each such run of rows as one call of their own, with the set in place of the one ring.
+struct RingPass {
+  const zka_rings* set;
+  const uint32_t* ring_of;   // the pass's rows (host or device)
+  int n;
+};
+// Rows [start[k], start[k + 1]) of a ring-set call form run k, of depth depth[k]; nmax is the largest depth used.
+struct RingRuns {
+  std::vector<uint32_t> start;
+  std::vector<int> depth;
+  int nmax = 0;
+};
+// ring_of is read on the host (4 bytes per row, copied when it is device memory) and checked against the set
+int ring_runs(zka_ctx* ctx, const zka_rings* set, const uint32_t* ring_of, uint32_t B, RingRuns& rr) {
+  std::vector<uint32_t> h(B);
+  if (is_device_ptr(ring_of)) {
+    copy_d2h(ctx->st, h.data(), ring_of, (size_t)B * 4);
+    sync(ctx->st);
+  } else {
+    memcpy(h.data(), ring_of, (size_t)B * 4);
+  }
+  for (uint32_t b = 0; b < B; b++)
+    if (h[b] >= set->R) return fail(ctx, ZKA_E_ARG, "ring_of[i] >= number of rings in the set");
+  for (uint32_t b = 0; b < B; b++) {
+    const int n = set->depth[h[b]];
+    if (b == 0 || n != rr.depth.back()) { rr.start.push_back(b); rr.depth.push_back(n); }
+    rr.nmax = std::max(rr.nmax, n);
+  }
+  rr.start.push_back(B);
+  return 0;
 }
 
 int gk_blocks(int n) { return 1 << (n - gk_block_bits(n)); }   // ring blocks of the GK polynomial kernels
@@ -982,6 +1029,50 @@ int zka_params_create(zka_ctx* ctx, const uint8_t h_nist[65], const uint8_t h_pr
 
 void zka_params_destroy(zka_params* P) { delete P; }
 
+// R rings in one device handle: the keys cross once, and one RingSetPrepTask launch prepares every ring of the set
+int zka_rings_create(zka_ctx* ctx, uint32_t R, const uint32_t* sizes, const uint8_t* keys, zka_rings** out) {
+  if (!ctx || !sizes || !keys || !out) return ZKA_E_ARG;
+  *out = nullptr;
+  if (R == 0) return fail(ctx, ZKA_E_ARG, "a ring set holds at least one ring");
+  // every ring takes at least 2 padded entries
+  if (R > (1u << 23)) return fail(ctx, ZKA_E_ARG, "ring set exceeds 2^24 padded entries");
+  std::unique_ptr<zka_rings> set(new zka_rings());
+  set->ctx = ctx;
+  set->R = R;
+  std::vector<uint32_t> key_off(R), base(R);
+  uint64_t nkeys = 0, total = 0;
+  for (uint32_t r = 0; r < R; r++) {
+    const uint32_t N = sizes[r];
+    if (N < 2 || N > (1u << 20)) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
+    const int n = ceil_log2(N);
+    set->size.push_back(N);
+    set->depth.push_back(n);
+    key_off[r] = (uint32_t)nkeys;
+    base[r] = (uint32_t)total;
+    nkeys += N;
+    total += 1ull << n;
+    if (total > (1ull << 24)) return fail(ctx, ZKA_E_ARG, "ring set exceeds 2^24 padded entries");
+  }
+  return guarded(ctx, [&] {
+    Stream& st = ctx->st;
+    DevBuf kbuf, obuf;
+    const uint8_t* d_keys = stage_in(st, kbuf, keys, (size_t)nkeys * 32);
+    uint32_t* d_off = obuf.get<uint32_t>(R);
+    uint32_t* d_base = set->ring_base.get<uint32_t>(R);
+    uint32_t* d_size = set->ring_size.get<uint32_t>(R);
+    uint32_t* ring_m = set->ring_m.get<uint32_t>((size_t)total * 8);
+    copy_h2d(st, d_off, key_off.data(), (size_t)R * 4);
+    copy_h2d(st, d_base, base.data(), (size_t)R * 4);
+    copy_h2d(st, d_size, set->size.data(), (size_t)R * 4);
+    launch(st, (long long)total, RingSetPrepTask{d_keys, d_off, d_base, d_size, ring_m, (int)R});
+    sync(st);
+    *out = set.release();
+    return 0;
+  });
+}
+
+void zka_rings_destroy(zka_rings* set) { delete set; }
+
 size_t zka_proof_max_len(uint32_t ring_size, uint32_t sec_level) {
   return (size_t)proof_len((int)sec_level, ceil_log2(ring_size), (int)sec_level);
 }
@@ -1150,20 +1241,21 @@ int zka_key_to_int(zka_ctx* ctx, uint32_t count, const uint8_t* pk, uint8_t* x_o
 // msg_hash / sig / which / ring are unused, the rows hold the repetitions only.
 // seeds (B x 32, mode 0 only) instead of a tape: every lane expands its chunk's draws into its own tape buffer
 // (SeedProveTapeTask), the draws before the challenge first, the item and GK draws after the scan.
+// rp (mode 0 only) instead of (ring, N): one pass of a ring-set call, every row against its own ring of the set.
 static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
                       const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* tape,
                       size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out,
                       int32_t* status, int mode, const uint8_t* base, const uint8_t* s_in, const uint8_t* q_in,
-                      const uint8_t* seeds = nullptr) {
+                      const uint8_t* seeds = nullptr, const RingPass* rp = nullptr) {
   if (!ctx || !P || !pk || (!tape && !seeds) || !proofs || !proof_len_out || !status) return ZKA_E_ARG;
-  if (mode == 0 && (!msg_hash || !sig || !which || !ring)) return ZKA_E_ARG;
+  if (mode == 0 && (!msg_hash || !sig || !which || (!ring && !rp))) return ZKA_E_ARG;
   if (mode == 1 && (!base || !s_in)) return ZKA_E_ARG;
   if (B == 0) return 0;
   // N = 1 makes hashPoints([]) throw in the reference (group.ts:223 reduce of an empty array)
-  if (mode == 0 && (N < 2 || N > (1u << 20))) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
+  if (mode == 0 && !rp && (N < 2 || N > (1u << 20))) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
   const int S = (int)P->sec_level;
-  const int n = mode == 0 ? ceil_log2(N) : 0;
-  if (proof_stride < (mode == 0 ? zka_proof_max_len(N, S) : (size_t)S * REP0_LEN)) return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len");
+  const int n = rp ? rp->n : mode == 0 ? ceil_log2(N) : 0;
+  if (proof_stride < (mode == 0 ? (size_t)proof_len(S, n, S) : (size_t)S * REP0_LEN)) return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len");
   const bool seeded = seeds != nullptr;
   if (!seeded && tape_stride < (size_t)32 * (mode == 0 ? prove_draws(0, n, S) : draws_before_items(S))) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
   // seeded: the library's tape rows hold every draw a proof can read (a multiple of 32 bytes, so 16-byte aligned rows)
@@ -1171,7 +1263,11 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
   return guarded(ctx, [&] {
     // ring + Lagrange matrix: once per call, on lane 0, finished before the lanes start
     const uint32_t* ring_m = nullptr;
-    if (mode == 0) {
+    if (rp) {
+      ring_m = (const uint32_t*)rp->set->ring_m.p;
+      prep_lagrange(ctx, ctx->st, n);
+      sync(ctx->st);
+    } else if (mode == 0) {
       ring_m = prep_ring(ctx, ctx->st, ring, N, n, true);
       sync(ctx->st);
     }
@@ -1194,7 +1290,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
     auto run_lane = [&](int li) {
       Lane& ln = ctx->lane(li);
       Stream& st = ln.st;
-      struct ChunkIn { const uint8_t *msg_hash, *sig, *pk, *tape, *base, *s_in, *q_in, *seeds; const uint32_t* which; } cin[2];
+      struct ChunkIn { const uint8_t *msg_hash, *sig, *pk, *tape, *base, *s_in, *q_in, *seeds; const uint32_t *which, *ring_of; } cin[2];
       auto issue_inputs = [&](uint32_t k, int slot) {
         const uint32_t b0 = off[k];
         const size_t Bc = off[k + 1] - b0;
@@ -1207,6 +1303,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         cin[slot].sig = rows(sig, 64);
         cin[slot].pk = rows(pk, 65);
         cin[slot].which = rows(which, 1);
+        cin[slot].ring_of = rows(rp ? rp->ring_of : nullptr, 1);
         cin[slot].base = rows(base, 65);
         cin[slot].s_in = rows(s_in, 32);
         cin[slot].q_in = rows(q_in, 65);
@@ -1256,6 +1353,11 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         c.tape_stride = seeded ? (size_t)32 * seed_draws : is_device_ptr(tape) ? tape_stride : dev_tape_stride;
         c.tape_draws = seeded ? (uint32_t)seed_draws : (uint32_t)(tape_stride / 32);
         c.ring_m = ring_m;
+        if (rp) {
+          c.ring_of = cin[slot].ring_of;
+          c.ring_base = (const uint32_t*)rp->set->ring_base.p;
+          c.ring_size = (const uint32_t*)rp->set->ring_size.p;
+        }
         const size_t S1 = (size_t)S + 1;
         const size_t nA = (size_t)Bc * S1;
         const size_t n1 = (size_t)Bc * (2 + 2 * S);
@@ -1320,9 +1422,9 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         launch(st, (long long)Bc * ((KEY_CAP + 15) / 16), P256RowsBlockTask{c.rpows, c.rrows, KEY_W_MIN, c.tab_count, c.tab_count + 1});
         {
           const long long np = (long long)Bc * KEY_CAP;
-          // points per thread from the EXPECTED table volume (at most min(N, Bc) distinct keys when every key is a ring
-          // member); the grid still covers the worst case
-          const uint32_t kest = std::min<uint32_t>(N, (uint32_t)Bc);
+          // points per thread from the EXPECTED table volume (at most min(N, Bc) distinct keys when every key is a member
+          // of the one ring; up to Bc with a ring set); the grid still covers the worst case
+          const uint32_t kest = rp ? (uint32_t)Bc : std::min<uint32_t>(N, (uint32_t)Bc);
           const int west = key_window_bits(kest, (uint32_t)Bc, (uint32_t)S + 2);
           const int ch = norm_chunk_for((long long)kest * fb_windows(west) * fb_entries(west), 5);
           launch(st, (np + ch - 1) / ch, P256NormTask{c.rrows, c.rtab, nullptr, nullptr, (int)np, ch, c.tab_count, 0, c.tab_count + 1});
@@ -1397,7 +1499,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         launch(st, (long long)Bc * FIN_PARTS, FinalizeTask{c});
         // --- results: on the output stream, behind this chunk's last kernel
         ev_record(ln.ev_done[slot], st);
-        if (ctx->progress && k_this < ctx->progress_cap) notify_progress(st, ctx->progress + k_this);
+        if (ctx->progress && !rp && k_this < ctx->progress_cap) notify_progress(st, ctx->progress + k_this);
         if (!po.dev || !lo.dev || !so.dev) {
           Stream& co = ln.cs_out;
           ev_wait(co, ln.ev_done[slot]);
@@ -1441,6 +1543,51 @@ int zka_prove_batch_seeded(zka_ctx* ctx, const zka_params* P, uint32_t B, const 
   if (!seeds) return ZKA_E_ARG;
   return prove_impl(ctx, P, B, msg_hash, sig, pk, which, ring, N, nullptr, 0, proofs, proof_stride, proof_len_out, status, 0,
                     nullptr, nullptr, nullptr, seeds);
+}
+
+// Ring-set prover: every maximal run of consecutive rows whose rings share a depth is one prove_impl pass on offset
+// pointers (tape or seeds, one of them null)
+static int prove_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* set, const uint32_t* ring_of, uint32_t B,
+                       const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which, const uint8_t* tape,
+                       size_t tape_stride, const uint8_t* seeds, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out,
+                       int32_t* status) {
+  if (!ctx || !P || !set || !ring_of || !msg_hash || !sig || !pk || !which || (!tape && !seeds) || !proofs || !proof_len_out || !status)
+    return ZKA_E_ARG;
+  if (set->ctx != ctx) return fail(ctx, ZKA_E_ARG, "ring set of another context");
+  if (B == 0) return 0;
+  return guarded(ctx, [&] {
+    RingRuns rr;
+    if (const int rc = ring_runs(ctx, set, ring_of, B, rr)) return rc;
+    const int S = (int)P->sec_level;
+    if (proof_stride < (size_t)proof_len(S, rr.nmax, S)) return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len");
+    if (tape && tape_stride < (size_t)32 * prove_draws(0, rr.nmax, S)) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
+    for (size_t k = 0; k + 1 < rr.start.size(); k++) {
+      const uint32_t r0 = rr.start[k], rows = rr.start[k + 1] - r0;
+      const RingPass rp{set, ring_of + r0, rr.depth[k]};
+      const int rc = prove_impl(ctx, P, rows, msg_hash + (size_t)r0 * 32, sig + (size_t)r0 * 64, pk + (size_t)r0 * 65, which + r0,
+                                nullptr, 0, tape ? tape + (size_t)r0 * tape_stride : nullptr, tape_stride,
+                                proofs + (size_t)r0 * proof_stride, proof_stride, proof_len_out + r0, status + r0, 0, nullptr, nullptr,
+                                nullptr, seeds ? seeds + (size_t)r0 * 32 : nullptr, &rp);
+      if (rc) return rc;
+    }
+    return 0;
+  });
+}
+
+int zka_prove_batch_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
+                          const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which, const uint8_t* tape,
+                          size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status) {
+  if (!tape) return ZKA_E_ARG;
+  return prove_rings(ctx, P, rings, ring_of, B, msg_hash, sig, pk, which, tape, tape_stride, nullptr, proofs, proof_stride,
+                     proof_len_out, status);
+}
+
+int zka_prove_batch_rings_seeded(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
+                                 const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which,
+                                 const uint8_t* seeds, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status) {
+  if (!seeds) return ZKA_E_ARG;
+  return prove_rings(ctx, P, rings, ring_of, B, msg_hash, sig, pk, which, nullptr, 0, seeds, proofs, proof_stride, proof_len_out,
+                     status);
 }
 
 // The tape a seed stands for (the rule of zk_seed.cuh): kind 0 all prove_draws(S, n, S) prover draws, kind 1 the verify
@@ -1680,7 +1827,7 @@ int zka_verify_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_
 static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                        uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                        const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples, int mode,
-                       const uint8_t* q_ext, const uint8_t* seeds = nullptr);
+                       const uint8_t* q_ext, const uint8_t* seeds = nullptr, const RingPass* rp = nullptr);
 
 int zka_verify_batch_ex(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                         uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
@@ -1696,28 +1843,72 @@ int zka_verify_batch_seeded(zka_ctx* ctx, const zka_params* P, uint32_t B, const
   return verify_impl(ctx, P, B, msg_hash, ring, N, proofs, proof_stride, proof_len, nullptr, 0, ok, status, samples, 0, nullptr, seeds);
 }
 
+// Ring-set verifier: one verify_impl pass per maximal run of rows whose rings share a depth (tape or seeds, one of them null)
+static int verify_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* set, const uint32_t* ring_of, uint32_t B,
+                        const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                        const uint8_t* tape, size_t tape_stride, const uint8_t* seeds, uint32_t samples, uint8_t* ok, int32_t* status) {
+  if (!ctx || !P || !set || !ring_of || !msg_hash || !proofs || !proof_len || (!tape && !seeds) || !ok || !status) return ZKA_E_ARG;
+  if (set->ctx != ctx) return fail(ctx, ZKA_E_ARG, "ring set of another context");
+  if (B == 0) return 0;
+  return guarded(ctx, [&] {
+    RingRuns rr;
+    if (const int rc = ring_runs(ctx, set, ring_of, B, rr)) return rc;
+    const int S = (int)P->sec_level, K = (int)samples;
+    if (K < 1) return fail(ctx, ZKA_E_ARG, "samples must be >= 1");
+    if (S < K) return fail(ctx, ZKA_E_ARG, "security level not achieved");
+    if (tape && tape_stride < verify_tape_len(rr.nmax, S, K)) return fail(ctx, ZKA_E_ARG, "tape_stride < zka_verify_tape_len");
+    for (size_t k = 0; k + 1 < rr.start.size(); k++) {
+      const uint32_t r0 = rr.start[k], rows = rr.start[k + 1] - r0;
+      const RingPass rp{set, ring_of + r0, rr.depth[k]};
+      const int rc = verify_impl(ctx, P, rows, msg_hash + (size_t)r0 * 32, nullptr, 0, proofs + (size_t)r0 * proof_stride, proof_stride,
+                                 proof_len + r0, tape ? tape + (size_t)r0 * tape_stride : nullptr, tape_stride, ok + r0, status + r0,
+                                 samples, 0, nullptr, seeds ? seeds + (size_t)r0 * 32 : nullptr, &rp);
+      if (rc) return rc;
+    }
+    return 0;
+  });
+}
+
+int zka_verify_batch_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
+                           const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                           const uint8_t* tape, size_t tape_stride, uint32_t samples, uint8_t* ok, int32_t* status) {
+  if (!tape) return ZKA_E_ARG;
+  return verify_rings(ctx, P, rings, ring_of, B, msg_hash, proofs, proof_stride, proof_len, tape, tape_stride, nullptr, samples, ok,
+                      status);
+}
+
+int zka_verify_batch_rings_seeded(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
+                                  const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                                  const uint8_t* seeds, uint32_t samples, uint8_t* ok, int32_t* status) {
+  if (!seeds) return ZKA_E_ARG;
+  return verify_rings(ctx, P, rings, ring_of, B, msg_hash, proofs, proof_stride, proof_len, nullptr, 0, seeds, samples, ok, status);
+}
+
 // mode 0: verifySignatureList; mode 1: verifyExp alone on assembled rows (msg_hash / ring unused, Q from q_ext)
 // seeds (B x 32, mode 0 only) instead of a tape: SeedVerifyTapeTask expands each chunk's verify layout on the lane's stream
+// rp (mode 0 only) instead of (ring, N): one pass of a ring-set call, every row against its own ring of the set
 static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                        uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                        const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples, int mode,
-                       const uint8_t* q_ext, const uint8_t* seeds) {
+                       const uint8_t* q_ext, const uint8_t* seeds, const RingPass* rp) {
   if (!ctx || !P || !proofs || !proof_len || (!tape && !seeds) || !ok || !status) return ZKA_E_ARG;
   if (B == 0) return 0;
-  if (N < 2 || N > (1u << 20)) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
+  if (!rp && (N < 2 || N > (1u << 20))) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
   const int S = (int)P->sec_level;
   const int K = (int)samples;
   if (K < 1) return fail(ctx, ZKA_E_ARG, "samples must be >= 1");
   // verifyExp throws 'security level not achieved' when secparam > pi.length (exp.ts:243-245)
   if (S < K) return fail(ctx, ZKA_E_ARG, "security level not achieved");
-  const int n = ceil_log2(N);
+  const int n = rp ? rp->n : ceil_log2(N);
   const bool seeded = seeds != nullptr;
   if (!seeded && tape_stride < (mode == 1 ? (size_t)V_IDX_PAD + (size_t)32 * 25 * K : verify_tape_len(n, S, K)))
     return fail(ctx, ZKA_E_ARG, "tape_stride < zka_verify_tape_len");
   const size_t seed_stride = verify_tape_len(n, S, K);   // a multiple of 16
   return guarded(ctx, [&] {
     const uint32_t* ring_m = nullptr;
-    if (mode == 0) {
+    if (rp) {
+      ring_m = (const uint32_t*)rp->set->ring_m.p;
+    } else if (mode == 0) {
       ring_m = prep_ring(ctx, ctx->st, ring, N, n, false);
       sync(ctx->st);
     }
@@ -1737,7 +1928,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
     // lane's stream; the copies of one lane overlap the kernels of the others
     // the inputs of a lane's NEXT chunk travel on the copy-in stream (second set of staging buffers) while the current
     // chunk computes; a chunk's kernels wait for its event only
-    struct VIn { const uint8_t* msg; const uint8_t* proofs; const uint32_t* plen; const uint8_t* tape; const uint8_t* seeds; };
+    struct VIn { const uint8_t* msg; const uint8_t* proofs; const uint32_t* plen; const uint8_t* tape; const uint8_t* seeds; const uint32_t* ring_of; };
     auto stage_chunk = [&](Lane& ln, int slot, uint32_t kk) {
       // ONE copy-in stream for all lanes of the call: the chunks' inputs cross PCIe in the order they were queued, each at
       // full bandwidth (with a copy stream per lane the first chunks and the prefetched ones were all in flight at once).
@@ -1765,6 +1956,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       if (seeded) v.tape = in.next().get<uint8_t>(Bc * seed_stride);   // filled by SeedVerifyTapeTask
       else v.tape = stage_in(ci, in.next(), tape + (size_t)b0 * tape_stride, Bc * tape_stride);
       v.seeds = stage_in(ci, in.next(), seeded ? seeds + (size_t)b0 * 32 : nullptr, Bc * 32);
+      v.ring_of = stage_in(ci, in.next(), rp ? rp->ring_of + b0 : nullptr, Bc);
       ev_record(ln.ev_small[slot], ci);
       return v;
     };
@@ -1798,6 +1990,10 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       c.tape = cur.tape;
       c.tape_stride = seeded ? seed_stride : tape_stride;
       c.ring_m = ring_m;
+      if (rp) {
+        c.ring_of = cur.ring_of;
+        c.ring_base = (const uint32_t*)rp->set->ring_base.p;
+      }
       if (seeded) {
         const SeedVerifyTapeTask vt{cur.seeds, const_cast<uint8_t*>(cur.tape), seed_stride, n, S, K};
         launch(st, (long long)Bc * vt.slots(), vt);

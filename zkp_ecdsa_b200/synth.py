@@ -146,6 +146,69 @@ class Workload:
         return [int.from_bytes(self.ring[i].tobytes(), 'big') for i in range(self.N)]
 
 
+def _p256_pub(k: int) -> bytes:
+    """k*G as 65 raw bytes (OpenSSL does the scalar multiplication)."""
+    from cryptography.hazmat.primitives import serialization
+    from cryptography.hazmat.primitives.asymmetric import ec
+    return ec.derive_private_key(k, ec.SECP256R1()).public_key().public_bytes(
+        serialization.Encoding.X962, serialization.PublicFormat.UncompressedPoint)
+
+
+class RingsWorkload:
+    """B signing instances over a ring set: row b proves membership in ring ring_of[b] of R rings of the given sizes.
+
+    Ring r holds min(rows of r, sizes[r]) signers of its own at DRBG-chosen slots (a partial Fisher-Yates shuffle); the
+    rows of ring r cycle through them, so a ring with one row has a signer of its own.  Filler entries are arbitrary
+    256-bit values.  `keys` is the rings' entries concatenated in ring order (the layout of zka_rings_create)."""
+
+    def __init__(self, B: int, sizes, ring_of, seed: int = 0):
+        self.B, self.seed = B, seed
+        self.sizes = [int(s) for s in sizes]
+        self.ring_of = np.asarray(ring_of, np.uint32).reshape(B).copy()
+        R = len(self.sizes)
+        assert R >= 1 and int(self.ring_of.max(initial=0)) < R
+        rows_of = [np.flatnonzero(self.ring_of == r) for r in range(R)]
+        d = Drbg(seed, 'rings-signers')
+        dn = Drbg(seed, 'rings-nonces')
+        dr = Drbg(seed, 'rings-fill')
+        self.rings = []
+        signer = {}                     # (ring, j) -> (secret key, public key, slot)
+        for r, N in enumerate(self.sizes):
+            ring = [dr.bytes(32) for _ in range(N)]
+            slots = list(range(N))
+            for j in range(min(len(rows_of[r]), N)):
+                i = j + int.from_bytes(d.bytes(8), 'big') % (N - j)   # (below() is for 256-bit moduli)
+                slots[j], slots[i] = slots[i], slots[j]
+                sk = d.below(P256_N - 1) + 1
+                pk = _p256_pub(sk)
+                ring[slots[j]] = pk[1:33]
+                signer[r, j] = (sk, pk, slots[j])
+            self.rings.append(np.frombuffer(b''.join(ring), np.uint8).reshape(N, 32).copy())
+        self.keys = np.concatenate(self.rings, axis=0)
+        self.msg_hash = np.zeros((B, 32), np.uint8)
+        self.sig = np.zeros((B, 64), np.uint8)
+        self.pk = np.zeros((B, 65), np.uint8)
+        self.which = np.zeros(B, np.uint32)
+        for r in range(R):
+            ns = min(len(rows_of[r]), self.sizes[r])
+            for j, b in enumerate(rows_of[r]):
+                sk, pk, slot = signer[r, j % ns]
+                digest = hashlib.sha256(b'zkattest-rings-%d' % b).digest()
+                while True:
+                    k = dn.below(P256_N - 1) + 1
+                    rr = int.from_bytes(_p256_pub(k)[1:33], 'big') % P256_N
+                    s = pow(k, -1, P256_N) * (int.from_bytes(digest, 'big') + rr * sk) % P256_N
+                    if rr and s:
+                        break
+                self.msg_hash[b] = np.frombuffer(digest, np.uint8)
+                self.sig[b] = np.frombuffer(rr.to_bytes(32, 'big') + s.to_bytes(32, 'big'), np.uint8)
+                self.pk[b] = np.frombuffer(pk, np.uint8)
+                self.which[b] = slot
+
+    def ring_ints(self, r: int):
+        return [int.from_bytes(v.tobytes(), 'big') for v in self.rings[r]]
+
+
 def params_rnd(seed: int = 0) -> bytes:
     d = Drbg(seed, 'params')
     return d.below(P256_N).to_bytes(32, 'big') + d.below(P256_P).to_bytes(32, 'big')
