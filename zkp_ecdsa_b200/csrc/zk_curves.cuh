@@ -128,7 +128,8 @@ enum { TOM_SQRTA = 0, TOM_INVSQRTA = 1, TOM_D1 = 2, TOM_GX1 = 3, TOM_GY = 4, TOM
 // ---- second image curve E2: -w^2 + v^2 = 1 + d2 w^2 v^2, (w, v) = (sqrt(-d1) x', 1/y) -------------
 // Used ONLY by the prover's fixed-base commitment kernel (all its points lie in the prime-order
 // subgroup generated by g, where the a = -1 formulas have no exceptional cases; gen_consts.py).
-// Table entry: (v - w, v + w, 2 d2 w v).  Mixed addition "madd-2008-hwcd-3": 7M.
+// Table entry: (v - w, v + w, 2 d2 w v).  Mixed addition "madd-2008-hwcd-3": 7M; a walk's first addition (to the
+// identity) is 1M (tom2_from_pre) and its last one, when only the normaliser reads the point, 3M (tom2_madd_end).
 // Field with the 258-bit multiplier INLINED at every use (no call, no argument marshalling): for loop bodies
 // that contain one mixed addition (7-8 products, ~40 KB of code) and are not unrolled.
 struct TompInl : Tomp {
@@ -169,6 +170,44 @@ ZK_HD void tom2_madd(TomPt& r, const TomPt& p, const TomPre& q) {   // q.x = v-w
   F::mul(r.y, G, H);
   if (kNeedT) F::mul(r.t, E, H);
   F::mul(r.z, Fv, G);
+}
+// First point of a walk that starts at the identity: tom2_madd of (0 : 1 : 0 : 1) and q has E = 2w, F = G = 2, H = 2v,
+// so the point is (2E : 2H : E H : 4).  1M instead of 7M.  q.x, q.y < p (table entries and their swap), so
+// E = q.y + p - q.x < 2p and X < 4p stay inside the bound of tom2_madd's lazy subtraction.
+template <class F = Tomp>
+ZK_HD void tom2_from_pre(TomPt& r, const TomPre& q) {
+  uint32_t E[9], H[9];
+#pragma unroll
+  for (int i = 0; i < 9; i++) E[i] = FpTom::p(i);
+  add_n<9>(E, E, q.y);
+  sub_n<9>(E, E, q.x);
+  F::add(H, q.y, q.x);
+  F::mul(r.t, E, H);
+  F::add(r.x, E, E);
+  F::add(r.y, H, H);
+  F::set_one(r.z);
+  F::add(r.z, r.z, r.z);
+  F::add(r.z, r.z, r.z);
+}
+// Last addition of a walk whose point only goes to TomNormTask{e2 = 1}: the E, F, G, H of tom2_madd, of which the
+// point is (E F : G H : E H : F G).  The normaliser needs x' sqrt(-d1) = E / G and y = F / H only, so the four
+// products X, Y, T, Z are left out: 3M instead of 7M.  Bounds: E < 10p, F < 12p, G < 6p, H < 4p.
+struct TomEfgh {
+  uint32_t e[9], f[9], g[9], h[9];
+};
+template <class F = Tomp>
+ZK_HD void tom2_madd_end(TomEfgh& r, const TomPt& p, const TomPre& q) {
+  uint32_t A[9], B[9], C[9], D[9];
+  F::sub(A, p.y, p.x);
+  F::mul(A, A, q.x);
+  F::add(B, p.y, p.x);
+  F::mul(B, B, q.y);
+  F::mul(C, p.t, q.k);
+  F::add(D, p.z, p.z);
+  F::sub(r.e, B, A);
+  F::sub(r.f, D, C);
+  F::add(r.g, D, C);
+  F::add(r.h, B, A);
 }
 
 ZK_HD void tom_set_identity(TomPt& p) {

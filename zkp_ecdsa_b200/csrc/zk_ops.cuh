@@ -56,10 +56,12 @@ enum : int {
   P256_AFF_WORDS = 16,
 #if defined(ZKA_PG_WAR256)
   TOM_PROJ_WORDS = 24,   // war256 build: homogeneous (X, Y, Z), 8 limbs each
+  TOM_E2_WORDS = 24,     // a commitment for the normaliser: (X, Y, Z) as well
   TOM_AFF_WORDS = 16,    // affine (x, y), Montgomery
   TOM_PRE_WORDS = 16,    // table entry / parsed point = affine (x, y): one 64-byte half line
 #else
   TOM_PROJ_WORDS = 28,   // X, Y, Z (T is not needed after the last addition) + 1 pad word: 7 x 16 bytes
+  TOM_E2_WORDS = 36,     // a commitment for the normaliser: E, F, G, H of its last addition (tom2_madd_end), 9 x 16 bytes
   TOM_AFF_WORDS = 18,    // x', y on the a'=1 image curve, Montgomery
   TOM_PRE_WORDS = 32,    // x', y, k = d' x' y + 5 pad words: one 128-byte line per entry
 #endif
@@ -106,6 +108,34 @@ ZK_HD void tom_ld_xyz(uint32_t* x, uint32_t* y, uint32_t* z, const uint32_t* m) 
 #endif
 #pragma unroll
   for (int i = 0; i < 9; i++) { x[i] = w[i]; y[i] = w[9 + i]; z[i] = w[18 + i]; }
+}
+// staged E2 commitments for the normaliser (E, F, G, H at words 0, 9, 18, 27 of a 144-byte slot): nine 16-byte transactions
+ZK_HD void tom_st_efgh(uint32_t* m, const TomEfgh& p) {
+  uint32_t w[36];
+#pragma unroll
+  for (int i = 0; i < 9; i++) { w[i] = p.e[i]; w[9 + i] = p.f[i]; w[18 + i] = p.g[i]; w[27 + i] = p.h[i]; }
+#if defined(__CUDA_ARCH__)
+  uint4* v = reinterpret_cast<uint4*>(m);
+#pragma unroll
+  for (int i = 0; i < 9; i++) v[i] = make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
+#else
+  for (int i = 0; i < 36; i++) m[i] = w[i];
+#endif
+}
+ZK_HD void tom_ld_efgh(uint32_t* e, uint32_t* f, uint32_t* g, uint32_t* h, const uint32_t* m) {
+  uint32_t w[36];
+#if defined(__CUDA_ARCH__)
+  const uint4* v = reinterpret_cast<const uint4*>(m);
+#pragma unroll
+  for (int i = 0; i < 9; i++) {
+    const uint4 u = v[i];
+    w[4 * i] = u.x; w[4 * i + 1] = u.y; w[4 * i + 2] = u.z; w[4 * i + 3] = u.w;
+  }
+#else
+  for (int i = 0; i < 36; i++) w[i] = m[i];
+#endif
+#pragma unroll
+  for (int i = 0; i < 9; i++) { e[i] = w[i]; f[i] = w[9 + i]; g[i] = w[18 + i]; h[i] = w[27 + i]; }
 }
 
 // negate a table entry of the a = -1 image curve: -(w, v) = (-w, v) swaps v - w and v + w and negates 2 d2 w v
@@ -486,15 +516,17 @@ struct TomTabE2Task {
 
 // Batched normalisation of tomEdwards256 points -> E1 affine (x', y) Montgomery (+ optional 67-byte
 // reference encoding of (x = x'/sqrt(a), y)).  e2 == 0: input is E1 projective (X:Y:Z);
-// e2 == 1: input is an E2 point (W:V:Z) from the commitment kernel: x' = W / (Z sqrt(-d1)), y = Z / V.
+// e2 == 1: input is (E, F, G, H) of the last addition of a commitment walk (tom2_madd_end):
+// x' = E / (G sqrt(-d1)) = E H / (G H sqrt(-d1)), y = F / H = F G / (G H).
 struct TomNormTask {
-  const uint32_t* proj;  // [count][27]
+  const uint32_t* proj;  // [count][stride]: (X, Y, Z) or (E, F, G, H)
   uint32_t* aff;         // [count][18] or null
   uint8_t* bytes;        // [count][BSTRIDE] or null
   int count;
   int chunk;             // points per thread (<= NORM_CHUNK_MAX)
   int e2;
   int aff_mod, aff_lim;  // the E1 affine pair is produced only for points with (index % aff_mod) < aff_lim
+  int stride;            // words per input slot: TOM_E2_WORDS or TOM_PROJ_WORDS (an (X, Y, Z) slot may be wider)
   ZK_HD static void canon2p(uint32_t* r) {   // value < 4p -> [0, p)
     uint32_t t[9], p2[9];
 #pragma unroll
@@ -511,63 +543,57 @@ struct TomNormTask {
     if (n > chunk) n = chunk;
     if (n <= 0) return;
     uint32_t pre[NORM_CHUNK_MAX][9];
-    uint32_t acc[9], z[9], v[9], den[9];
+    uint32_t acc[9], z[9], h[9], den[9];
     F::set_one(acc);
     for (int k = 0; k < n; k++) {
-      const uint32_t* src = proj + (size_t)(lo + k) * TOM_PROJ_WORDS;
-      uint32_t xx[9];
-      tom_ld_xyz(xx, v, z, src);
-      if (e2) F::mul(den, z, v); else copy_n<9>(den, z);
-      F::mul(acc, acc, den);   // Z != 0 (complete curve); V != 0 inside the prime-order subgroup
+      const uint32_t* src = proj + (size_t)(lo + k) * stride;
+      uint32_t xx[9], yy[9];
+      if (e2) {
+        tom_ld_efgh(xx, yy, z, h, src);
+        F::mul(den, z, h);       // G H
+      } else {
+        tom_ld_xyz(xx, yy, den, src);
+      }
+      F::mul(acc, acc, den);   // Z != 0 (complete curve); G, H != 0 inside the prime-order subgroup
       copy_n<9>(pre[k], acc);
     }
-    uint32_t inv[9], isa[9], is2[9], isd[9], one_plain[9];
+    uint32_t inv[9], cxk[9], is2[9], one_plain[9];
     F::inv(inv, acc);
-    tom_const(isa, TOM_INVSQRTA);
+    tom_const(cxk, e2 ? TOM_INVSQRTND : TOM_INVSQRTA);   // 1 / sqrt(-d) or 1 / sqrt(a): x of the encoding
     tom_const(is2, TOM_INVSQRTND1);
-    tom_const(isd, TOM_INVSQRTND);
     zero_n<9>(one_plain);
     one_plain[0] = 1;
     for (int k = n - 1; k >= 0; k--) {
-      const uint32_t* src = proj + (size_t)(lo + k) * TOM_PROJ_WORDS;
+      const uint32_t* src = proj + (size_t)(lo + k) * stride;
       uint32_t X[9], Y[9], di[9];
-      tom_ld_xyz(X, Y, z, src);
-      if (e2) F::mul(den, z, Y); else copy_n<9>(den, z);
+      if (e2) {                         // over den = G H:  x' sqrt(-d1) = E H / den,  y = F G / den
+        tom_ld_efgh(X, Y, z, h, src);
+        F::mul(den, z, h);
+        F::mul(X, X, h);
+        F::mul(Y, Y, z);
+      } else {
+        tom_ld_xyz(X, Y, den, src);
+      }
       if (k > 0) F::mul(di, inv, pre[k - 1]); else copy_n<9>(di, inv);   // Montgomery residue of 1/den
       F::mul(inv, inv, den);
       if (bytes) {
         // D = 1/den as a PLAIN integer: a Montgomery product with it leaves Montgomery form, so the
         // reference coordinates come out without separate from_mont multiplications
+        // e2: x = E H D / sqrt(-d),  y = F G D;  E1: x = X D / sqrt(a),  y = Y D
         uint32_t Dp[9], cx[9], cy[9];
         F::mul(Dp, di, one_plain);
-        if (e2) {                       // x = W V D / sqrt(-d),  y = Z^2 D
-          F::mul(cx, X, Y);
-          F::mul(cx, cx, isd);
-          F::mul(cx, cx, Dp);
-          F::sqr(cy, z);
-          F::mul(cy, cy, Dp);
-        } else {                        // x = X D / sqrt(a),  y = Y D
-          F::mul(cx, X, isa);
-          F::mul(cx, cx, Dp);
-          F::mul(cy, Y, Dp);
-        }
+        F::mul(cx, X, cxk);
+        F::mul(cx, cx, Dp);
+        F::mul(cy, Y, Dp);
         canon2p(cx);
         canon2p(cy);
         store_point_words<9, 33>(bytes + (size_t)(lo + k) * BSTRIDE, 0x04u, cx, cy);
       }
       if (aff && ((lo + k) % aff_mod) < aff_lim) {
         uint32_t x[9], y[9];
-        if (e2) {
-          uint32_t zi[9], vi[9];
-          F::mul(zi, di, Y);       // 1/Z
-          F::mul(vi, di, z);       // 1/V
-          F::mul(x, X, zi);
-          F::mul(x, x, is2);       // x' = W / (Z sqrt(-d1))
-          F::mul(y, z, vi);        // y = Z / V
-        } else {
-          F::mul(x, X, di);
-          F::mul(y, Y, di);
-        }
+        F::mul(x, X, di);
+        if (e2) F::mul(x, x, is2);     // x' = E / (G sqrt(-d1))
+        F::mul(y, Y, di);
         uint32_t* a = aff + (size_t)(lo + k) * TOM_AFF_WORDS;
         st<9>(a, x);
         st<9>(a + 9, y);
@@ -576,40 +602,57 @@ struct TomNormTask {
   }
 };
 
+// entry |d| of window j of a signed-digit E2 table [nwin][ne][32], negated for a negative digit
+ZK_HD void tom2_ld_entry(TomPre& q, const uint32_t* tab, int j, size_t ne, uint32_t d, bool neg) {
+  tom_ld_pre(q, tab + ((size_t)j * ne + d) * TOM_PRE_WORDS);
+  tom2_pre_neg(q, neg);
+}
+
 // Pedersen commitment in the proof group:  C = v*g + r*h   (pedersen.ts:53-58, gk.ts:88-92),
-// both bases fixed => two positional tables, 2*nwin mixed additions, no doublings.
+// both bases fixed => two positional tables, 2*nwin mixed additions, no doublings.  The walk starts at the entry of
+// v's first window (tom2_from_pre, 1M) and, for the normaliser, ends with tom2_madd_end (3M): 1 + (2 nwin - 2) * 7 + 3
+// products instead of 2 nwin * 7.  A zero digit selects entry 0, the identity.
 struct TomCommitTask {
   const uint32_t* jv;    // [count][8] canonical value scalars (mod tom.order)
   const uint32_t* jr;    // [count][8] canonical blinders
   const uint32_t* gtab;  // [nwin][2^w][32]
   const uint32_t* htab;
-  uint32_t* proj;        // [count][27]  E2 point (W:V:Z) -> TomNormTask{e2 = 1}
+  uint32_t* proj;        // [count][TOM_E2_WORDS] (E, F, G, H) -> TomNormTask{e2 = 1}; xyz: [count][TOM_PROJ_WORDS]
   int w, nwin;
+  int xyz = 0;           // 1: a full last addition, E2 (W : V : Z) for readers other than the normaliser (pg_fixed_to_msm)
   ZK_HD void operator()(int t) const {
     uint32_t v[8], r[8];
     ld<8>(v, jv + (size_t)t * 8);
     ld<8>(r, jr + (size_t)t * 8);
-    TomPt acc;
-    tom_set_identity(acc);
     const size_t ne = (size_t)fb_entries(w);
     uint32_t cv = 0, cr = 0;
-    for (int j = 0; j < nwin; j++) {
-      TomPre q;
-      bool nv, nr;
-      const uint32_t dv = signed_digit(v, j, w, cv, nv), dr = signed_digit(r, j, w, cr, nr);
-      tom_ld_pre(q, gtab + ((size_t)j * ne + dv) * TOM_PRE_WORDS);
-      tom2_pre_neg(q, nv);
+    bool nv, nr;
+    TomPre q;
+    uint32_t dv = signed_digit(v, 0, w, cv, nv);
+    tom2_ld_entry(q, gtab, 0, ne, dv, nv);
+    TomPt acc;
+    tom2_from_pre(acc, q);
+    for (int j = 0;; j++) {
+      const uint32_t dr = signed_digit(r, j, w, cr, nr);
+      tom2_ld_entry(q, htab, j, ne, dr, nr);
+      if (j == nwin - 1) break;
       tom2_madd<true>(acc, acc, q);     // a = -1 image curve E2: 7M per lookup
-      tom_ld_pre(q, htab + ((size_t)j * ne + dr) * TOM_PRE_WORDS);
-      tom2_pre_neg(q, nr);
+      dv = signed_digit(v, j + 1, w, cv, nv);
+      tom2_ld_entry(q, gtab, j + 1, ne, dv, nv);
       tom2_madd<true>(acc, acc, q);
     }
-    uint32_t* o = proj + (size_t)t * TOM_PROJ_WORDS;
-    tom_st_xyz(o, acc.x, acc.y, acc.z);
+    if (xyz) {
+      tom2_madd<false>(acc, acc, q);
+      tom_st_xyz(proj + (size_t)t * TOM_PROJ_WORDS, acc.x, acc.y, acc.z);
+    } else {
+      TomEfgh e;
+      tom2_madd_end(e, acc, q);
+      tom_st_efgh(proj + (size_t)t * TOM_E2_WORDS, e);
+    }
   }
 };
 
-struct TomCommitGTask {   // one thread per (item, g-part): K = v*g as an extended E2 point
+struct TomCommitGTask {   // one thread per (item, g-part): K = v*g as an extended E2 point, from v's first entry
   const uint32_t* jv;     // [items*34][8]
   const uint32_t* gtab;
   uint32_t* ext;          // [items*28][36]
@@ -618,28 +661,29 @@ struct TomCommitGTask {   // one thread per (item, g-part): K = v*g as an extend
     const int item = t / GJOBS_PER_ITEM, g = t % GJOBS_PER_ITEM;
     uint32_t v[8];
     ld<8>(v, jv + ((size_t)item * JOBS_PER_ITEM + item_job_of_gpart(g)) * 8);
-    TomPt acc;
-    tom_set_identity(acc);
     const size_t ne = (size_t)fb_entries(w);
     uint32_t carry = 0;
+    bool neg;
+    TomPre q;
+    const uint32_t d0 = signed_digit(v, 0, w, carry, neg);
+    tom2_ld_entry(q, gtab, 0, ne, d0, neg);
+    TomPt acc;
+    tom2_from_pre<TompCommit>(acc, q);
 #pragma unroll 1
-    for (int j = 0; j < nwin; j++) {
-      TomPre q;
-      bool neg;
+    for (int j = 1; j < nwin; j++) {
       const uint32_t d = signed_digit(v, j, w, carry, neg);
-      tom_ld_pre(q, gtab + ((size_t)j * ne + d) * TOM_PRE_WORDS);
-      tom2_pre_neg(q, neg);
+      tom2_ld_entry(q, gtab, j, ne, d, neg);
       tom2_madd<true, TompCommit>(acc, acc, q);
     }
     uint32_t* o = ext + (size_t)t * TOM_EXT_WORDS;
     st<9>(o, acc.x); st<9>(o + 9, acc.y); st<9>(o + 18, acc.t); st<9>(o + 27, acc.z);
   }
 };
-struct TomCommitHTask {   // one thread per job: C = K + r*h
+struct TomCommitHTask {   // one thread per job: C = K + r*h, ending in tom2_madd_end for the normaliser
   const uint32_t* jr;     // [items*34][8]
   const uint32_t* htab;
   const uint32_t* ext;    // [items*28][36]
-  uint32_t* proj;         // [items*34][28]
+  uint32_t* proj;         // [items*34][TOM_E2_WORDS]  (E, F, G, H) -> TomNormTask{e2 = 1}
   int w, nwin;
   ZK_HD void operator()(int t) const {
     const int item = t / JOBS_PER_ITEM, jb = t % JOBS_PER_ITEM;
@@ -650,16 +694,19 @@ struct TomCommitHTask {   // one thread per job: C = K + r*h
     ld<9>(acc.x, s); ld<9>(acc.y, s + 9); ld<9>(acc.t, s + 18); ld<9>(acc.z, s + 27);
     const size_t ne = (size_t)fb_entries(w);
     uint32_t carry = 0;
+    bool neg;
+    TomPre q;
 #pragma unroll 1
-    for (int j = 0; j < nwin; j++) {
-      TomPre q;
-      bool neg;
+    for (int j = 0; j < nwin - 1; j++) {
       const uint32_t d = signed_digit(r, j, w, carry, neg);
-      tom_ld_pre(q, htab + ((size_t)j * ne + d) * TOM_PRE_WORDS);
-      tom2_pre_neg(q, neg);
+      tom2_ld_entry(q, htab, j, ne, d, neg);
       tom2_madd<true, TompCommit>(acc, acc, q);
     }
-    tom_st_xyz(proj + (size_t)t * TOM_PROJ_WORDS, acc.x, acc.y, acc.z);
+    const uint32_t d = signed_digit(r, nwin - 1, w, carry, neg);
+    tom2_ld_entry(q, htab, nwin - 1, ne, d, neg);
+    TomEfgh e;
+    tom2_madd_end<TompCommit>(e, acc, q);
+    tom_st_efgh(proj + (size_t)t * TOM_E2_WORDS, e);
   }
 };
 

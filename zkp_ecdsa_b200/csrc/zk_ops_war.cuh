@@ -33,6 +33,7 @@ struct TomNormTask {
   int chunk;             // points per thread (<= NORM_CHUNK_MAX)
   int e2;
   int aff_mod, aff_lim;  // the affine pair is produced only for points with (index % aff_mod) < aff_lim
+  int stride;            // words per input slot (TOM_PROJ_WORDS = TOM_E2_WORDS)
   ZK_HD void operator()(int t) const {
     using F = Warp;
     const int lo = t * chunk;
@@ -44,7 +45,7 @@ struct TomNormTask {
     F::set_one(one);
     copy_n<8>(acc, one);
     for (int k = 0; k < n; k++) {
-      ld<8>(z, proj + (size_t)(lo + k) * TOM_PROJ_WORDS + 16);
+      ld<8>(z, proj + (size_t)(lo + k) * stride + 16);
       if (is_zero_n<8>(z)) copy_n<8>(z, one);
       F::mul(acc, acc, z);
       copy_n<8>(pre[k], acc);
@@ -52,7 +53,7 @@ struct TomNormTask {
     uint32_t inv[8];
     F::inv(inv, acc);
     for (int k = n - 1; k >= 0; k--) {
-      const uint32_t* src = proj + (size_t)(lo + k) * TOM_PROJ_WORDS;
+      const uint32_t* src = proj + (size_t)(lo + k) * stride;
       ld<8>(z, src + 16);
       const bool isinf = is_zero_n<8>(z);
       if (isinf) copy_n<8>(z, one);
@@ -80,7 +81,9 @@ struct TomNormTask {
   }
 };
 
-// Pedersen commitment in the proof group:  C = v*g + r*h   (pedersen.ts:53-58, gk.ts:88-92)
+// Pedersen commitment in the proof group:  C = v*g + r*h   (pedersen.ts:53-58, gk.ts:88-92).  Both walks run on one
+// Jacobian accumulator that starts at the identity: jac_madd takes the first non-zero digit's entry as (x : y : 1)
+// without products, as the tomEdwards256 walks start at their first entry.
 struct TomCommitTask {
   const uint32_t* jv;    // [count][8] canonical value scalars (mod war256.order = p256.p)
   const uint32_t* jr;    // [count][8] canonical blinders
@@ -88,14 +91,17 @@ struct TomCommitTask {
   const uint32_t* htab;
   uint32_t* proj;        // [count][24]
   int w, nwin;
+  int xyz = 0;           // the tomEdwards256 build's output-form flag; the output here is always (X, Y, Z)
   ZK_HD void operator()(int t) const {
     uint32_t v[8], r[8];
     ld<8>(v, jv + (size_t)t * 8);
     ld<8>(r, jr + (size_t)t * 8);
+    WarJac aj;
+    war_set_identity_jac(aj);
+    war_accum_fixed_jac(aj, gtab, v, w);
+    war_accum_fixed_jac(aj, htab, r, w);
     WarPt acc;
-    war_set_identity(acc);
-    war_accum_fixed(acc, gtab, v, w);
-    war_accum_fixed(acc, htab, r, w);
+    war_jac_to_hom(acc, aj);
     war_st_proj(proj + (size_t)t * TOM_PROJ_WORDS, acc);
   }
 };
@@ -109,9 +115,11 @@ struct TomCommitGTask {   // one thread per (item, g-part): K = v*g
     const int item = t / GJOBS_PER_ITEM, g = t % GJOBS_PER_ITEM;
     uint32_t v[8];
     ld<8>(v, jv + ((size_t)item * JOBS_PER_ITEM + item_job_of_gpart(g)) * 8);
+    WarJac aj;
+    war_set_identity_jac(aj);
+    war_accum_fixed_jac(aj, gtab, v, w);
     WarPt acc;
-    war_set_identity(acc);
-    war_accum_fixed(acc, gtab, v, w);
+    war_jac_to_hom(acc, aj);
     war_st_proj(ext + (size_t)t * TOM_EXT_WORDS, acc);
   }
 };

@@ -718,7 +718,7 @@ struct DerivedTask {
   struct Store {   // derived point d of item `it`, projective (the address is formed at each store)
     const ProveCtx& c;
     int it;
-    ZK_HD void operator()(int d, const TomPt& p) const { tom_st_xyz(c.s2_proj + c.s2_der(it, d) * TOM_PROJ_WORDS, p.x, p.y, p.z); }
+    ZK_HD void operator()(int d, const TomPt& p) const { tom_st_xyz(c.s2_proj + c.s2_der(it, d) * TOM_E2_WORDS, p.x, p.y, p.z); }
   };
   ZK_HD void ldaff(TomPt& p, const uint32_t* aff, size_t idx) const {
     uint32_t x[PGL], y[PGL];

@@ -443,13 +443,15 @@ inline void launch_p256_norm(Stream& st, const uint32_t* proj, uint32_t* aff, ui
   const int ch = norm_chunk_for(count, bytes ? 7 : 5);
   launch(st, (count + ch - 1) / ch, P256NormTask{proj, aff, bytes, inf, (int)count, ch});
 }
-// e2 = 1: the points come from TomCommitTask (a = -1 image curve E2); e2 = 0: E1 projective
+// e2 = 1: the points come from TomCommitTask / TomCommitHTask (E, F, G, H on the a = -1 image curve E2, TOM_E2_WORDS
+// apart); e2 = 0: E1 projective (X, Y, Z), TOM_PROJ_WORDS apart unless `stride` says otherwise
 // aff may be null; otherwise the E1 affine pair is written for points with (index % aff_mod) < aff_lim
 inline void launch_tom_norm(Stream& st, const uint32_t* proj, uint32_t* aff, uint8_t* bytes, long long count, int e2,
-                            int aff_mod = 1, int aff_lim = 1) {
+                            int aff_mod = 1, int aff_lim = 1, int stride = 0) {
   if (count <= 0) return;
   const int ch = norm_chunk_for(count);
-  launch(st, (count + ch - 1) / ch, TomNormTask{proj, aff, bytes, (int)count, ch, e2, aff_mod, aff_lim});
+  if (stride == 0) stride = e2 ? TOM_E2_WORDS : TOM_PROJ_WORDS;
+  launch(st, (count + ch - 1) / ch, TomNormTask{proj, aff, bytes, (int)count, ch, e2, aff_mod, aff_lim, stride});
 }
 
 // ---- table construction -------------------------------------------------------------------
@@ -736,16 +738,17 @@ void prove_items_gk(Stream& st, const ProveCtx& c, uint32_t* gext, bool items, b
     launch(st, nj, TomCommitHTask{c.s2_jr, c.th_tab, gext, c.s2_proj, c.tom_w, c.tom_nwin});
   }
   if (gk)
-    launch(st, ng, TomCommitTask{c.s2_jv + g0 * 8, c.s2_jr + g0 * 8, c.tg_tab, c.th_tab, c.s2_proj + g0 * TOM_PROJ_WORDS, c.tom_w,
+    launch(st, ng, TomCommitTask{c.s2_jv + g0 * 8, c.s2_jr + g0 * 8, c.tg_tab, c.th_tab, c.s2_proj + g0 * TOM_E2_WORDS, c.tom_w,
                                  c.tom_nwin});
   if (items) {
     // only T1x, T1y (jobs 0, 1 of each item) are needed again as points (DerivedTask)
     launch_tom_norm(st, c.s2_proj, c.s2_aff, c.s2_bytes, nj, 1, JOBS_PER_ITEM, 2);
     launch(st, M, DerivedTask{c});
-    // derived points come from complete E1 additions, the GK commitments from the commit kernel (E2)
-    launch_tom_norm(st, c.s2_proj + nj * TOM_PROJ_WORDS, nullptr, c.s2_bytes + nj * BSTRIDE, nd, 0);
+    // derived points come from complete E1 additions, the GK commitments from the commit kernel (E2); every s2 slot
+    // is TOM_E2_WORDS wide, a derived point's (X, Y, Z) fills the first TOM_PROJ_WORDS of one
+    launch_tom_norm(st, c.s2_proj + nj * TOM_E2_WORDS, nullptr, c.s2_bytes + nj * BSTRIDE, nd, 0, 1, 1, TOM_E2_WORDS);
   }
-  if (gk) launch_tom_norm(st, c.s2_proj + g0 * TOM_PROJ_WORDS, nullptr, c.s2_bytes + g0 * BSTRIDE, ng, 1);
+  if (gk) launch_tom_norm(st, c.s2_proj + g0 * TOM_E2_WORDS, nullptr, c.s2_bytes + g0 * BSTRIDE, ng, 1);
   if (items) {
     launch(st, M * HASHES_PER_ITEM, ItemHashTask{c});
     launch(st, M * 7, ItemEmitTask{c});
@@ -1095,7 +1098,7 @@ int zka_tom_commit_batch(zka_ctx* ctx, const zka_params* P, uint32_t count, cons
     const uint8_t* dr = stage_in(st, in.next(), r, (size_t)count * 32);
     uint32_t* jv = w.take<uint32_t>((size_t)count * 8);
     uint32_t* jr = w.take<uint32_t>((size_t)count * 8);
-    uint32_t* proj = w.take<uint32_t>((size_t)count * TOM_PROJ_WORDS);
+    uint32_t* proj = w.take<uint32_t>((size_t)count * TOM_E2_WORDS);
     uint32_t* aff = w.take<uint32_t>((size_t)count * TOM_AFF_WORDS);
     uint8_t* bytes = w.take<uint8_t>((size_t)count * BSTRIDE);
     const Output<uint8_t> o(out, WP);
@@ -1198,7 +1201,7 @@ int zka_params_generate(zka_ctx* ctx, const uint8_t rnd[64], uint8_t h_nist[65],
     Cursor in(ctx->in[0]), w(ctx->w);
     uint32_t* jv = w.take<uint32_t>(8);
     uint32_t* jr = w.take<uint32_t>(8);
-    uint32_t* proj = w.take<uint32_t>(TOM_PROJ_WORDS);
+    uint32_t* proj = w.take<uint32_t>(TOM_E2_WORDS);
     uint32_t* aff = w.take<uint32_t>(TOM_AFF_WORDS);
     uint8_t* bytes = w.take<uint8_t>(BSTRIDE);
     uint8_t* d_rnd = in.take<uint8_t>(32);
@@ -1380,7 +1383,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         c.pa_A_inf = w.take<uint8_t>(nA);
         c.s1_jv = w.take<uint32_t>(n1 * 8);
         c.s1_jr = w.take<uint32_t>(n1 * 8);
-        c.s1_proj = w.take<uint32_t>(n1 * TOM_PROJ_WORDS);
+        c.s1_proj = w.take<uint32_t>(n1 * TOM_E2_WORDS);
         c.s1_aff = w.take<uint32_t>(n1 * TOM_AFF_WORDS);
         c.s1_bytes = w.take<uint8_t>(n1 * BSTRIDE);
         c.chal = w.take<uint32_t>((size_t)Bc * 3);
@@ -1481,7 +1484,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8
         const size_t n2 = c.s2_count();
         c.s2_jv = w.take<uint32_t>(n2 * 8);
         c.s2_jr = w.take<uint32_t>(n2 * 8);
-        c.s2_proj = w.take<uint32_t>(n2 * TOM_PROJ_WORDS);
+        c.s2_proj = w.take<uint32_t>(n2 * TOM_E2_WORDS);
         c.s2_aff = w.take<uint32_t>(n2 * TOM_AFF_WORDS);
         c.s2_bytes = w.take<uint8_t>(n2 * BSTRIDE);
         c.secrets = w.take<uint32_t>((size_t)M * SECRETS_PER_ITEM * 8);
@@ -1675,7 +1678,7 @@ int zka_prove_membership_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, co
       const size_t ng = (size_t)Bc * 4 * n;
       c.s2_jv = w.take<uint32_t>(ng * 8);
       c.s2_jr = w.take<uint32_t>(ng * 8);
-      c.s2_proj = w.take<uint32_t>(ng * TOM_PROJ_WORDS);
+      c.s2_proj = w.take<uint32_t>(ng * TOM_E2_WORDS);
       c.s2_bytes = w.take<uint8_t>(ng * BSTRIDE);
       c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * n * gk_blocks(n) * 8);
       c.proof_stride = proof_stride;
@@ -1716,7 +1719,7 @@ static int prove_sub(zka_ctx* ctx, const zka_params* P, int kind, uint32_t B, co
       const size_t nj = (size_t)Bc * J;
       uint32_t* jv = w.take<uint32_t>(nj * 8);
       uint32_t* jr = w.take<uint32_t>(nj * 8);
-      uint32_t* proj = w.take<uint32_t>(nj * TOM_PROJ_WORDS);
+      uint32_t* proj = w.take<uint32_t>(nj * TOM_E2_WORDS);
       uint8_t* bytes = w.take<uint8_t>(nj * BSTRIDE);
       uint8_t* d_com = co.rows(ob.next(), b0, Bc);
       uint8_t* d_prf = po.rows(ob.next(), b0, Bc);
@@ -1782,12 +1785,12 @@ int zka_prove_pointadd_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, cons
       c.rep_off = w.take<uint32_t>(Bc);
       c.s1_jv = w.take<uint32_t>(n1 * 8);
       c.s1_jr = w.take<uint32_t>(n1 * 8);
-      c.s1_proj = w.take<uint32_t>(n1 * TOM_PROJ_WORDS);
+      c.s1_proj = w.take<uint32_t>(n1 * TOM_E2_WORDS);
       c.s1_aff = w.take<uint32_t>(n1 * TOM_AFF_WORDS);
       c.s1_bytes = w.take<uint8_t>(n1 * BSTRIDE);
       c.s2_jv = w.take<uint32_t>(n2 * 8);
       c.s2_jr = w.take<uint32_t>(n2 * 8);
-      c.s2_proj = w.take<uint32_t>(n2 * TOM_PROJ_WORDS);
+      c.s2_proj = w.take<uint32_t>(n2 * TOM_E2_WORDS);
       c.s2_aff = w.take<uint32_t>(n2 * TOM_AFF_WORDS);
       c.s2_bytes = w.take<uint8_t>(n2 * BSTRIDE);
       c.secrets = w.take<uint32_t>((size_t)Bc * SECRETS_PER_ITEM * 8);
@@ -2022,7 +2025,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       c.sp_T_inf = w.take<uint8_t>(ns);
       c.ta_jv = w.take<uint32_t>(ns * 2 * 8);
       c.ta_jr = w.take<uint32_t>(ns * 2 * 8);
-      c.ta_proj = w.take<uint32_t>(ns * 2 * TOM_PROJ_WORDS);
+      c.ta_proj = w.take<uint32_t>(ns * 2 * TOM_E2_WORDS);
       c.ta_aff = w.take<uint32_t>(ns * 2 * TOM_AFF_WORDS);
       c.td_proj = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_PROJ_WORDS);
       c.td_aff = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_AFF_WORDS);
@@ -2095,7 +2098,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
       launch(st, Bc, VReduceTask{c});
       launch(st, (long long)Bc * ET, VParseEntriesTask{c.proofs, proof_stride, c.ent_off, c.ent_pre, ET});
       if (mode == 0) launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, proof_stride, gk_offs, c.gk_pre, ngk});
-      launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin});
+      launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin, 1});
       // chunk-wide aggregate check (zk_verify_agg.cuh): the sum over all proofs of the chunk of the three linear
       // combinations, as ONE wide-window MSM per group; when both sums are the identity the per-proof MSMs below
       // return at once
@@ -2143,7 +2146,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint
         // fixed-base parts: one commitment for the summed tomEdwards256 scalars, a two-level sum of the P-256 points
         launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, fpart, Bc});
         launch(st, 1, AggFixSumTask{ctl, fpart, fjv, fjr, fgroups});
-        launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom_w, c.tom_nwin});
+        launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom_w, c.tom_nwin, 1});
         launch(sb, ngroups, AggNistFixPartTask{ctl, c.nfix, npart, Bc});
         int nleft = ngroups;            // second level: at most Bc / 1024 partial sums reach the final thread
         const uint32_t* nsum = npart;
@@ -2284,7 +2287,7 @@ int zka_verify_membership_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, c
       dev_memset(st, c.fx_jr, 0, (size_t)Bc * 2 * 8 * 4);
       verify_gk(st, c, gk_offs);
       launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, row_stride, gk_offs, c.gk_pre, ngk});
-      launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin});
+      launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin, 1});
       launch(st, (long long)Bc * MSM_NWIN, MsmTomWindowTask{c.gk_scalar, c.gk_pre, nullptr, ngk, 0, 0, ngk, V_SEG, 1, c.win_g});
       launch(st, Bc, MsmTomCombineTask{c.win_g, c.fx_proj, c.id_flags, 2, 0, 0});
       launch(st, Bc, VGkOnlyFinalTask{c});
@@ -2330,7 +2333,7 @@ static int verify_sub(zka_ctx* ctx, const zka_params* P, int kind, uint32_t B, c
       launch(st, Bc, VSubProofTask{kind, rows, stride, d_tape, tape_stride, (const uint8_t*)ctx->tg_bytes.p, ent_scalar, ent_off,
                                    fx_jv, fx_jr, d_st, d_ok});
       launch(st, (long long)Bc * SUB_ENT_MAX, VParseEntriesTask{rows, stride, ent_off, ent_pre, SUB_ENT_MAX});
-      launch(st, (long long)Bc * 2, TomCommitTask{fx_jv, fx_jr, ctx->tg.tab, P->th.tab, fx_proj, ctx->tom_w, ctx->tom_nwin});
+      launch(st, (long long)Bc * 2, TomCommitTask{fx_jv, fx_jr, ctx->tg.tab, P->th.tab, fx_proj, ctx->tom_w, ctx->tom_nwin, 1});
       launch(st, (long long)Bc * MSM_NWIN, MsmTomWindowTask{ent_scalar, ent_pre, nullptr, SUB_ENT_MAX, 0, 0, ne, V_SEG, 1, win});
       launch(st, Bc, MsmTomCombineTask{win, fx_proj, flags, 2, 1, 1});
       launch(st, Bc, VSubFinalTask{d_st, flags, d_ok});
