@@ -154,36 +154,18 @@ ZK_HD bool draw_checked(uint32_t* r, const ProveCtx& c, int b, int draw) {
 struct PreKeyTask {   // validate and store the public key (everything the key tables depend on)
   ProveCtx c;
   ZK_HD void operator()(int b) const {
-    using Fp = P256p;
     c.status[b] = ZKA_OK;
-    const uint8_t* pkb = c.pk + (size_t)b * 65;
-    uint32_t px[8], py[8];
-    limbs_from_be<8>(px, pkb + 1, 32);
-    limbs_from_be<8>(py, pkb + 33, 32);
     P256Aff pk;
-    bool ok = (pkb[0] == 0x04);
-    // weier.ts:74-89 does not range-check x,y; isOnGroup works mod p.  Reduce then test.
-    reduce_once<FpP256>(px);
-    reduce_once<FpP256>(py);
-    Fp::to_mont(pk.x, px);
-    Fp::to_mont(pk.y, py);
-    ok = ok && p256_on_curve(pk.x, pk.y);
-    if (!ok) {
+    bool inf;
+    if (!p256_parse(pk, inf, c.pk + (size_t)b * 65) || inf) {   // the identity is no key either
       ZK_SET_STATUS(c.status + b, ZKA_ERR_INVALID_PK);
       // keep going with the generator so later stages stay well defined
       p256_set_generator(pk);
     }
     p256_st_aff(c.pk_aff + (size_t)b * 16, pk);
     if (c.mode == 1) {   // the tables are built for paramsNIST.g, an input of its own
-      const uint8_t* bb = c.base + (size_t)b * 65;
-      limbs_from_be<8>(px, bb + 1, 32);
-      limbs_from_be<8>(py, bb + 33, 32);
-      reduce_once<FpP256>(px);
-      reduce_once<FpP256>(py);
       P256Aff g;
-      Fp::to_mont(g.x, px);
-      Fp::to_mont(g.y, py);
-      if (!(bb[0] == 0x04 && p256_on_curve(g.x, g.y))) {
+      if (!p256_parse(g, inf, c.base + (size_t)b * 65) || inf) {
         ZK_SET_STATUS(c.status + b, ZKA_ERR_INVALID_PK);
         p256_set_generator(g);
       }
@@ -212,19 +194,8 @@ struct PreTask {      // the scalars of the statement and Q = z1*G
       Fn::set_one(u);
       st<8>(c.u12 + (size_t)b * 16 + 8, u);
       P256Aff Qa;
-      bool qinf = true;
-      if (c.q_in) {
-        const uint8_t* qb = c.q_in + (size_t)b * 65;
-        uint32_t qx[8], qy[8];
-        limbs_from_be<8>(qx, qb + 1, 32);
-        limbs_from_be<8>(qy, qb + 33, 32);
-        qinf = (qb[0] == 0) && is_zero_n<8>(qx) && is_zero_n<8>(qy);
-        reduce_once<FpP256>(qx);
-        reduce_once<FpP256>(qy);
-        Fp::to_mont(Qa.x, qx);
-        Fp::to_mont(Qa.y, qy);
-        if (!qinf && !(qb[0] == 0x04 && p256_on_curve(Qa.x, Qa.y))) { ZK_SET_STATUS(c.status + b, ZKA_ERR_INVALID_PK); qinf = true; }
-      }
+      bool qinf = true;   // no Q, the identity, or an invalid Q (flagged): no Q term
+      if (c.q_in && !p256_parse(Qa, qinf, c.q_in + (size_t)b * 65)) { ZK_SET_STATUS(c.status + b, ZKA_ERR_INVALID_PK); qinf = true; }
       if (qinf) p256_set_generator(Qa);
       p256_st_aff(c.q_aff + (size_t)b * 16, Qa);
       c.q_inf[b] = qinf ? 1 : 0;
@@ -665,45 +636,19 @@ struct ItemScalarsTask {
       else if (m == 1) { x = i8;  y = i9;  z = i10; rx = m8;  ry = r9;  rz = m10; }
       else if (m == 2) { x = i10; y = i10; z = i11; rx = m10; ry = m10; rz = m11; }
       else             { x = i10; y = i12; z = i13; rx = m10; ry = r12; rz = m13; }
-      const int dm = d0 + item_mult_draw(m);
-      uint32_t kx[8], ky[8], kz[8], ra[8], mkx[8], t[8], u[8], r4[8];
-      draw_checked<FpP256>(kx, c, b, dm + 0);
-      draw_checked<FpP256>(ky, c, b, dm + 1);
-      draw_checked<FpP256>(kz, c, b, dm + 2);
-      F::to_mont(mkx, kx);
-      const int j0 = JOB_MULT0 + 6 * m;
-      // C4 = Cy*x = (x y) g + (x ry) h ; r4 = ry*x   (mult.ts:103-104)
-      F::mul(t, x, y);
-      F::mul(r4, x, ry);
-      F::from_mont(u, r4);
-      job(it, j0 + 0, t, u);
-      // Ax, Ay, Az, A4_1 = commit(k_x), commit(k_y), commit(k_z), commit(k_z) (mult.ts:110-113)
-      draw_checked<FpP256>(ra, c, b, dm + 3);
-      job_raw(it, j0 + 1, kx, ra);
-      draw_checked<FpP256>(ra, c, b, dm + 4);
-      job_raw(it, j0 + 2, ky, ra);
-      draw_checked<FpP256>(ra, c, b, dm + 5);
-      job_raw(it, j0 + 3, kz, ra);
-      draw_checked<FpP256>(ra, c, b, dm + 6);
-      job_raw(it, j0 + 4, kz, ra);
-      // A4_2 = Cy*k_x = (k_x y) g + (k_x ry) h   (mult.ts:114)
-      F::mul(t, mkx, y);
-      F::mul(u, mkx, ry);
-      F::from_mont(u, u);
-      job(it, j0 + 5, t, u);
+      const int dm = d0 + item_mult_draw(m), j0 = JOB_MULT0 + 6 * m;
+      uint32_t r4[8];
+      mult_openings([&](int k, const uint32_t* v, const uint32_t* r) { job_raw(it, j0 + k, v, r); },
+                    [&](int q, uint32_t* r) { draw_checked<FpP256>(r, c, b, dm + q); }, x, y, ry, r4);
       uint32_t* sm = sec + (size_t)m * 7 * 8;
       st8v(sm, x); st8v(sm + 8, y); st8v(sm + 16, z);
       st8v(sm + 24, rx); st8v(sm + 32, ry); st8v(sm + 40, rz); st8v(sm + 48, r4);
     }
     // the two EqualityProofs (pointAdd.ts:151-160): (x, r1, r2)
     for (int e = 0; e < 2; e++) {
-      const int de = d0 + (e == 0 ? IT_EQ0 : IT_EQ1);
-      uint32_t kk[8], ra[8];
-      draw_checked<FpP256>(kk, c, b, de + 0);
-      draw_checked<FpP256>(ra, c, b, de + 1);
-      job_raw(it, JOB_EQ0 + 2 * e, kk, ra);
-      draw_checked<FpP256>(ra, c, b, de + 2);
-      job_raw(it, JOB_EQ0 + 2 * e + 1, kk, ra);
+      const int de = d0 + (e == 0 ? IT_EQ0 : IT_EQ1), j0 = JOB_EQ0 + 2 * e;
+      equality_openings([&](int k, const uint32_t* v, const uint32_t* r) { job_raw(it, j0 + k, v, r); },
+                        [&](int q, uint32_t* r) { draw_checked<FpP256>(r, c, b, de + q); });
       uint32_t* se = sec + (size_t)(28 + 3 * e) * 8;
       st8v(se, e == 0 ? i11 : i13);
       st8v(se + 8, e == 0 ? m11 : m13);
@@ -770,14 +715,6 @@ struct ItemHashTask {
   }
 };
 
-// response t = k - c*w  (mod q): k canonical, w Montgomery, c canonical 80-bit
-ZK_HD void response(uint32_t* t, const uint32_t* k_canon, const uint32_t* cc, const uint32_t* w_mont) {
-  using F = Tomq;
-  uint32_t cw[8];
-  F::mul(cw, cc, w_mont);   // c * (w R) / R = c*w, canonical
-  F::sub(t, k_canon, cw);
-}
-
 // Stage 8 — responses + byte assembly of one 0-bit repetition (exp.ts:212-225,
 // pointAdd.ts:162, mult.ts:122-130, equality.ts:73-77).  One thread per (item, part):
 // part 0..3 MultProof m, 4..5 EqualityProof e, 6 repetition header/tail.  Each part writes its
@@ -799,39 +736,22 @@ struct ItemEmitTask {
       ByteWriter o(pa + 4 * WP + m * MULT_LEN);
 #pragma unroll
       for (int p = 0; p < 6; p++) o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_MULT0 + 6 * m + p) * BSTRIDE);
-      uint32_t cc[8], c3[3], kk[8], w[8], r[8];
+      uint32_t cc[8], c3[3];
       ld<3>(c3, c.item_chal + (it * HASHES_PER_ITEM + m) * 3);
       challenge_to_limbs(cc, c3);
-      const int dm = d0 + item_mult_draw(m);
-      const uint32_t* sm = sec + (size_t)m * 7 * 8;
-      // t_x t_y t_z t_rx t_ry t_rz t_r4 ; k's: kx ky kz Ax.r Ay.r Az.r A4_1.r ; w: x y z rx ry rz r4
-#pragma unroll
-      for (int q = 0; q < 7; q++) {
-        tape_draw(kk, c.tape_of(b), dm + q);
-        reduce_once<FpP256>(kk);
-        ld8v(w, sm + q * 8);
-        response(r, kk, cc, w);
-        o.put_scalar<WS>(r);
-      }
+      const uint32_t* sm = sec + (size_t)m * 7 * 8;   // x y z rx ry rz r4
+      sigma_responses<7>(o, cc, c.tape_of(b), d0 + item_mult_draw(m), [&](int q, uint32_t* w) { ld8v(w, sm + q * 8); });
       o.finish();
     } else if (part < 6) {
       const int e = part - 4;
       ByteWriter o(pa + 4 * WP + 4 * MULT_LEN + e * EQ_LEN);
       o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_EQ0 + 2 * e) * BSTRIDE);
       o.put_point<WP>(c.s2_bytes + c.s2_job(it, JOB_EQ0 + 2 * e + 1) * BSTRIDE);
-      uint32_t cc[8], c3[3], kk[8], w[8], r[8];
+      uint32_t cc[8], c3[3];
       ld<3>(c3, c.item_chal + (it * HASHES_PER_ITEM + 4 + e) * 3);
       challenge_to_limbs(cc, c3);
-      const int de = d0 + (e == 0 ? IT_EQ0 : IT_EQ1);
-      const uint32_t* se = sec + (size_t)(28 + 3 * e) * 8;
-#pragma unroll
-      for (int q = 0; q < 3; q++) {   // t_x = k - c x ; t_r1 = A1.r - c C1.r ; t_r2 = A2.r - c C2.r
-        tape_draw(kk, c.tape_of(b), de + q);
-        reduce_once<FpP256>(kk);
-        ld8v(w, se + q * 8);
-        response(r, kk, cc, w);
-        o.put_scalar<WS>(r);
-      }
+      const uint32_t* se = sec + (size_t)(28 + 3 * e) * 8;   // x, C1.r, C2.r
+      sigma_responses<3>(o, cc, c.tape_of(b), d0 + (e == 0 ? IT_EQ0 : IT_EQ1), [&](int q, uint32_t* w) { ld8v(w, se + q * 8); });
       o.finish();
     } else {
       // z = alpha - s1, z2 = r_i - comS1.r  (mod n)  (exp.ts:186,221); r1 = T1x.r, r2 = T1y.r
@@ -1214,27 +1134,21 @@ struct SubProveJobsTask {
     uint32_t* v = jv + (size_t)b * J * 8;
     uint32_t* r = jr + (size_t)b * J * 8;
     bool ok = true;
+    const int j0 = kind == 0 ? 2 : 3;   // the proof's own points follow the statement's
+    auto job = [&](int k, const uint32_t* vk, const uint32_t* rk) { st<8>(v + 8 * (j0 + k), vk); st<8>(r + 8 * (j0 + k), rk); };
+    auto draw = [&](int q, uint32_t* d) { ok = rd(d, dr, q) && ok; };
     if (kind == 0) {
-      uint32_t x[8], r1[8], r2[8], k[8], ra[8], rb[8];
+      uint32_t x[8], r1[8], r2[8];
       rd(x, sc); rd(r1, sc + 32); rd(r2, sc + 64);      // newScalar reduces the statement's values
-      ok = rd(k, dr, 0) && ok; ok = rd(ra, dr, 1) && ok; ok = rd(rb, dr, 2) && ok;
       st<8>(v, x); st<8>(r, r1); st<8>(v + 8, x); st<8>(r + 8, r2);
-      st<8>(v + 16, k); st<8>(r + 16, ra); st<8>(v + 24, k); st<8>(r + 24, rb);
+      equality_openings(job, draw);
     } else {
-      uint32_t x[8], y[8], z[8], rx[8], ry[8], rz[8], kx[8], ky[8], kz[8], a1[8], a2[8], a3[8], a4[8];
-      rd(x, sc); rd(y, sc + 32); rd(z, sc + 64); rd(rx, sc + 96); rd(ry, sc + 128); rd(rz, sc + 160);
-      ok = rd(kx, dr, 0) && ok; ok = rd(ky, dr, 1) && ok; ok = rd(kz, dr, 2) && ok;
-      ok = rd(a1, dr, 3) && ok; ok = rd(a2, dr, 4) && ok; ok = rd(a3, dr, 5) && ok; ok = rd(a4, dr, 6) && ok;
-      uint32_t xm[8], kxm[8], t[8], u[8];
-      F::to_mont(xm, x);
-      F::to_mont(kxm, kx);
-      st<8>(v, x); st<8>(r, rx); st<8>(v + 8, y); st<8>(r + 8, ry); st<8>(v + 16, z); st<8>(r + 16, rz);
-      F::mul(t, xm, y); F::mul(u, xm, ry);              // C4 = Cy*x = (x y) g + (x ry) h   (mult.ts:103-104)
-      st<8>(v + 24, t); st<8>(r + 24, u);
-      st<8>(v + 32, kx); st<8>(r + 32, a1); st<8>(v + 40, ky); st<8>(r + 40, a2);
-      st<8>(v + 48, kz); st<8>(r + 48, a3); st<8>(v + 56, kz); st<8>(r + 56, a4);
-      F::mul(t, kxm, y); F::mul(u, kxm, ry);            // A4_2 = Cy*k_x                    (mult.ts:114)
-      st<8>(v + 64, t); st<8>(r + 64, u);
+      uint32_t s[6][8];   // x y z rx ry rz
+      for (int q = 0; q < 6; q++) rd(s[q], sc + 32 * q);
+      for (int k = 0; k < 3; k++) { st<8>(v + 8 * k, s[k]); st<8>(r + 8 * k, s[3 + k]); }
+      uint32_t xm[8], ym[8], rym[8], r4[8];
+      F::to_mont(xm, s[0]); F::to_mont(ym, s[1]); F::to_mont(rym, s[4]);
+      mult_openings(job, draw, xm, ym, rym, r4);
     }
     if (!ok) ZK_SET_STATUS(status + b, ZKA_ERR_TAPE_RANGE);
   }
@@ -1262,32 +1176,22 @@ struct SubProveEmitTask {
     const uint8_t* pb = bytes + (size_t)b * J * BSTRIDE;
     const uint8_t* sc = scalars + (size_t)b * (kind == 0 ? 3 : 6) * 32;
     const uint8_t* dr = tape + (size_t)b * tape_stride;
-    Sha256 h;
-    h.init();
-    for (int j = 0; j < J; j++) h.update(pb + (size_t)j * BSTRIDE, WP);
-    uint32_t c3[3], cc[8];
-    h.final80(c3);
+    uint32_t c3[3], cc[8];   // the challenge hashes the statement, then the proof's own points: every job in order
+    hash_points80(c3, [&](int j, int& len) { len = WP; return pb + (size_t)j * BSTRIDE; }, J);
     challenge_to_limbs(cc, c3);
     ByteWriter oc(com), o(out);
     for (int j = 0; j < nc; j++) oc.put_point<WP>(pb + (size_t)j * BSTRIDE);
     oc.finish();
     for (int j = nc; j < J; j++) o.put_point<WP>(pb + (size_t)j * BSTRIDE);
-    auto resp = [&](int q, const uint32_t* w_canon) {   // response q, with draw q of the row
-      uint32_t k[8], wm[8], t[8];
-      tape_draw(k, dr, q);
-      reduce_once<FpP256>(k);
-      F::to_mont(wm, w_canon);
-      response(t, k, cc, wm);
-      o.put_scalar<WS>(t);
+    // the secrets are the statement's scalars in row order, then (mult) r4 = x ry, the blinder of C4 (job 3)
+    auto w = [&](int q, uint32_t* wm) {
+      uint32_t s[8];
+      if (q < 6) { limbs_from_be<8>(s, sc + 32 * q, 32); reduce_once<FpP256>(s); }
+      else ld<8>(s, jr + ((size_t)b * J + 3) * 8);
+      F::to_mont(wm, s);
     };
-    uint32_t w[8];
-    if (kind == 0) {   // t_x = k - c x, t_r1 = A1.r - c r1, t_r2 = A2.r - c r2
-      for (int q = 0; q < 3; q++) { limbs_from_be<8>(w, sc + 32 * q, 32); reduce_once<FpP256>(w); resp(q, w); }
-    } else {           // t_x t_y t_z t_rx t_ry t_rz t_r4
-      for (int q = 0; q < 6; q++) { limbs_from_be<8>(w, sc + 32 * q, 32); reduce_once<FpP256>(w); resp(q, w); }
-      ld<8>(w, jr + ((size_t)b * J + 3) * 8);
-      resp(6, w);
-    }
+    if (kind == 0) sigma_responses<3>(o, cc, dr, 0, w);
+    else sigma_responses<7>(o, cc, dr, 0, w);
     o.finish();
   }
 };
@@ -1302,22 +1206,13 @@ struct PaddSetupTask {
   const uint8_t* tape;      // [B][tape_stride] 38 draws
   size_t tape_stride;
   uint8_t* itape;           // [B][c.tape_stride]
-  ZK_HD bool parse(P256Aff& a, const uint8_t* pb) const {
-    uint32_t x[8], y[8];
-    limbs_from_be<8>(x, pb + 1, 32);
-    limbs_from_be<8>(y, pb + 33, 32);
-    reduce_once<FpP256>(x);
-    reduce_once<FpP256>(y);
-    P256p::to_mont(a.x, x);
-    P256p::to_mont(a.y, y);
-    return pb[0] == 0x04 && p256_on_curve(a.x, a.y);
-  }
   ZK_HD void operator()(int b) const {
     c.status[b] = ZKA_OK;
     P256Aff P, Q, R;
+    bool infP, infQ, infR;
     const uint8_t* pb = points + (size_t)b * 3 * 65;
-    const bool okP = parse(P, pb), okQ = parse(Q, pb + 65), okR = parse(R, pb + 130);
-    if (!okP || !okQ || !okR) {     // not on the curve, or an identity encoding: 'P/Q/R is at infinity' (pointAdd.ts:113-124)
+    const bool okP = p256_parse(P, infP, pb), okQ = p256_parse(Q, infQ, pb + 65), okR = p256_parse(R, infR, pb + 130);
+    if (!okP || !okQ || !okR || infP || infQ || infR) {   // not on the curve, or 'P/Q/R is at infinity' (pointAdd.ts:113-124)
       ZK_SET_STATUS(c.status + b, ZKA_ERR_INVALID_PK);
       p256_set_generator(P); p256_set_generator(Q); p256_set_generator(R);
     } else {

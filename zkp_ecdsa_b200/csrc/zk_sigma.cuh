@@ -4,8 +4,10 @@
 //   /root/reference/src/commit/mult.ts:93-175      MultProof: prove, aggregateMult (5 relations)
 //   /root/reference/src/exp/pointAdd.ts:92-259     PointAddProof: four MultProofs and two EqualityProofs
 //
-// One place each for: which commitments make up the statement of every sub-proof (the wiring), the five derived
-// commitments, the deserialisation checks of a proof body, and the relation folds of the verifiers.
+// One place each for: the point and scalar encodings (the proof group's and P-256's), which commitments make up the
+// statement of every sub-proof (the wiring), the five derived commitments, the prover steps of a MultProof and an
+// EqualityProof (openings and responses), the deserialisation checks of a proof body, and the relation folds of the
+// verifiers.
 #pragma once
 #include "zk_ops.cuh"
 
@@ -46,6 +48,27 @@ ZK_HD bool tom_parse(uint32_t* xm, uint32_t* ym, const uint8_t* b) {
 ZK_HD bool wscalar_parse(uint32_t* r, const uint8_t* b) {   // WS bytes (33 tomEdwards256 / 32 war256), mod the group order
   limbs_from_be<8>(r, b + (WS - 32), 32);
   return (WS == 32 || b[0] == 0) && lt_p<FpP256>(r);
+}
+// P-256 point encoding -> affine Montgomery; returns validity.  65 zero bytes are the identity: inf is set, a holds the
+// generator and the encoding counts as valid (each caller decides whether it accepts the identity).  Otherwise the tag
+// must be 0x04 and the point on the curve; as in weier.ts:74-89 a coordinate in [p, 2^256) stands for its residue.  An
+// invalid encoding leaves its reduced coordinates in a.
+ZK_HD bool p256_parse(P256Aff& a, bool& inf, const uint8_t* b) {
+  uint32_t x[8], y[8];
+  limbs_from_be<8>(x, b + 1, 32);
+  limbs_from_be<8>(y, b + 33, 32);
+  inf = (b[0] == 0) && is_zero_n<8>(x) && is_zero_n<8>(y);
+  if (inf) { p256_set_generator(a); return true; }
+  reduce_once<FpP256>(x);
+  reduce_once<FpP256>(y);
+  P256p::to_mont(a.x, x);
+  P256p::to_mont(a.y, y);
+  return b[0] == 0x04 && p256_on_curve(a.x, a.y);
+}
+// scalar encodings (group.ts:62-66 deserializeScalar: value < order)
+ZK_HD bool nscalar_parse(uint32_t* r, const uint8_t* b) {   // 32 bytes, mod p256.n
+  limbs_from_be<8>(r, b, 32);
+  return lt_p<FnP256>(r);
 }
 // a verifier draw (Relation.drain): 32 bytes below p256.n (nist) or the proof group's order
 ZK_HD bool vdraw(uint32_t* r, const uint8_t* p, bool nist) {
@@ -150,6 +173,64 @@ ZK_HD void point_add_expand(uint32_t (*in)[8], const uint32_t (*a)[8]) {
   F::sub(in[3], a[PA_CINTY], a[PA_C9]);                                   // C4: -C9 + Cint2
   copy_n<8>(in[4], a[PA_C9]);                                             // C5:  C9
   copy_n<8>(in[5], a[PA_CINTY]);                                          // C6:  Cint2
+}
+
+// ---- prover steps (mult.ts:93-131, equality.ts:60-78) --------------------------------------------------------------
+// Every point a sub-proof emits is a commitment whose opening the prover knows, so the openings are handed to
+// job(k, v, r) (canonical value and blinder of point k) for the fixed-base commitment kernel.  draw(q, r) yields the
+// sub-proof's draw q, canonical.  All mod q = tom.order.
+//
+// MultProof with statement x, y (Montgomery) and blinder ry of Cy (Montgomery): points C4 Ax Ay Az A4_1 A4_2, draws
+// k_x k_y k_z Ax.r Ay.r Az.r A4_1.r.  C4 = Cy*x = (x y) g + (x ry) h and A4_2 = Cy*k_x = (k_x y) g + (k_x ry) h
+// (mult.ts:103-114).  Leaves r4 = x ry (Montgomery), the secret of t_r4.
+template <class Job, class Draw>
+ZK_HD void mult_openings(const Job& job, const Draw& draw, const uint32_t* xm, const uint32_t* ym, const uint32_t* rym,
+                         uint32_t* r4) {
+  using F = Tomq;
+  uint32_t kx[8], ky[8], kz[8], mkx[8], ra[8], t[8], u[8];
+  draw(0, kx);
+  draw(1, ky);
+  draw(2, kz);
+  F::to_mont(mkx, kx);
+  F::mul(t, xm, ym); F::from_mont(t, t);
+  F::mul(r4, xm, rym); F::from_mont(u, r4);
+  job(0, t, u);
+  draw(3, ra); job(1, kx, ra);   // Ax, Ay, Az, A4_1 = commit(k_x), commit(k_y), commit(k_z), commit(k_z)
+  draw(4, ra); job(2, ky, ra);
+  draw(5, ra); job(3, kz, ra);
+  draw(6, ra); job(4, kz, ra);
+  F::mul(t, mkx, ym); F::from_mont(t, t);
+  F::mul(u, mkx, rym); F::from_mont(u, u);
+  job(5, t, u);
+}
+// EqualityProof: points A1 A2 = commit(k) under the blinders of draws 1 and 2, draws k A1.r A2.r
+template <class Job, class Draw>
+ZK_HD void equality_openings(const Job& job, const Draw& draw) {
+  uint32_t k[8], ra[8];
+  draw(0, k);
+  draw(1, ra); job(0, k, ra);
+  draw(2, ra); job(1, k, ra);
+}
+// response t = k - c*w  (mod q): k canonical, w Montgomery, c canonical 80-bit
+ZK_HD void response(uint32_t* t, const uint32_t* k_canon, const uint32_t* cc, const uint32_t* w_mont) {
+  using F = Tomq;
+  uint32_t cw[8];
+  F::mul(cw, cc, w_mont);   // c * (w R) / R = c*w, canonical
+  F::sub(t, k_canon, cw);
+}
+// the NQ responses of a sub-proof (7 for a MultProof: t_x t_y t_z t_rx t_ry t_rz t_r4; 3 for an EqualityProof: t_x t_r1
+// t_r2) to o: response q takes draw d0 + q of the tape row and the secret w(q, wm) (Montgomery).  cc: the challenge.
+template <int NQ, class W>
+ZK_HD void sigma_responses(ByteWriter& o, const uint32_t* cc, const uint8_t* row, int d0, const W& w) {
+#pragma unroll
+  for (int q = 0; q < NQ; q++) {
+    uint32_t k[8], wm[8], t[8];
+    tape_draw(k, row, d0 + q);
+    reduce_once<FpP256>(k);
+    w(q, wm);
+    response(t, k, cc, wm);
+    o.put_scalar<WS>(t);
+  }
 }
 
 // ---- deserialisation checks (deserializePoint / deserializeScalar would throw) --------------------------------------

@@ -139,26 +139,6 @@ struct VerifyCtx {
   ZK_HD size_t td_pt(size_t sample, int j) const { return sample * DERS_PER_ITEM + j; }
 };
 
-// ---- small helpers ------------------------------------------------------------------------
-// P-256 point encoding -> affine Montgomery. identity (65 zero bytes) -> inf.
-ZK_HD bool p256_parse(P256Aff& a, bool& inf, const uint8_t* b) {
-  uint32_t x[8], y[8];
-  limbs_from_be<8>(x, b + 1, 32);
-  limbs_from_be<8>(y, b + 33, 32);
-  inf = (b[0] == 0) && is_zero_n<8>(x) && is_zero_n<8>(y);
-  if (inf) { p256_set_generator(a); return true; }
-  reduce_once<FpP256>(x);
-  reduce_once<FpP256>(y);
-  P256p::to_mont(a.x, x);
-  P256p::to_mont(a.y, y);
-  return b[0] == 0x04 && p256_on_curve(a.x, a.y);
-}
-// scalar encodings (group.ts:62-66 deserializeScalar: value < order)
-ZK_HD bool nscalar_parse(uint32_t* r, const uint8_t* b) {   // 32 bytes, mod p256.n
-  limbs_from_be<8>(r, b, 32);
-  return lt_p<FnP256>(r);
-}
-
 // ---------------------------------------------------------------------------------------------
 // V1 — layout, statement (zkpAttestList.ts:153-164) and R/Q.  One thread per proof.
 // ---------------------------------------------------------------------------------------------

@@ -35,18 +35,10 @@ struct ParsePointsTask {   // host bytes -> affine Montgomery (+ validity), used
   uint8_t* inf;          // [count] (P-256 identity given as 65 zero bytes)
   ZK_HD void operator()(int t) const {
     if (nist) {
-      const uint8_t* b = nist + (size_t)t * 65;
-      uint32_t x[8], y[8];
-      limbs_from_be<8>(x, b + 1, 32);
-      limbs_from_be<8>(y, b + 33, 32);
-      bool allz = (b[0] == 0) && is_zero_n<8>(x) && is_zero_n<8>(y);
-      reduce_once<FpP256>(x);
-      reduce_once<FpP256>(y);
       P256Aff a;
-      P256p::to_mont(a.x, x);
-      P256p::to_mont(a.y, y);
-      bool ok = allz || (b[0] == 0x04 && p256_on_curve(a.x, a.y));
-      if (!ok || allz) p256_set_generator(a);
+      bool allz;
+      const bool ok = p256_parse(a, allz, nist + (size_t)t * 65);
+      if (!ok) p256_set_generator(a);
       p256_st_aff(nist_aff + (size_t)t * 16, a);
       if (bad) bad[t] = ok ? 0 : 1;
       if (inf) inf[t] = allz ? 1 : 0;
