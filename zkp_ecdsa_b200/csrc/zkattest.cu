@@ -637,38 +637,106 @@ const uint32_t* prep_ring(zka_ctx* ctx, Stream& st, const uint8_t* ring, uint32_
   return ring_m;
 }
 
-// One pass of a ring-set call: consecutive rows whose rings share the depth n.  A chunk's launch geometry (B n GK threads,
-// 4n + 1 GK scalars per proof, the verify tape layout, the seeded spans) assumes one n, so prove_impl / verify_impl run
-// each such run of rows as one call of their own, with the set in place of the one ring.
-struct RingPass {
-  const zka_rings* set;
-  const uint32_t* ring_of;   // the pass's rows (host or device)
-  int n;
-};
-// Rows [start[k], start[k + 1]) of a ring-set call form run k, of depth depth[k]; nmax is the largest depth used.
-struct RingRuns {
-  std::vector<uint32_t> start;
-  std::vector<int> depth;
-  int nmax = 0;
-};
-// ring_of is read on the host (4 bytes per row, copied when it is device memory) and checked against the set
-int ring_runs(zka_ctx* ctx, const zka_rings* set, const uint32_t* ring_of, uint32_t B, RingRuns& rr) {
-  std::vector<uint32_t> h(B);
-  if (is_device_ptr(ring_of)) {
-    copy_d2h(ctx->st, h.data(), ring_of, (size_t)B * 4);
-    sync(ctx->st);
-  } else {
-    memcpy(h.data(), ring_of, (size_t)B * 4);
+// The per-row arguments of a batched prove call (host or device), exactly one of tape / seeds set.  proveExp alone reads
+// base / s_in / q_in instead of msg_hash / sig / which; ring_of is set for a ring-set call.
+struct ProveRows {
+  const uint8_t *msg_hash{}, *sig{}, *pk{}, *base{}, *s_in{}, *q_in{}, *tape{}, *seeds{};
+  const uint32_t *which{}, *ring_of{};
+  size_t tape_stride{}, proof_stride{};
+  uint8_t* proofs{}; uint32_t* proof_len{}; int32_t* status{};
+  ProveRows() = default;
+  ProveRows(uint8_t* proofs, size_t stride, uint32_t* len, int32_t* status) : proof_stride(stride), proofs(proofs), proof_len(len), status(status) {}
+  // the rows from r0 on, null pointers left null (the one place that knows each row's width)
+  ProveRows at(size_t r0) const {
+    ProveRows v = *this;
+    auto skip = [r0](auto*& p, size_t width) { if (p) p += r0 * width; };
+    skip(v.msg_hash, 32); skip(v.sig, 64); skip(v.pk, 65); skip(v.which, 1); skip(v.ring_of, 1); skip(v.base, 65);
+    skip(v.s_in, 32); skip(v.q_in, 65); skip(v.seeds, 32); skip(v.tape, tape_stride);
+    skip(v.proofs, proof_stride); skip(v.proof_len, 1); skip(v.status, 1);
+    return v;
   }
-  for (uint32_t b = 0; b < B; b++)
-    if (h[b] >= set->R) return fail(ctx, ZKA_E_ARG, "ring_of[i] >= number of rings in the set");
-  for (uint32_t b = 0; b < B; b++) {
-    const int n = set->depth[h[b]];
-    if (b == 0 || n != rr.depth.back()) { rr.start.push_back(b); rr.depth.push_back(n); }
-    rr.nmax = std::max(rr.nmax, n);
+};
+// The same for a batched verify call; q_ext (verifyExp alone, device memory) holds each row's Q
+struct VerifyRows {
+  const uint8_t *msg_hash{}, *proofs{}, *tape{}, *seeds{}, *q_ext{};
+  const uint32_t *proof_len{}, *ring_of{};
+  size_t proof_stride{}, tape_stride{};
+  uint8_t* ok{}; int32_t* status{};
+  VerifyRows() = default;
+  VerifyRows(const uint8_t* proofs, size_t stride, const uint32_t* len, uint8_t* ok, int32_t* status)
+      : proofs(proofs), proof_len(len), proof_stride(stride), ok(ok), status(status) {}
+  VerifyRows at(size_t r0) const {
+    VerifyRows v = *this;
+    auto skip = [r0](auto*& p, size_t width) { if (p) p += r0 * width; };
+    skip(v.msg_hash, 32); skip(v.proofs, proof_stride); skip(v.proof_len, 1); skip(v.tape, tape_stride); skip(v.seeds, 32);
+    skip(v.ring_of, 1); skip(v.q_ext, NP); skip(v.ok, 1); skip(v.status, 1);
+    return v;
   }
-  rr.start.push_back(B);
-  return 0;
+};
+
+// Where the rows of a batched call find their ring: one ring of N keys for every row, or one pass of a set, whose rows
+// (ring_of) all have rings of depth n (a set call enters ring_passes as pass(set, 0)).  proveExp / verifyExp alone have
+// neither and keep N = 2.
+struct RingSrc {
+  const uint8_t* ring; uint32_t N;   // one ring, or
+  const zka_rings* set; int n;       // one pass of a set
+  static RingSrc one(const uint8_t* ring, uint32_t N) { return {ring, N, nullptr, ceil_log2(N)}; }
+  static RingSrc pass(const zka_rings* set, int n) { return {nullptr, 0, set, n}; }
+  static RingSrc none(int n) { return {nullptr, 2, nullptr, n}; }
+  // the call's ring on the device and, for the prover, the Lagrange matrix: once per call, done before the lanes start
+  const uint32_t* prepare(zka_ctx* ctx, bool lagrange) const {
+    if (!set && !ring) return nullptr;
+    const uint32_t* ring_m = set ? (const uint32_t*)set->ring_m.p : prep_ring(ctx, ctx->st, ring, N, n, lagrange);
+    if (set && lagrange) prep_lagrange(ctx, ctx->st, n);
+    if (!set || lagrange) sync(ctx->st);   // (the verifier's pass of a set queues nothing)
+    return ring_m;
+  }
+  // a chunk's ring fields; ring_of: the chunk's rows of it on the device
+  template <class Ctx>
+  void fill(Ctx& c, const uint32_t* ring_m, const uint32_t* ring_of) const {
+    c.ring_m = ring_m;
+    if (!set) return;
+    c.ring_of = ring_of;
+    c.ring_base = (const uint32_t*)set->ring_base.p;
+    if constexpr (std::is_same<Ctx, ProveCtx>::value) c.ring_size = (const uint32_t*)set->ring_size.p;
+  }
+};
+
+// A batched call after its null checks: its ring's checks, check(largest depth used), then pass(r0, count, ring) on rows
+// [r0, r0 + count): all B rows for one ring (or none), else each run of consecutive rows whose rings share a depth, as a
+// chunk's launch geometry (B n GK threads, 4n + 1 GK scalars per proof, the verify tape layout, the seeded spans) assumes
+// one n.  A set's ring_of is read on the host (4 bytes per row, copied when it is device memory).
+template <class Check, class Pass>
+int ring_passes(zka_ctx* ctx, const RingSrc& ring, const uint32_t* ring_of, uint32_t B, Check check, Pass pass) {
+  if (ring.set && ring.set->ctx != ctx) return fail(ctx, ZKA_E_ARG, "ring set of another context");
+  if (B == 0) return 0;
+  return guarded(ctx, [&] {
+    if (!ring.set) {
+      // N = 1 makes hashPoints([]) throw in the reference (group.ts:223 reduce of an empty array)
+      if (ring.N < 2 || ring.N > (1u << 20)) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
+      const int rc = check(ring.n);
+      return rc ? rc : pass(0u, B, ring);
+    }
+    std::vector<uint32_t> h(B), start;
+    if (is_device_ptr(ring_of)) {
+      copy_d2h(ctx->st, h.data(), ring_of, (size_t)B * 4);
+      sync(ctx->st);
+    } else {
+      memcpy(h.data(), ring_of, (size_t)B * 4);
+    }
+    const std::vector<int>& depth = ring.set->depth;
+    int nmax = 0;
+    for (uint32_t b = 0; b < B; b++) {
+      if (h[b] >= ring.set->R) return fail(ctx, ZKA_E_ARG, "ring_of[i] >= number of rings in the set");
+      if (b == 0 || depth[h[b]] != depth[h[b - 1]]) start.push_back(b);
+      nmax = std::max(nmax, depth[h[b]]);
+    }
+    start.push_back(B);
+    if (const int rc = check(nmax)) return rc;
+    for (size_t k = 0; k + 1 < start.size(); k++)
+      if (const int rc = pass(start[k], start[k + 1] - start[k], RingSrc::pass(ring.set, depth[h[start[k]]]))) return rc;
+    return 0;
+  });
 }
 
 int gk_blocks(int n) { return 1 << (n - gk_block_bits(n)); }   // ring blocks of the GK polynomial kernels
@@ -1233,294 +1301,282 @@ int zka_key_to_int(zka_ctx* ctx, uint32_t count, const uint8_t* pk, uint8_t* x_o
 
 // ------------------------------------------------------------------------------- prove
 // mode 0: proveSignatureList.  mode 1: proveExp alone (exp.ts:126-231) — base / s_in / q_in are the statement,
-// msg_hash / sig / which / ring are unused, the rows hold the repetitions only.
+// msg_hash / sig / which are unused, the rows hold the repetitions only.
 // seeds (B x 32, mode 0 only) instead of a tape: every lane expands its chunk's draws into its own tape buffer
 // (SeedProveTapeTask), the draws before the challenge first, the item and GK draws after the scan.
-// rp (mode 0 only) instead of (ring, N): one pass of a ring-set call, every row against its own ring of the set.
-static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
-                      const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* tape,
-                      size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out,
-                      int32_t* status, int mode, const uint8_t* base, const uint8_t* s_in, const uint8_t* q_in,
-                      const uint8_t* seeds = nullptr, const RingPass* rp = nullptr) {
-  if (!ctx || !P || !pk || (!tape && !seeds) || !proofs || !proof_len_out || !status) return ZKA_E_ARG;
-  if (mode == 0 && (!msg_hash || !sig || !which || (!ring && !rp))) return ZKA_E_ARG;
-  if (mode == 1 && (!base || !s_in)) return ZKA_E_ARG;
-  if (B == 0) return 0;
-  // N = 1 makes hashPoints([]) throw in the reference (group.ts:223 reduce of an empty array)
-  if (mode == 0 && !rp && (N < 2 || N > (1u << 20))) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
-  const int S = (int)P->sec_level;
-  const int n = rp ? rp->n : mode == 0 ? ceil_log2(N) : 0;
-  if (proof_stride < (mode == 0 ? (size_t)proof_len(S, n, S) : (size_t)S * REP0_LEN)) return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len");
-  const bool seeded = seeds != nullptr;
-  if (!seeded && tape_stride < (size_t)32 * (mode == 0 ? prove_draws(0, n, S) : draws_before_items(S))) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
+static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const ProveRows& rows, const RingSrc& ring, int mode) {
+  const int S = (int)P->sec_level, n = ring.n;
+  const bool seeded = rows.seeds != nullptr;
   // seeded: the library's tape rows hold every draw a proof can read (a multiple of 32 bytes, so 16-byte aligned rows)
   const int seed_draws = prove_draws(S, n, S);
-  return guarded(ctx, [&] {
-    // ring + Lagrange matrix: once per call, on lane 0, finished before the lanes start
-    const uint32_t* ring_m = nullptr;
-    if (rp) {
-      ring_m = (const uint32_t*)rp->set->ring_m.p;
-      prep_lagrange(ctx, ctx->st, n);
-      sync(ctx->st);
-    } else if (mode == 0) {
-      ring_m = prep_ring(ctx, ctx->st, ring, N, n, true);
-      sync(ctx->st);
-    }
-    const Output<uint8_t> po(proofs, proof_stride);
-    const Output<uint32_t> lo(proof_len_out, 1);
-    const Output<int32_t> so(status, 1);
-    const int lanes = ctx->nlanes;
-    const size_t dev_tape_stride = (tape_stride + 15) & ~(size_t)15;   // row pitch of a host tape staged on the device
-    const bool all_dev = po.dev && is_device_ptr(seeded ? seeds : tape);
-    const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)(all_dev ? ctx->chunk : std::min(ctx->chunk, ctx->host_chunk)), lanes, !all_dev);
-    const uint32_t nchunks = (uint32_t)off.size() - 1;
-    const int used = (int)std::min<uint32_t>((uint32_t)lanes, nchunks);
-    const bool trace = getenv("ZKA_TRACE") != nullptr;
-    const auto t_call = std::chrono::steady_clock::now();
-    auto ms_now = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call).count(); };
-    std::atomic<uint32_t> next_chunk((uint32_t)used);
-    // Every lane claims chunks from a shared counter (one ahead of the one it is computing, so that its inputs are
-    // already on their way).  Within a lane, chunks are software-pipelined over three streams when buffers live in
-    // host memory (staging buffers double-buffered by slot).
-    auto run_lane = [&](int li) {
-      Lane& ln = ctx->lane(li);
-      Stream& st = ln.st;
-      struct ChunkIn { const uint8_t *msg_hash, *sig, *pk, *tape, *base, *s_in, *q_in, *seeds; const uint32_t *which, *ring_of; } cin[2];
-      auto issue_inputs = [&](uint32_t k, int slot) {
-        const uint32_t b0 = off[k];
-        const size_t Bc = off[k + 1] - b0;
-        Stream& ci = ln.cs_in;
-        Cursor in(ln.in[slot]);
-        DevBuf& tape_buf = in.next();   // first, like the verifier's proof rows: the largest inputs share one buffer
-        auto rows = [&](auto* p, size_t width) { return stage_in(ci, in.next(), p ? p + b0 * width : p, Bc * width); };
-        ev_wait(ci, ln.ev_done[slot]);   // the chunk that used these staging buffers before has finished reading them
-        cin[slot].msg_hash = rows(msg_hash, 32);
-        cin[slot].sig = rows(sig, 64);
-        cin[slot].pk = rows(pk, 65);
-        cin[slot].which = rows(which, 1);
-        cin[slot].ring_of = rows(rp ? rp->ring_of : nullptr, 1);
-        cin[slot].base = rows(base, 65);
-        cin[slot].s_in = rows(s_in, 32);
-        cin[slot].q_in = rows(q_in, 65);
-        cin[slot].seeds = rows(seeds, 32);
-        ev_record(ln.ev_small[slot], ci);
-        if (seeded) {
-          // filled on the lane's stream by SeedProveTapeTask; nothing crosses PCIe
-          cin[slot].tape = tape_buf.get<uint8_t>(Bc * (size_t)32 * seed_draws);
-        } else if (is_device_ptr(tape)) {
-          cin[slot].tape = tape + (size_t)b0 * tape_stride;
-        } else if (!ctx->tape_split && dev_tape_stride == tape_stride) {
-          cin[slot].tape = stage_in(ci, tape_buf, tape + (size_t)b0 * tape_stride, Bc * tape_stride);
-        } else {
-          // host tape: staged at a row pitch of a multiple of 16 (dev_tape_stride), so that every draw is read with
-          // 16-byte loads whatever the caller's stride.  With tape_split only the draws used before the challenge
-          // (3 + 4S of up to 3 + 44S + 5n) travel now; the item and GK draws of each proof follow after the challenge,
-          // when their number is known
-          uint8_t* dt = tape_buf.get<uint8_t>(Bc * dev_tape_stride);
-          const size_t width = ctx->tape_split ? std::min(tape_stride, (size_t)32 * draws_before_items(S)) : tape_stride;
-          copy_d2h_2d(ci, dt, dev_tape_stride, tape + (size_t)b0 * tape_stride, tape_stride, width, Bc);
-          cin[slot].tape = dt;
-        }
-        ev_record(ln.ev_tape[slot], ci);
-      };
-      // the first `used` chunks are dealt statically (lane threads start at slightly different times); later ones are
-      // claimed from the shared counter at the mid-pipeline synchronisation point of the current chunk, when about
-      // half of its kernels are queued: early enough for the next inputs to travel behind them, late enough that a
-      // lane that started first does not grab the chunks of lanes that are still starting
-      uint32_t k = (uint32_t)li;
-      int slot = 0;
-      if (k < nchunks) issue_inputs(k, slot);
-      for (; k < nchunks; slot ^= 1) {
-        const uint32_t b0 = off[k];
-        const int Bc = (int)(off[k + 1] - b0);
-        const uint32_t k_this = k;
-        const double t_begin = ms_now();
-        ev_wait(st, ln.ev_small[slot]);
-        ev_wait(st, ln.ev_out[slot]);    // the proofs of chunk k-2 have left the output staging buffers
-        ProveCtx c = prove_ctx(ctx, P, Bc, S, (int)N, n);
-        c.mode = mode; c.head_len = mode == 0 ? HEAD_LEN : 0;
-        c.base = cin[slot].base; c.s_in = cin[slot].s_in; c.q_in = cin[slot].q_in;
-        c.msg_hash = cin[slot].msg_hash;
-        c.sig = cin[slot].sig;
-        c.pk = cin[slot].pk;
-        c.which = cin[slot].which;
-        c.tape = cin[slot].tape;
-        c.tape_stride = seeded ? (size_t)32 * seed_draws : is_device_ptr(tape) ? tape_stride : dev_tape_stride;
-        c.tape_draws = seeded ? (uint32_t)seed_draws : (uint32_t)(tape_stride / 32);
-        c.ring_m = ring_m;
-        if (rp) {
-          c.ring_of = cin[slot].ring_of;
-          c.ring_base = (const uint32_t*)rp->set->ring_base.p;
-          c.ring_size = (const uint32_t*)rp->set->ring_size.p;
-        }
-        const size_t S1 = (size_t)S + 1;
-        const size_t nA = (size_t)Bc * S1;
-        const size_t n1 = (size_t)Bc * (2 + 2 * S);
-        Cursor w(ln.w);
-        c.s1 = w.take<uint32_t>((size_t)Bc * 8);
-        c.pk_aff = w.take<uint32_t>((size_t)Bc * 16);
-        c.q_aff = w.take<uint32_t>((size_t)Bc * 16);
-        c.q_inf = w.take<uint8_t>(Bc);
-        c.r_aff = w.take<uint32_t>((size_t)Bc * 16);
-        c.r_bytes = w.take<uint8_t>((size_t)Bc * BSTRIDE);
-        c.rpows = w.take<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
-        c.rrows = w.take<uint32_t>((size_t)Bc * KEY_CAP * P256_PROJ_WORDS);
-        c.rtab = w.take<uint32_t>((size_t)Bc * KEY_CAP * P256_AFF_WORDS);
-        c.pa_T = w.take<uint32_t>(nA * P256_PROJ_WORDS);
-        c.pa_A = w.take<uint32_t>(nA * P256_PROJ_WORDS);
-        c.pa_T_aff = w.take<uint32_t>(nA * 16);
-        c.pa_T_inf = w.take<uint8_t>(nA);
-        c.pa_A_aff = w.take<uint32_t>(nA * 16);
-        c.pa_A_bytes = w.take<uint8_t>(nA * BSTRIDE);
-        c.pa_A_inf = w.take<uint8_t>(nA);
-        c.s1_jv = w.take<uint32_t>(n1 * 8);
-        c.s1_jr = w.take<uint32_t>(n1 * 8);
-        c.s1_proj = w.take<uint32_t>(n1 * TOM_E2_WORDS);
-        c.s1_aff = w.take<uint32_t>(n1 * TOM_AFF_WORDS);
-        c.s1_bytes = w.take<uint8_t>(n1 * BSTRIDE);
-        c.chal = w.take<uint32_t>((size_t)Bc * 3);
-        c.zcount = w.take<uint32_t>(Bc);
-        c.item_base = w.take<uint32_t>(Bc);
-        c.item_total = w.take<uint32_t>(2);
-        c.rep_off = w.take<uint32_t>((size_t)Bc * S);
-        c.gk_off = w.take<uint32_t>(Bc);
-        c.gk_dv = w.take<uint32_t>((size_t)Bc * n * 8);
-        c.gk_x = w.take<uint32_t>((size_t)Bc * 3);
-        c.u12 = w.take<uint32_t>((size_t)Bc * 16);
-        c.tab_of = w.take<uint32_t>(Bc);
-        c.tab_rep = w.take<uint32_t>((size_t)Bc * 2);
-        c.tab_count = w.take<uint32_t>(2);
-        c.which_s = w.take<uint32_t>(Bc);
-        uint32_t* base_aff = w.take_if<uint32_t>(mode == 1, (size_t)Bc * 16);
-        c.base_aff = mode == 0 ? c.pk_aff : base_aff;
-        c.proof_stride = proof_stride;
-        Cursor ob(ln.out[slot]);
-        c.proofs = po.rows(ob.next(), b0, Bc);
-        c.proof_len = lo.rows(ob.next(), b0, Bc);
-        c.status = so.rows(ob.next(), b0, Bc);
-  
-        // --- statement + per-proof tables of pk, then R = u1*G + u2*pk on the tables
-        launch(st, Bc, PreKeyTask{c});
-        // one table per DISTINCT key of the chunk (grids are sized for Bc tables, surplus threads return)
-        launch(st, Bc, KeyDedupTask{c});
-        launch(st, Bc, KeyRankTask{c});
-        launch(st, Bc, KeyAssignTask{c});
-        {
-          const int Bp = (Bc + 31) & ~31;
-          launch(st, (long long)Bp + Bc,
-                 PowsAndPreTask{P256PowsTask{c.base_aff, nullptr, c.rpows, Bc, RT_NWIN, RT_W, c.tab_rep, c.tab_count, c.tab_count + 1}, PreTask{c}, Bp});
-        }
-        // the window bits of these tables are chosen on the device from the number of distinct keys (tab_count[1]);
-        // grids are sized for the worst case, surplus threads return
-        // (one thread per (key, window, block of 16 entries): keys x windows x blocks <= Bc x KEY_CAP / 16 by the memory
-        // rule of key_window_bits, e.g. 0.2 Bc keys x 33 x 8 at w = 8 or Bc x 52 x 1 at w = 5)
-        launch(st, (long long)Bc * ((KEY_CAP + 15) / 16), P256RowsBlockTask{c.rpows, c.rrows, KEY_W_MIN, c.tab_count, c.tab_count + 1});
-        {
-          const long long np = (long long)Bc * KEY_CAP;
-          // points per thread from the EXPECTED table volume (at most min(N, Bc) distinct keys when every key is a member
-          // of the one ring; up to Bc with a ring set); the grid still covers the worst case
-          const uint32_t kest = rp ? (uint32_t)Bc : std::min<uint32_t>(N, (uint32_t)Bc);
-          const int west = key_window_bits(kest, (uint32_t)Bc, (uint32_t)S + 2);
-          const int ch = norm_chunk_for((long long)kest * fb_windows(west) * fb_entries(west), 5);
-          launch(st, (np + ch - 1) / ch, P256NormTask{c.rrows, c.rtab, nullptr, nullptr, (int)np, ch, c.tab_count, 0, c.tab_count + 1});
-        }
-        // --- phase A (first consumer of the tape) and R = u1*G + u2*pk side by side
-        ev_wait(st, ln.ev_tape[slot]);
-        if (seeded) {
-          const int d1 = draws_before_items(S);
-          launch(st, (long long)Bc * d1, SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, 0, d1, nullptr});
-        }
-        {
-          const int nAp = (int)((nA + 31) & ~(size_t)31);
-          launch(st, (long long)nAp + Bc, PhaseAAndRPointTask{PhaseAP256Task{c}, RPointTask{c}, (int)nA, nAp});
-        }
-        launch_p256_norm(st, c.pa_T, c.pa_T_aff, nullptr, c.pa_T_inf, (long long)(nA));
-        launch_p256_norm(st, c.pa_A, c.pa_A_aff, c.pa_A_bytes, c.pa_A_inf, (long long)(nA));
-        if (mode == 1) launch(st, Bc, ExpStatementTask{c});
-        prove_store1(st, c);
-        // --- challenge, layout
-        launch(st, Bc, ExpChallengeTask{c});
-        launch(st, 1, ScanTask{c});
-        uint32_t tot2[2] = {0, 0};
-        copy_d2h(st, tot2, c.item_total, 8);
-        const bool tape_host = !seeded && ctx->tape_split && !is_device_ptr(tape);
-        sync(st);
-        if (seeded) {
-          // the item and GK draws of each proof, up to the longest proof of the chunk (zmax = tot2[1])
-          const int d1 = draws_before_items(S), span = prove_draws((int)tot2[1], n, S) - d1;
-          launch(st, (long long)Bc * span, SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, d1, span, c.zcount});
-        } else if (tape_host) {
-          // second part of the tape: draws [3 + 4S, 3 + 4S + 40 zmax + 5n) of every row in one strided copy
-          // (zmax = the largest zero-bit count of the chunk)
-          const size_t o0 = (size_t)32 * draws_before_items(S);
-          const size_t o1 = std::min(tape_stride, (size_t)32 * prove_draws((int)tot2[1], n, S));
-          if (o1 > o0)
-            copy_d2h_2d(st, const_cast<uint8_t*>(c.tape) + o0, c.tape_stride, tape + (size_t)b0 * tape_stride + o0, tape_stride, o1 - o0, Bc);
-        }
-        const double t_mid = ms_now();
-        {
-          const uint32_t kn = next_chunk.fetch_add(1);
-          if (kn < nchunks) issue_inputs(kn, slot ^ 1);
-          k = kn;
-        }
-        const uint32_t M = tot2[0];
-        const size_t max_len = mode == 0 ? (size_t)proof_len((int)tot2[1], n, S)
-                                         : (size_t)tot2[1] * REP0_LEN + (size_t)(S - (int)tot2[1]) * REP1_LEN;
-        c.M = (int)M;
-        c.item_b = w.take<uint32_t>(M);
-        c.item_i = w.take<uint32_t>(M);
-        c.item_k = w.take<uint32_t>(M);
-        c.pb_T1 = w.take<uint32_t>((size_t)M * P256_PROJ_WORDS);
-        c.pb_T1_aff = w.take<uint32_t>((size_t)M * 16);
-        c.pb_T1_inf = w.take<uint8_t>(M);
-        const size_t n2 = c.s2_count();
-        c.s2_jv = w.take<uint32_t>(n2 * 8);
-        c.s2_jr = w.take<uint32_t>(n2 * 8);
-        c.s2_proj = w.take<uint32_t>(n2 * TOM_E2_WORDS);
-        c.s2_aff = w.take<uint32_t>(n2 * TOM_AFF_WORDS);
-        c.s2_bytes = w.take<uint8_t>(n2 * BSTRIDE);
-        c.secrets = w.take<uint32_t>((size_t)M * SECRETS_PER_ITEM * 8);
-        c.item_inv = w.take<uint32_t>((size_t)M * 8);
-        c.item_chal = w.take<uint32_t>((size_t)M * HASHES_PER_ITEM * 3);
-        c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * n * gk_blocks(n) * 8);
-        uint32_t* gext = w.take<uint32_t>((size_t)M * GJOBS_PER_ITEM * TOM_EXT_WORDS);
-        launch(st, Bc, ItemsTask{c});
-        // --- phase B
-        launch(st, M, PhaseBP256Task{c});
-        launch_p256_norm(st, c.pb_T1, c.pb_T1_aff, nullptr, c.pb_T1_inf, (long long)(M));
-        prove_items_gk(st, c, gext, true, true);
-        launch(st, (long long)nA, RepEmitTask{c});
-        if (mode == 0) launch(st, Bc, GkEmitTask{c});
-        launch(st, (long long)Bc * FIN_PARTS, FinalizeTask{c});
-        // --- results: on the output stream, behind this chunk's last kernel
-        ev_record(ln.ev_done[slot], st);
-        if (ctx->progress && !rp && k_this < ctx->progress_cap) notify_progress(st, ctx->progress + k_this);
-        if (!po.dev || !lo.dev || !so.dev) {
-          Stream& co = ln.cs_out;
-          ev_wait(co, ln.ev_done[slot]);
-          // only the bytes up to the longest proof of the chunk are copied back (rows are stride-padded)
-          // (one cudaMemcpyAsync per row with its exact length: 8192 driver calls per step cost more than
-          // the ~25 % of padding they save)
-          po.copy_back_2d(co, b0, c.proofs, Bc, max_len);
-          lo.copy_back(co, b0, c.proof_len, Bc);
-          so.copy_back(co, b0, c.status, Bc);
-          ev_record(ln.ev_out[slot], co);
-        }
-        if (trace) {
-          const double t_enq = ms_now();
-          sync(st);
-          const double t_comp = ms_now();
-          sync(ln.cs_out);
-          fprintf(stderr, "TRACE lane %d chunk %u rows %d begin %.2f mid %.2f enqueued %.2f computed %.2f copied %.2f\n", li, k_this, Bc,
-                  t_begin, t_mid, t_enq, t_comp, ms_now());
-        }
+  const uint32_t* ring_m = ring.prepare(ctx, true);
+  const Output<uint8_t> po(rows.proofs, rows.proof_stride);
+  const Output<uint32_t> lo(rows.proof_len, 1);
+  const Output<int32_t> so(rows.status, 1);
+  const int lanes = ctx->nlanes;
+  const size_t dev_tape_stride = (rows.tape_stride + 15) & ~(size_t)15;   // row pitch of a host tape staged on the device
+  const bool all_dev = po.dev && is_device_ptr(seeded ? rows.seeds : rows.tape);
+  const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)(all_dev ? ctx->chunk : std::min(ctx->chunk, ctx->host_chunk)), lanes, !all_dev);
+  const uint32_t nchunks = (uint32_t)off.size() - 1;
+  const int used = (int)std::min<uint32_t>((uint32_t)lanes, nchunks);
+  const bool trace = getenv("ZKA_TRACE") != nullptr;
+  const auto t_call = std::chrono::steady_clock::now();
+  auto ms_now = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call).count(); };
+  std::atomic<uint32_t> next_chunk((uint32_t)used);
+  // Every lane claims chunks from a shared counter (one ahead of the one it is computing, so that its inputs are
+  // already on their way).  Within a lane, chunks are software-pipelined over three streams when buffers live in
+  // host memory (staging buffers double-buffered by slot).
+  auto run_lane = [&](int li) {
+    Lane& ln = ctx->lane(li);
+    Stream& st = ln.st;
+    ProveRows cin[2];   // each slot's chunk, its inputs on the device
+    auto issue_inputs = [&](uint32_t k, int slot) {
+      // the chunk's rows of an input: from its first row to the next chunk's
+      const ProveRows r = rows.at(off[k]), e = rows.at(off[k + 1]);
+      const size_t Bc = off[k + 1] - off[k];
+      Stream& ci = ln.cs_in;
+      Cursor in(ln.in[slot]);
+      DevBuf& tape_buf = in.next();   // first, like the verifier's proof rows: the largest inputs share one buffer
+      auto stage = [&](auto* p, auto* end) { return stage_in(ci, in.next(), p, (size_t)(end - p)); };
+      ev_wait(ci, ln.ev_done[slot]);   // the chunk that used these staging buffers before has finished reading them
+      ProveRows& d = cin[slot];
+      d.msg_hash = stage(r.msg_hash, e.msg_hash);
+      d.sig = stage(r.sig, e.sig);
+      d.pk = stage(r.pk, e.pk);
+      d.which = stage(r.which, e.which);
+      d.ring_of = stage(r.ring_of, e.ring_of);
+      d.base = stage(r.base, e.base);
+      d.s_in = stage(r.s_in, e.s_in);
+      d.q_in = stage(r.q_in, e.q_in);
+      d.seeds = stage(r.seeds, e.seeds);
+      ev_record(ln.ev_small[slot], ci);
+      if (seeded) {
+        // filled on the lane's stream by SeedProveTapeTask; nothing crosses PCIe
+        d.tape = tape_buf.get<uint8_t>(Bc * (size_t)32 * seed_draws);
+      } else if (is_device_ptr(rows.tape)) {
+        d.tape = r.tape;
+      } else if (!ctx->tape_split && dev_tape_stride == rows.tape_stride) {
+        d.tape = stage_in(ci, tape_buf, r.tape, (size_t)(e.tape - r.tape));
+      } else {
+        // host tape: staged at a row pitch of a multiple of 16 (dev_tape_stride), so that every draw is read with
+        // 16-byte loads whatever the caller's stride.  With tape_split only the draws used before the challenge
+        // (3 + 4S of up to 3 + 44S + 5n) travel now; the item and GK draws of each proof follow after the challenge,
+        // when their number is known
+        uint8_t* dt = tape_buf.get<uint8_t>(Bc * dev_tape_stride);
+        const size_t width = ctx->tape_split ? std::min(rows.tape_stride, (size_t)32 * draws_before_items(S)) : rows.tape_stride;
+        copy_d2h_2d(ci, dt, dev_tape_stride, r.tape, rows.tape_stride, width, Bc);
+        d.tape = dt;
       }
-      sync(ln.cs_in);
-      sync(ln.cs_out);
-      sync(st);
+      ev_record(ln.ev_tape[slot], ci);
     };
-    run_lanes(ctx, used, run_lane);
+    // the first `used` chunks are dealt statically (lane threads start at slightly different times); later ones are
+    // claimed from the shared counter at the mid-pipeline synchronisation point of the current chunk, when about
+    // half of its kernels are queued: early enough for the next inputs to travel behind them, late enough that a
+    // lane that started first does not grab the chunks of lanes that are still starting
+    uint32_t k = (uint32_t)li;
+    int slot = 0;
+    if (k < nchunks) issue_inputs(k, slot);
+    for (; k < nchunks; slot ^= 1) {
+      const uint32_t b0 = off[k];
+      const int Bc = (int)(off[k + 1] - b0);
+      const uint32_t k_this = k;
+      const double t_begin = ms_now();
+      ev_wait(st, ln.ev_small[slot]);
+      ev_wait(st, ln.ev_out[slot]);    // the proofs of chunk k-2 have left the output staging buffers
+      ProveCtx c = prove_ctx(ctx, P, Bc, S, (int)ring.N, n);
+      c.mode = mode; c.head_len = mode == 0 ? HEAD_LEN : 0;
+      c.base = cin[slot].base; c.s_in = cin[slot].s_in; c.q_in = cin[slot].q_in;
+      c.msg_hash = cin[slot].msg_hash;
+      c.sig = cin[slot].sig;
+      c.pk = cin[slot].pk;
+      c.which = cin[slot].which;
+      c.tape = cin[slot].tape;
+      c.tape_stride = seeded ? (size_t)32 * seed_draws : is_device_ptr(rows.tape) ? rows.tape_stride : dev_tape_stride;
+      c.tape_draws = seeded ? (uint32_t)seed_draws : (uint32_t)(rows.tape_stride / 32);
+      ring.fill(c, ring_m, cin[slot].ring_of);
+      const size_t S1 = (size_t)S + 1;
+      const size_t nA = (size_t)Bc * S1;
+      const size_t n1 = (size_t)Bc * (2 + 2 * S);
+      Cursor w(ln.w);
+      c.s1 = w.take<uint32_t>((size_t)Bc * 8);
+      c.pk_aff = w.take<uint32_t>((size_t)Bc * 16);
+      c.q_aff = w.take<uint32_t>((size_t)Bc * 16);
+      c.q_inf = w.take<uint8_t>(Bc);
+      c.r_aff = w.take<uint32_t>((size_t)Bc * 16);
+      c.r_bytes = w.take<uint8_t>((size_t)Bc * BSTRIDE);
+      c.rpows = w.take<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
+      c.rrows = w.take<uint32_t>((size_t)Bc * KEY_CAP * P256_PROJ_WORDS);
+      c.rtab = w.take<uint32_t>((size_t)Bc * KEY_CAP * P256_AFF_WORDS);
+      c.pa_T = w.take<uint32_t>(nA * P256_PROJ_WORDS);
+      c.pa_A = w.take<uint32_t>(nA * P256_PROJ_WORDS);
+      c.pa_T_aff = w.take<uint32_t>(nA * 16);
+      c.pa_T_inf = w.take<uint8_t>(nA);
+      c.pa_A_aff = w.take<uint32_t>(nA * 16);
+      c.pa_A_bytes = w.take<uint8_t>(nA * BSTRIDE);
+      c.pa_A_inf = w.take<uint8_t>(nA);
+      c.s1_jv = w.take<uint32_t>(n1 * 8);
+      c.s1_jr = w.take<uint32_t>(n1 * 8);
+      c.s1_proj = w.take<uint32_t>(n1 * TOM_E2_WORDS);
+      c.s1_aff = w.take<uint32_t>(n1 * TOM_AFF_WORDS);
+      c.s1_bytes = w.take<uint8_t>(n1 * BSTRIDE);
+      c.chal = w.take<uint32_t>((size_t)Bc * 3);
+      c.zcount = w.take<uint32_t>(Bc);
+      c.item_base = w.take<uint32_t>(Bc);
+      c.item_total = w.take<uint32_t>(2);
+      c.rep_off = w.take<uint32_t>((size_t)Bc * S);
+      c.gk_off = w.take<uint32_t>(Bc);
+      c.gk_dv = w.take<uint32_t>((size_t)Bc * n * 8);
+      c.gk_x = w.take<uint32_t>((size_t)Bc * 3);
+      c.u12 = w.take<uint32_t>((size_t)Bc * 16);
+      c.tab_of = w.take<uint32_t>(Bc);
+      c.tab_rep = w.take<uint32_t>((size_t)Bc * 2);
+      c.tab_count = w.take<uint32_t>(2);
+      c.which_s = w.take<uint32_t>(Bc);
+      uint32_t* base_aff = w.take_if<uint32_t>(mode == 1, (size_t)Bc * 16);
+      c.base_aff = mode == 0 ? c.pk_aff : base_aff;
+      c.proof_stride = rows.proof_stride;
+      Cursor ob(ln.out[slot]);
+      c.proofs = po.rows(ob.next(), b0, Bc);
+      c.proof_len = lo.rows(ob.next(), b0, Bc);
+      c.status = so.rows(ob.next(), b0, Bc);
+
+      // --- statement + per-proof tables of pk, then R = u1*G + u2*pk on the tables
+      launch(st, Bc, PreKeyTask{c});
+      // one table per DISTINCT key of the chunk (grids are sized for Bc tables, surplus threads return)
+      launch(st, Bc, KeyDedupTask{c});
+      launch(st, Bc, KeyRankTask{c});
+      launch(st, Bc, KeyAssignTask{c});
+      {
+        const int Bp = (Bc + 31) & ~31;
+        launch(st, (long long)Bp + Bc,
+               PowsAndPreTask{P256PowsTask{c.base_aff, nullptr, c.rpows, Bc, RT_NWIN, RT_W, c.tab_rep, c.tab_count, c.tab_count + 1}, PreTask{c}, Bp});
+      }
+      // the window bits of these tables are chosen on the device from the number of distinct keys (tab_count[1]);
+      // grids are sized for the worst case, surplus threads return
+      // (one thread per (key, window, block of 16 entries): keys x windows x blocks <= Bc x KEY_CAP / 16 by the memory
+      // rule of key_window_bits, e.g. 0.2 Bc keys x 33 x 8 at w = 8 or Bc x 52 x 1 at w = 5)
+      launch(st, (long long)Bc * ((KEY_CAP + 15) / 16), P256RowsBlockTask{c.rpows, c.rrows, KEY_W_MIN, c.tab_count, c.tab_count + 1});
+      {
+        const long long np = (long long)Bc * KEY_CAP;
+        // points per thread from the EXPECTED table volume (at most min(N, Bc) distinct keys when every key is a member
+        // of the one ring; up to Bc with a ring set); the grid still covers the worst case
+        const uint32_t kest = ring.set ? (uint32_t)Bc : std::min<uint32_t>(ring.N, (uint32_t)Bc);
+        const int west = key_window_bits(kest, (uint32_t)Bc, (uint32_t)S + 2);
+        const int ch = norm_chunk_for((long long)kest * fb_windows(west) * fb_entries(west), 5);
+        launch(st, (np + ch - 1) / ch, P256NormTask{c.rrows, c.rtab, nullptr, nullptr, (int)np, ch, c.tab_count, 0, c.tab_count + 1});
+      }
+      // --- phase A (first consumer of the tape) and R = u1*G + u2*pk side by side
+      ev_wait(st, ln.ev_tape[slot]);
+      if (seeded) {
+        const int d1 = draws_before_items(S);
+        launch(st, (long long)Bc * d1, SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, 0, d1, nullptr});
+      }
+      {
+        const int nAp = (int)((nA + 31) & ~(size_t)31);
+        launch(st, (long long)nAp + Bc, PhaseAAndRPointTask{PhaseAP256Task{c}, RPointTask{c}, (int)nA, nAp});
+      }
+      launch_p256_norm(st, c.pa_T, c.pa_T_aff, nullptr, c.pa_T_inf, (long long)(nA));
+      launch_p256_norm(st, c.pa_A, c.pa_A_aff, c.pa_A_bytes, c.pa_A_inf, (long long)(nA));
+      if (mode == 1) launch(st, Bc, ExpStatementTask{c});
+      prove_store1(st, c);
+      // --- challenge, layout
+      launch(st, Bc, ExpChallengeTask{c});
+      launch(st, 1, ScanTask{c});
+      uint32_t tot2[2] = {0, 0};
+      copy_d2h(st, tot2, c.item_total, 8);
+      const bool tape_host = !seeded && ctx->tape_split && !is_device_ptr(rows.tape);
+      sync(st);
+      if (seeded) {
+        // the item and GK draws of each proof, up to the longest proof of the chunk (zmax = tot2[1])
+        const int d1 = draws_before_items(S), span = prove_draws((int)tot2[1], n, S) - d1;
+        launch(st, (long long)Bc * span, SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, d1, span, c.zcount});
+      } else if (tape_host) {
+        // second part of the tape: draws [3 + 4S, 3 + 4S + 40 zmax + 5n) of every row in one strided copy
+        // (zmax = the largest zero-bit count of the chunk)
+        const size_t o0 = (size_t)32 * draws_before_items(S);
+        const size_t o1 = std::min(rows.tape_stride, (size_t)32 * prove_draws((int)tot2[1], n, S));
+        if (o1 > o0)
+          copy_d2h_2d(st, const_cast<uint8_t*>(c.tape) + o0, c.tape_stride, rows.at(b0).tape + o0, rows.tape_stride, o1 - o0, Bc);
+      }
+      const double t_mid = ms_now();
+      {
+        const uint32_t kn = next_chunk.fetch_add(1);
+        if (kn < nchunks) issue_inputs(kn, slot ^ 1);
+        k = kn;
+      }
+      const uint32_t M = tot2[0];
+      const size_t max_len = mode == 0 ? (size_t)proof_len((int)tot2[1], n, S)
+                                       : (size_t)tot2[1] * REP0_LEN + (size_t)(S - (int)tot2[1]) * REP1_LEN;
+      c.M = (int)M;
+      c.item_b = w.take<uint32_t>(M);
+      c.item_i = w.take<uint32_t>(M);
+      c.item_k = w.take<uint32_t>(M);
+      c.pb_T1 = w.take<uint32_t>((size_t)M * P256_PROJ_WORDS);
+      c.pb_T1_aff = w.take<uint32_t>((size_t)M * 16);
+      c.pb_T1_inf = w.take<uint8_t>(M);
+      const size_t n2 = c.s2_count();
+      c.s2_jv = w.take<uint32_t>(n2 * 8);
+      c.s2_jr = w.take<uint32_t>(n2 * 8);
+      c.s2_proj = w.take<uint32_t>(n2 * TOM_E2_WORDS);
+      c.s2_aff = w.take<uint32_t>(n2 * TOM_AFF_WORDS);
+      c.s2_bytes = w.take<uint8_t>(n2 * BSTRIDE);
+      c.secrets = w.take<uint32_t>((size_t)M * SECRETS_PER_ITEM * 8);
+      c.item_inv = w.take<uint32_t>((size_t)M * 8);
+      c.item_chal = w.take<uint32_t>((size_t)M * HASHES_PER_ITEM * 3);
+      c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * n * gk_blocks(n) * 8);
+      uint32_t* gext = w.take<uint32_t>((size_t)M * GJOBS_PER_ITEM * TOM_EXT_WORDS);
+      launch(st, Bc, ItemsTask{c});
+      // --- phase B
+      launch(st, M, PhaseBP256Task{c});
+      launch_p256_norm(st, c.pb_T1, c.pb_T1_aff, nullptr, c.pb_T1_inf, (long long)(M));
+      prove_items_gk(st, c, gext, true, true);
+      launch(st, (long long)nA, RepEmitTask{c});
+      if (mode == 0) launch(st, Bc, GkEmitTask{c});
+      launch(st, (long long)Bc * FIN_PARTS, FinalizeTask{c});
+      // --- results: on the output stream, behind this chunk's last kernel
+      ev_record(ln.ev_done[slot], st);
+      if (ctx->progress && !ring.set && k_this < ctx->progress_cap) notify_progress(st, ctx->progress + k_this);
+      if (!po.dev || !lo.dev || !so.dev) {
+        Stream& co = ln.cs_out;
+        ev_wait(co, ln.ev_done[slot]);
+        // only the bytes up to the longest proof of the chunk are copied back (rows are stride-padded)
+        // (one cudaMemcpyAsync per row with its exact length: 8192 driver calls per step cost more than
+        // the ~25 % of padding they save)
+        po.copy_back_2d(co, b0, c.proofs, Bc, max_len);
+        lo.copy_back(co, b0, c.proof_len, Bc);
+        so.copy_back(co, b0, c.status, Bc);
+        ev_record(ln.ev_out[slot], co);
+      }
+      if (trace) {
+        const double t_enq = ms_now();
+        sync(st);
+        const double t_comp = ms_now();
+        sync(ln.cs_out);
+        fprintf(stderr, "TRACE lane %d chunk %u rows %d begin %.2f mid %.2f enqueued %.2f computed %.2f copied %.2f\n", li, k_this, Bc,
+                t_begin, t_mid, t_enq, t_comp, ms_now());
+      }
+    }
+    sync(ln.cs_in);
+    sync(ln.cs_out);
+    sync(st);
+  };
+  run_lanes(ctx, used, run_lane);
+  return 0;
+}
+
+// Every batched prove call: its argument checks (strides against the deepest ring used), then its prove_impl passes
+static int prove_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const ProveRows& rows, const RingSrc& ring, int mode) {
+  if (!ctx || !P || !rows.pk || (!rows.tape && !rows.seeds) || !rows.proofs || !rows.proof_len || !rows.status) return ZKA_E_ARG;
+  if (mode == 0 && (!rows.msg_hash || !rows.sig || !rows.which || !(ring.set ? (const void*)rows.ring_of : ring.ring))) return ZKA_E_ARG;
+  if (mode == 1 && (!rows.base || !rows.s_in)) return ZKA_E_ARG;
+  const int S = (int)P->sec_level;
+  auto check = [&](int n) {
+    if (rows.proof_stride < (mode == 0 ? (size_t)proof_len(S, n, S) : (size_t)S * REP0_LEN)) return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len");
+    if (rows.tape && rows.tape_stride < (size_t)32 * (mode == 0 ? prove_draws(0, n, S) : draws_before_items(S))) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
     return 0;
+  };
+  return ring_passes(ctx, ring, rows.ring_of, B, check, [&](uint32_t r0, uint32_t count, const RingSrc& pass) {
+    return prove_impl(ctx, P, count, rows.at(r0), pass, mode);
   });
 }
 
@@ -1528,61 +1584,33 @@ int zka_prove_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t
                     const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* tape,
                     size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out,
                     int32_t* status) {
-  return prove_impl(ctx, P, B, msg_hash, sig, pk, which, ring, N, tape, tape_stride, proofs, proof_stride, proof_len_out, status, 0,
-                    nullptr, nullptr, nullptr);
+  ProveRows r(proofs, proof_stride, proof_len_out, status);
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.tape = tape; r.tape_stride = tape_stride;
+  return prove_batch(ctx, P, B, r, RingSrc::one(ring, N), 0);
 }
 
 int zka_prove_batch_seeded(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
                            const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* seeds,
                            uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status) {
-  if (!seeds) return ZKA_E_ARG;
-  return prove_impl(ctx, P, B, msg_hash, sig, pk, which, ring, N, nullptr, 0, proofs, proof_stride, proof_len_out, status, 0,
-                    nullptr, nullptr, nullptr, seeds);
-}
-
-// Ring-set prover: every maximal run of consecutive rows whose rings share a depth is one prove_impl pass on offset
-// pointers (tape or seeds, one of them null)
-static int prove_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* set, const uint32_t* ring_of, uint32_t B,
-                       const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which, const uint8_t* tape,
-                       size_t tape_stride, const uint8_t* seeds, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out,
-                       int32_t* status) {
-  if (!ctx || !P || !set || !ring_of || !msg_hash || !sig || !pk || !which || (!tape && !seeds) || !proofs || !proof_len_out || !status)
-    return ZKA_E_ARG;
-  if (set->ctx != ctx) return fail(ctx, ZKA_E_ARG, "ring set of another context");
-  if (B == 0) return 0;
-  return guarded(ctx, [&] {
-    RingRuns rr;
-    if (const int rc = ring_runs(ctx, set, ring_of, B, rr)) return rc;
-    const int S = (int)P->sec_level;
-    if (proof_stride < (size_t)proof_len(S, rr.nmax, S)) return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len");
-    if (tape && tape_stride < (size_t)32 * prove_draws(0, rr.nmax, S)) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
-    for (size_t k = 0; k + 1 < rr.start.size(); k++) {
-      const uint32_t r0 = rr.start[k], rows = rr.start[k + 1] - r0;
-      const RingPass rp{set, ring_of + r0, rr.depth[k]};
-      const int rc = prove_impl(ctx, P, rows, msg_hash + (size_t)r0 * 32, sig + (size_t)r0 * 64, pk + (size_t)r0 * 65, which + r0,
-                                nullptr, 0, tape ? tape + (size_t)r0 * tape_stride : nullptr, tape_stride,
-                                proofs + (size_t)r0 * proof_stride, proof_stride, proof_len_out + r0, status + r0, 0, nullptr, nullptr,
-                                nullptr, seeds ? seeds + (size_t)r0 * 32 : nullptr, &rp);
-      if (rc) return rc;
-    }
-    return 0;
-  });
+  ProveRows r(proofs, proof_stride, proof_len_out, status);
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.seeds = seeds;
+  return prove_batch(ctx, P, B, r, RingSrc::one(ring, N), 0);
 }
 
 int zka_prove_batch_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
                           const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which, const uint8_t* tape,
                           size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status) {
-  if (!tape) return ZKA_E_ARG;
-  return prove_rings(ctx, P, rings, ring_of, B, msg_hash, sig, pk, which, tape, tape_stride, nullptr, proofs, proof_stride,
-                     proof_len_out, status);
+  ProveRows r(proofs, proof_stride, proof_len_out, status);
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.ring_of = ring_of; r.tape = tape; r.tape_stride = tape_stride;
+  return prove_batch(ctx, P, B, r, RingSrc::pass(rings, 0), 0);
 }
 
 int zka_prove_batch_rings_seeded(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
                                  const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which,
                                  const uint8_t* seeds, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status) {
-  if (!seeds) return ZKA_E_ARG;
-  return prove_rings(ctx, P, rings, ring_of, B, msg_hash, sig, pk, which, nullptr, 0, seeds, proofs, proof_stride, proof_len_out,
-                     status);
+  ProveRows r(proofs, proof_stride, proof_len_out, status);
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.ring_of = ring_of; r.seeds = seeds;
+  return prove_batch(ctx, P, B, r, RingSrc::pass(rings, 0), 0);
 }
 
 // The tape a seed stands for (the rule of zk_seed.cuh): kind 0 all prove_draws(S, n, S) prover draws, kind 1 the verify
@@ -1625,8 +1653,9 @@ int zka_seed_tape(zka_ctx* ctx, int kind, uint32_t B, const uint8_t* seeds, uint
 int zka_prove_exp_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* base, const uint8_t* s, const uint8_t* pk,
                         const uint8_t* q, const uint8_t* tape, size_t tape_stride, uint8_t* proofs, size_t proof_stride,
                         uint32_t* proof_len, int32_t* status) {
-  return prove_impl(ctx, P, B, nullptr, nullptr, pk, nullptr, nullptr, 2, tape, tape_stride, proofs, proof_stride, proof_len, status, 1,
-                    base, s, q);
+  ProveRows r(proofs, proof_stride, proof_len, status);
+  r.base = base; r.s_in = s; r.pk = pk; r.q_in = q; r.tape = tape; r.tape_stride = tape_stride;
+  return prove_batch(ctx, P, B, r, RingSrc::none(0), 1);
 }
 
 // proveMembership(params = ProofGroup, com, index, ring) (gk.ts:94-195) for B commitments over one ring.
@@ -1812,6 +1841,318 @@ size_t zka_verify_tape_len_ex(uint32_t ring_size, uint32_t sec_level, uint32_t s
   return verify_tape_len(ceil_log2(ring_size), (int)sec_level, (int)samples);
 }
 
+// mode 0: verifySignatureList; mode 1: verifyExp alone on assembled rows (msg_hash unused, Q from q_ext)
+// seeds (B x 32, mode 0 only) instead of a tape: SeedVerifyTapeTask expands each chunk's verify layout on the lane's stream
+static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const VerifyRows& rows, const RingSrc& ring,
+                       uint32_t samples, int mode) {
+  const int S = (int)P->sec_level, K = (int)samples, n = ring.n;
+  const bool seeded = rows.seeds != nullptr;
+  const size_t seed_stride = verify_tape_len(n, S, K);   // a multiple of 16
+  const uint32_t* ring_m = ring.prepare(ctx, false);
+  const Output<uint8_t> oo(rows.ok, 1);
+  const Output<int32_t> so(rows.status, 1);
+  const int lanes = ctx->nlanes;
+  const bool all_dev = is_device_ptr(rows.proofs) && is_device_ptr(seeded ? rows.seeds : rows.tape);
+  // (two equal chunks per lane instead of the tapered host schedule: no gain at batch 8192, slower at batch 1024)
+  const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)std::min(ctx->chunk, all_dev ? 4096 : std::min(4096, ctx->host_chunk)), lanes, !all_dev);
+  const uint32_t nchunks = (uint32_t)off.size() - 1;
+  const int used = (int)std::min<uint32_t>((uint32_t)lanes, nchunks);
+  std::atomic<uint32_t> next_chunk((uint32_t)used);
+  const bool trace = getenv("ZKA_TRACE") != nullptr;
+  const auto t_call = std::chrono::steady_clock::now();
+  auto ms_now = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call).count(); };
+  // every lane starts with chunk `li` and then claims chunks from a shared counter: copy-in, kernels and copy-out of a chunk are sequential on the
+  // lane's stream; the copies of one lane overlap the kernels of the others
+  // the inputs of a lane's NEXT chunk travel on the copy-in stream (second set of staging buffers) while the current
+  // chunk computes; a chunk's kernels wait for its event only
+  auto stage_chunk = [&](Lane& ln, int slot, uint32_t kk) {
+    // ONE copy-in stream for all lanes of the call: the chunks' inputs cross PCIe in the order they were queued, each at
+    // full bandwidth (with a copy stream per lane the first chunks and the prefetched ones were all in flight at once).
+    std::lock_guard<std::mutex> copy_lock(ctx->copy_mu);
+    Stream& ci = ctx->cs_in;
+    Cursor in(ln.in[slot]);
+    DevBuf& rows_buf = in.next();   // first, like the prover's tape: the largest inputs share one buffer
+    // the chunk's rows of an input: from its first row to the next chunk's (q_ext is device memory already)
+    const VerifyRows r = rows.at(off[kk]), e = rows.at(off[kk + 1]);
+    const size_t Bc = off[kk + 1] - off[kk], proof_stride = rows.proof_stride;
+    auto stage = [&](auto* p, auto* end) { return stage_in(ci, in.next(), p, (size_t)(end - p)); };
+    VerifyRows v = r;
+    v.msg_hash = stage(r.msg_hash, e.msg_hash);
+    if (is_device_ptr(rows.proofs) || is_device_ptr(rows.proof_len)) {
+      v.proofs = stage_in(ci, rows_buf, r.proofs, (size_t)(e.proofs - r.proofs));
+    } else {
+      // host rows: only the bytes up to the longest proof of the chunk cross PCIe (rows are stride-padded;
+      // a length above the stride is rejected by VLayoutTask without reading the row)
+      size_t w = 0;
+      for (size_t i = 0; i < Bc; i++) w = std::max<size_t>(w, r.proof_len[i]);
+      w = std::min(proof_stride, (w + 15) & ~(size_t)15);
+      uint8_t* dp = rows_buf.get<uint8_t>(Bc * proof_stride);
+      copy_d2h_2d(ci, dp, proof_stride, r.proofs, proof_stride, w, Bc);
+      v.proofs = dp;
+    }
+    v.proof_len = stage(r.proof_len, e.proof_len);
+    if (seeded) v.tape = in.next().get<uint8_t>(Bc * seed_stride);   // filled by SeedVerifyTapeTask
+    else v.tape = stage(r.tape, e.tape);
+    v.seeds = stage(r.seeds, e.seeds);
+    v.ring_of = stage(r.ring_of, e.ring_of);
+    ev_record(ln.ev_small[slot], ci);
+    return v;
+  };
+  // the first chunk of every lane is queued here, in chunk order, before any lane prefetches its second one (otherwise a
+  // lane queues its first chunk and its prefetch back to back, and another lane's first inputs land late)
+  std::vector<VerifyRows> first((size_t)used);
+  for (int li = 0; li < used; li++) first[(size_t)li] = stage_chunk(ctx->lane(li), 0, (uint32_t)li);
+  auto run_lane = [&](int li) {
+    Lane& ln = ctx->lane(li);
+    Stream& st = ln.st;
+    uint32_t k = (uint32_t)li;
+    if (k >= nchunks) return;
+    int slot = 0;
+    VerifyRows cur = first[(size_t)li];
+    for (;;) {
+    // claim the next chunk now and send its inputs on their way (the other slot's buffers were last read by the chunk
+    // before this one, which ended with a stream synchronisation)
+    const uint32_t kn = next_chunk.fetch_add(1);
+    VerifyRows nxt{};
+    if (kn < nchunks) nxt = stage_chunk(ln, slot ^ 1, kn);
+    ev_wait(st, ln.ev_small[slot]);
+    const uint32_t b0 = off[k];
+    const int Bc = (int)(off[k + 1] - b0);
+    const double t_begin = trace ? ms_now() : 0.0;
+    VerifyCtx c = verify_ctx(ctx, P, Bc, S, (int)ring.N, n, K, mode);
+    c.q_ext = cur.q_ext;
+    c.msg_hash = cur.msg_hash;
+    c.proofs = cur.proofs;
+    c.proof_stride = rows.proof_stride;
+    c.proof_len = cur.proof_len;
+    c.tape = cur.tape;
+    c.tape_stride = seeded ? seed_stride : rows.tape_stride;
+    ring.fill(c, ring_m, cur.ring_of);
+    if (seeded) {
+      const SeedVerifyTapeTask vt{cur.seeds, const_cast<uint8_t*>(cur.tape), seed_stride, n, S, K};
+      launch(st, (long long)Bc * vt.slots(), vt);
+    }
+    double t_in = 0.0;
+    if (trace) { sync(st); t_in = ms_now(); }
+    const size_t ns = (size_t)Bc * K;
+    const int ET = c.ent_tom(), EN = c.ent_nist(), SG = c.segs();
+    const int ngk = 4 * n + 1;
+    Cursor w(ln.w);
+    c.rep_off = w.take<uint32_t>((size_t)Bc * S);
+    c.gk_off = w.take<uint32_t>(Bc);
+    c.tagbits = w.take<uint32_t>((size_t)Bc * 3);
+    c.chal = w.take<uint32_t>((size_t)Bc * 3);
+    c.gk_ok_len = w.take<uint8_t>(Bc);
+    c.r_aff = w.take<uint32_t>((size_t)Bc * 16);
+    c.q_aff = w.take<uint32_t>((size_t)Bc * 16);
+    c.q_inf = w.take<uint8_t>(Bc);
+    c.rpows = w.take<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
+    c.rrows = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_PROJ_WORDS);
+    c.rtab = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_AFF_WORDS);
+    c.samp_idx = w.take<uint32_t>(ns);
+    c.samp_draw = w.take<uint32_t>(ns);
+    c.sp_T = w.take<uint32_t>(ns * P256_PROJ_WORDS);
+    c.sp_T_aff = w.take<uint32_t>(ns * 16);
+    c.sp_T_inf = w.take<uint8_t>(ns);
+    c.ta_jv = w.take<uint32_t>(ns * 2 * 8);
+    c.ta_jr = w.take<uint32_t>(ns * 2 * 8);
+    c.ta_proj = w.take<uint32_t>(ns * 2 * TOM_E2_WORDS);
+    c.ta_aff = w.take<uint32_t>(ns * 2 * TOM_AFF_WORDS);
+    c.td_proj = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_PROJ_WORDS);
+    c.td_aff = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_AFF_WORDS);
+    c.td_bytes = w.take<uint8_t>(ns * DERS_PER_ITEM * BSTRIDE);
+    c.item_chal = w.take<uint32_t>(ns * HASHES_PER_ITEM * 3);
+    c.ent_scalar = w.take<uint32_t>((size_t)Bc * ET * 8);
+    c.ent_off = w.take<uint32_t>((size_t)Bc * ET);
+    c.ent_pre = w.take<uint32_t>((size_t)Bc * ET * TOM_PRE_WORDS);
+    c.ent_cnt = w.take<uint32_t>(ns);
+    c.part = w.take<uint32_t>(ns * V_PART_WORDS);
+    // the small per-proof arrays before the entries and windows: the prover of this lane has small arrays at the
+    // same places of the pool, so these share its buffers without growing them much
+    c.fx_jv = w.take<uint32_t>((size_t)Bc * 2 * 8);
+    c.fx_jr = w.take<uint32_t>((size_t)Bc * 2 * 8);
+    c.fx_proj = w.take<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
+    c.nfix = w.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
+    c.id_flags = w.take<uint8_t>((size_t)Bc * 3);
+    c.gk_tape_bad = w.take_if<uint8_t>(mode == 0, Bc);
+    c.nent_scalar = w.take<uint32_t>((size_t)Bc * EN * 8);
+    c.nent_aff = w.take<uint32_t>((size_t)Bc * EN * 16);
+    c.nent_skip = w.take<uint8_t>((size_t)Bc * EN);
+    c.gk_scalar = w.take<uint32_t>((size_t)Bc * ngk * 8);
+    c.gk_pre = w.take<uint32_t>((size_t)Bc * ngk * TOM_PRE_WORDS);
+    uint32_t* gk_offs = w.take<uint32_t>((size_t)Bc * ngk);
+    c.win_w = w.take<uint32_t>((size_t)Bc * SG * MSM_NWIN * 36);
+    c.win_g = w.take<uint32_t>((size_t)Bc * MSM_NWIN * 36);
+    c.win_n = w.take<uint32_t>((size_t)Bc * MSM_NWIN_N * P256_PROJ_WORDS);
+    c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * gk_blocks(n) * 8);
+    Cursor ob(ln.out[0]);
+    c.ok = oo.rows(ob.next(), b0, Bc);
+    c.status = so.rows(ob.next(), b0, Bc);
+
+    launch(st, Bc, VLayoutTask{c});
+    launch(st, (long long)Bc * (S + 1), VValidateTask{c});
+    {
+      // the per-proof tables of R (a 255-doubling chain per proof, rows, normalisation: no status writes) run beside the
+      // Fiat-Shamir hash of the repetitions (one thread per proof, 16 KB) unless per-kernel profiling is on
+      const bool fork = !st.profiling;
+      Stream& sr = fork ? ln.aux[0] : st;
+      if (fork) { ev_record(ln.ev_fork, st); ev_wait(sr, ln.ev_fork); }
+      launch(sr, Bc, P256PowsTask{c.r_aff, nullptr, c.rpows, Bc, RT_NWIN, RT_W});
+      launch(sr, (long long)Bc * RT_NWIN, P256RowsSignedTask{c.rpows, c.rrows});
+      launch_p256_norm(sr, c.rrows, c.rtab, nullptr, nullptr, (long long)Bc * RT_ENTRIES);
+      launch(st, Bc, VChallengeTask{c});
+      if (fork) { ev_record(ln.ev_join[0], sr); ev_wait(st, ln.ev_join[0]); }
+    }
+    // the Groth-Kohlweiss chain (ring polynomial, relations, offsets) only needs the layout: it runs on a side stream
+    // beside the sampled-repetition chain; its tape-range status is folded in by VReduceTask (same precedence)
+    const bool gk_fork = mode == 0 && !st.profiling;
+    if (gk_fork) {
+      ev_record(ln.ev_fork, st);
+      ev_wait(ln.aux[1], ln.ev_fork);
+      verify_gk(ln.aux[1], c, gk_offs);
+      ev_record(ln.ev_join[1], ln.aux[1]);
+    }
+    launch(st, (long long)ns, VSampleP256Task{c});
+    launch_p256_norm(st, c.sp_T, c.sp_T_aff, nullptr, c.sp_T_inf, (long long)(ns));
+    launch(st, (long long)ns, VSampleJobsTask{c});
+    launch(st, (long long)ns * 2, TomCommitTask{c.ta_jv, c.ta_jr, c.tg_tab, c.th_tab, c.ta_proj, c.tom_w, c.tom_nwin});
+    launch_tom_norm(st, c.ta_proj, c.ta_aff, nullptr, (long long)(ns * 2), 1);
+    launch(st, (long long)ns, VDerivedTask{c});
+    launch_tom_norm(st, c.td_proj, nullptr, c.td_bytes, (long long)(ns * DERS_PER_ITEM), 0);
+    launch(st, (long long)ns * HASHES_PER_ITEM, VItemHashTask{c});
+    dev_memset(st, c.ent_off, 0, (size_t)Bc * ET * 4);
+    launch(st, (long long)ns, VRelationsTask{c});
+    if (mode == 0) {
+      if (gk_fork) ev_wait(st, ln.ev_join[1]);
+      else verify_gk(st, c, gk_offs);
+    }
+    launch(st, Bc, VReduceTask{c});
+    launch(st, (long long)Bc * ET, VParseEntriesTask{c.proofs, c.proof_stride, c.ent_off, c.ent_pre, ET});
+    if (mode == 0) launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, c.proof_stride, gk_offs, c.gk_pre, ngk});
+    launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin, 1});
+    // chunk-wide aggregate check (zk_verify_agg.cuh): the sum over all proofs of the chunk of the three linear
+    // combinations, as ONE wide-window MSM per group; when both sums are the identity the per-proof MSMs below
+    // return at once
+    uint32_t* ctl = nullptr;
+    if (ctx->agg && mode == 0) {
+      Cursor A(ln.agg);
+      const int fgroups = (Bc * 2 + 63) / 64, ngroups = (Bc + 31) / 32, ngroups2 = (ngroups + 31) / 32;
+      ctl = A.take<uint32_t>(AGG_CTL_WORDS);
+#if !defined(ZKA_PG_WAR256)
+      uint32_t* tpart = A.take<uint32_t>((size_t)Bc * (K + 1) * 2 * PG_EXT_WORDS);
+#endif
+      uint32_t* fpart = A.take<uint32_t>((size_t)fgroups * 16);
+      uint32_t* fjv = A.take<uint32_t>(8);
+      uint32_t* fjr = A.take<uint32_t>(8);
+      uint32_t* fproj = A.take<uint32_t>(TOM_PROJ_WORDS);
+      uint32_t* npart = A.take<uint32_t>((size_t)ngroups * P256_PROJ_WORDS);
+      uint32_t* npart2 = A.take_if<uint32_t>(ngroups > 32, (size_t)ngroups2 * P256_PROJ_WORDS);
+      dev_memset(st, ctl, 0, AGG_CTL_WORDS * 4);
+      launch(st, Bc, AggGateTask{c, ctl});
+      const AggTomSrc tsrc{c.ent_scalar, c.ent_pre, c.ent_cnt, c.gk_scalar, c.gk_pre, Bc, ET, K, ngk};
+      const AggNistSrc nsrc{c.nent_scalar, c.nent_aff, c.nent_skip, Bc, EN};
+      // three independent chains from here to AggFinalTask: the tomEdwards256 MSM (this stream), the torsion guard and the
+      // P-256 MSM with its fixed parts (two side streams; with per-kernel profiling on, everything stays on one stream
+      // so that the event pairs time one kernel at a time).  A skip flag raised by the torsion guard may reach the MSM
+      // kernels late — they then only do work AggFinalTask discards.
+      const bool fork = !st.profiling;
+      Stream& sa = fork ? ln.aux[0] : st;
+      Stream& sb = fork ? ln.aux[1] : st;
+      if (fork) {
+        ev_record(ln.ev_fork, st);
+        ev_wait(sa, ln.ev_fork);
+        ev_wait(sb, ln.ev_fork);
+      }
+#if !defined(ZKA_PG_WAR256)
+      // cofactor 4: no small-order components, or the per-proof path decides
+      launch(sa, (long long)Bc * (K + 1) * 2, AggTorsionPartTask{tsrc, ctl, tpart});
+      launch(sa, Bc, AggTorsionTask{tpart, ctl, K});
+#endif
+      const AggPlan tp = agg_plan((double)Bc * (0.5 * K * V_ENT_PER_SAMPLE + 2 + ngk), ctx->agg_c);
+      const AggPlan np = agg_plan((double)Bc * EN, 0);
+      ctx->agg_c_last = tp.D.c;
+      const uint32_t *tA, *tB, *nA, *nB;
+      agg_msm(st, Cursor(ln.agg_tom), tsrc, tp, ctl, &tA, &tB);
+      agg_msm(sb, Cursor(ln.agg_nist), nsrc, np, ctl, &nA, &nB);
+      // fixed-base parts: one commitment for the summed tomEdwards256 scalars, a two-level sum of the P-256 points
+      launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, fpart, Bc});
+      launch(st, 1, AggFixSumTask{ctl, fpart, fjv, fjr, fgroups});
+      launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom_w, c.tom_nwin, 1});
+      launch(sb, ngroups, AggNistFixPartTask{ctl, c.nfix, npart, Bc});
+      int nleft = ngroups;            // second level: at most Bc / 1024 partial sums reach the final thread
+      const uint32_t* nsum = npart;
+      if (nleft > 32) {
+        launch(sb, ngroups2, AggNistFixPartTask{ctl, npart, npart2, nleft});
+        nsum = npart2;
+        nleft = ngroups2;
+      }
+      if (fork) {
+        ev_record(ln.ev_join[0], sa);
+        ev_record(ln.ev_join[1], sb);
+        ev_wait(st, ln.ev_join[0]);
+        ev_wait(st, ln.ev_join[1]);
+      }
+      launch(st, 33, AggFinalTask{ctl, tA, tB, fproj, tp.D.nwin, tp.D.c, nA, nB, nsum, np.D.nwin, np.D.c, nleft});
+      c.agg_ctl = ctl;
+    }
+    {
+      const int nW = Bc * SG * MSM_NWIN, nWp = (nW + 31) & ~31, nG = Bc * MSM_NWIN;
+      launch(st, (long long)nWp + nG,
+             MsmTomWindowBothTask{MsmTomWindowTask{c.ent_scalar, c.ent_pre, c.ent_cnt, ET, K, V_ENT_PER_SAMPLE, 2, V_SEG, SG, c.win_w},
+                                  MsmTomWindowTask{c.gk_scalar, c.gk_pre, nullptr, ngk, 0, 0, mode == 0 ? ngk : 0, V_SEG, 1, c.win_g}, nW, nWp, nG, ctl});
+    }
+    launch(st, (long long)Bc * MSM_NWIN_N, MsmP256WindowTask{c.nent_scalar, c.nent_aff, c.nent_skip, c.win_n, EN, ctl});
+    {
+      const int Bp = (Bc + 31) & ~31;
+      launch(st, 3ll * Bp, MsmCombineAllTask{MsmTomCombineTask{c.win_g, c.fx_proj, c.id_flags, 2, 0, 0},
+                                             MsmTomCombineTask{c.win_w, c.fx_proj, c.id_flags, 2, 1, 1, SG},
+                                             MsmP256CombineTask{c.win_n, c.nfix, c.id_flags}, Bc, Bp, ctl});
+    }
+    launch(st, Bc, VFinalTask{c});
+    oo.copy_back(st, b0, c.ok, Bc);
+    so.copy_back(st, b0, c.status, Bc);
+    uint32_t hctl[AGG_CTL_WORDS] = {0, 0, 0, 0};
+    if (ctl) copy_d2h(st, hctl, ctl, sizeof(hctl));
+    const double t_enq = trace ? ms_now() : 0.0;
+    sync(st);
+    if (trace)
+      fprintf(stderr, "VTRACE lane %d chunk %u rows %d begin %.2f inputs_on_device %.2f enqueued %.2f done %.2f\n", li, k, Bc, t_begin, t_in,
+              t_enq, ms_now());
+    if (ctl) {
+      std::lock_guard<std::mutex> g(ctx->stat_mu);
+      if (hctl[AGG_TOM_PASS] && hctl[AGG_NIST_PASS]) ctx->agg_pass++;
+      else ctx->agg_fail++;
+    }
+    if (kn >= nchunks) break;
+    k = kn;
+    cur = nxt;
+    slot ^= 1;
+  }
+  };
+  run_lanes(ctx, used, run_lane);
+  sync(ctx->cs_in);
+  return 0;
+}
+
+// Every batched verify call: its argument checks (tape stride against the deepest ring used), then its verify_impl passes
+static int verify_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const VerifyRows& rows, const RingSrc& ring,
+                        uint32_t samples, int mode) {
+  if (!ctx || !P || !rows.proofs || !rows.proof_len || (!rows.tape && !rows.seeds) || !rows.ok || !rows.status) return ZKA_E_ARG;
+  if (mode == 0 && (!rows.msg_hash || !(ring.set ? (const void*)rows.ring_of : ring.ring))) return ZKA_E_ARG;
+  const int S = (int)P->sec_level, K = (int)samples;
+  auto check = [&](int n) {
+    if (K < 1) return fail(ctx, ZKA_E_ARG, "samples must be >= 1");
+    // verifyExp throws 'security level not achieved' when secparam > pi.length (exp.ts:243-245)
+    if (S < K) return fail(ctx, ZKA_E_ARG, "security level not achieved");
+    if (rows.tape && rows.tape_stride < (mode == 1 ? (size_t)V_IDX_PAD + (size_t)32 * 25 * K : verify_tape_len(n, S, K)))
+      return fail(ctx, ZKA_E_ARG, "tape_stride < zka_verify_tape_len");
+    return 0;
+  };
+  return ring_passes(ctx, ring, rows.ring_of, B, check, [&](uint32_t r0, uint32_t count, const RingSrc& pass) {
+    return verify_impl(ctx, P, count, rows.at(r0), pass, samples, mode);
+  });
+}
+
 int zka_verify_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                      uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                      const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status) {
@@ -1819,381 +2160,36 @@ int zka_verify_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_
   return zka_verify_batch_ex(ctx, P, B, msg_hash, ring, N, proofs, proof_stride, proof_len, tape, tape_stride, ok, status, V_SAMPLES);
 }
 
-static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
-                       uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
-                       const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples, int mode,
-                       const uint8_t* q_ext, const uint8_t* seeds = nullptr, const RingPass* rp = nullptr);
-
 int zka_verify_batch_ex(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                         uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                         const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples) {
-  if (!msg_hash || !ring) return ZKA_E_ARG;
-  return verify_impl(ctx, P, B, msg_hash, ring, N, proofs, proof_stride, proof_len, tape, tape_stride, ok, status, samples, 0, nullptr);
+  VerifyRows r(proofs, proof_stride, proof_len, ok, status);
+  r.msg_hash = msg_hash; r.tape = tape; r.tape_stride = tape_stride;
+  return verify_batch(ctx, P, B, r, RingSrc::one(ring, N), samples, 0);
 }
 
 int zka_verify_batch_seeded(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
                             uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                             const uint8_t* seeds, uint32_t samples, uint8_t* ok, int32_t* status) {
-  if (!msg_hash || !ring || !seeds) return ZKA_E_ARG;
-  return verify_impl(ctx, P, B, msg_hash, ring, N, proofs, proof_stride, proof_len, nullptr, 0, ok, status, samples, 0, nullptr, seeds);
-}
-
-// Ring-set verifier: one verify_impl pass per maximal run of rows whose rings share a depth (tape or seeds, one of them null)
-static int verify_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* set, const uint32_t* ring_of, uint32_t B,
-                        const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
-                        const uint8_t* tape, size_t tape_stride, const uint8_t* seeds, uint32_t samples, uint8_t* ok, int32_t* status) {
-  if (!ctx || !P || !set || !ring_of || !msg_hash || !proofs || !proof_len || (!tape && !seeds) || !ok || !status) return ZKA_E_ARG;
-  if (set->ctx != ctx) return fail(ctx, ZKA_E_ARG, "ring set of another context");
-  if (B == 0) return 0;
-  return guarded(ctx, [&] {
-    RingRuns rr;
-    if (const int rc = ring_runs(ctx, set, ring_of, B, rr)) return rc;
-    const int S = (int)P->sec_level, K = (int)samples;
-    if (K < 1) return fail(ctx, ZKA_E_ARG, "samples must be >= 1");
-    if (S < K) return fail(ctx, ZKA_E_ARG, "security level not achieved");
-    if (tape && tape_stride < verify_tape_len(rr.nmax, S, K)) return fail(ctx, ZKA_E_ARG, "tape_stride < zka_verify_tape_len");
-    for (size_t k = 0; k + 1 < rr.start.size(); k++) {
-      const uint32_t r0 = rr.start[k], rows = rr.start[k + 1] - r0;
-      const RingPass rp{set, ring_of + r0, rr.depth[k]};
-      const int rc = verify_impl(ctx, P, rows, msg_hash + (size_t)r0 * 32, nullptr, 0, proofs + (size_t)r0 * proof_stride, proof_stride,
-                                 proof_len + r0, tape ? tape + (size_t)r0 * tape_stride : nullptr, tape_stride, ok + r0, status + r0,
-                                 samples, 0, nullptr, seeds ? seeds + (size_t)r0 * 32 : nullptr, &rp);
-      if (rc) return rc;
-    }
-    return 0;
-  });
+  VerifyRows r(proofs, proof_stride, proof_len, ok, status);
+  r.msg_hash = msg_hash; r.seeds = seeds;
+  return verify_batch(ctx, P, B, r, RingSrc::one(ring, N), samples, 0);
 }
 
 int zka_verify_batch_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
                            const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                            const uint8_t* tape, size_t tape_stride, uint32_t samples, uint8_t* ok, int32_t* status) {
-  if (!tape) return ZKA_E_ARG;
-  return verify_rings(ctx, P, rings, ring_of, B, msg_hash, proofs, proof_stride, proof_len, tape, tape_stride, nullptr, samples, ok,
-                      status);
+  VerifyRows r(proofs, proof_stride, proof_len, ok, status);
+  r.msg_hash = msg_hash; r.ring_of = ring_of; r.tape = tape; r.tape_stride = tape_stride;
+  return verify_batch(ctx, P, B, r, RingSrc::pass(rings, 0), samples, 0);
 }
 
 int zka_verify_batch_rings_seeded(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
                                   const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
                                   const uint8_t* seeds, uint32_t samples, uint8_t* ok, int32_t* status) {
-  if (!seeds) return ZKA_E_ARG;
-  return verify_rings(ctx, P, rings, ring_of, B, msg_hash, proofs, proof_stride, proof_len, nullptr, 0, seeds, samples, ok, status);
-}
-
-// mode 0: verifySignatureList; mode 1: verifyExp alone on assembled rows (msg_hash / ring unused, Q from q_ext)
-// seeds (B x 32, mode 0 only) instead of a tape: SeedVerifyTapeTask expands each chunk's verify layout on the lane's stream
-// rp (mode 0 only) instead of (ring, N): one pass of a ring-set call, every row against its own ring of the set
-static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
-                       uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
-                       const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples, int mode,
-                       const uint8_t* q_ext, const uint8_t* seeds, const RingPass* rp) {
-  if (!ctx || !P || !proofs || !proof_len || (!tape && !seeds) || !ok || !status) return ZKA_E_ARG;
-  if (B == 0) return 0;
-  if (!rp && (N < 2 || N > (1u << 20))) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
-  const int S = (int)P->sec_level;
-  const int K = (int)samples;
-  if (K < 1) return fail(ctx, ZKA_E_ARG, "samples must be >= 1");
-  // verifyExp throws 'security level not achieved' when secparam > pi.length (exp.ts:243-245)
-  if (S < K) return fail(ctx, ZKA_E_ARG, "security level not achieved");
-  const int n = rp ? rp->n : ceil_log2(N);
-  const bool seeded = seeds != nullptr;
-  if (!seeded && tape_stride < (mode == 1 ? (size_t)V_IDX_PAD + (size_t)32 * 25 * K : verify_tape_len(n, S, K)))
-    return fail(ctx, ZKA_E_ARG, "tape_stride < zka_verify_tape_len");
-  const size_t seed_stride = verify_tape_len(n, S, K);   // a multiple of 16
-  return guarded(ctx, [&] {
-    const uint32_t* ring_m = nullptr;
-    if (rp) {
-      ring_m = (const uint32_t*)rp->set->ring_m.p;
-    } else if (mode == 0) {
-      ring_m = prep_ring(ctx, ctx->st, ring, N, n, false);
-      sync(ctx->st);
-    }
-    const Output<uint8_t> oo(ok, 1);
-    const Output<int32_t> so(status, 1);
-    const int lanes = ctx->nlanes;
-    const bool all_dev = is_device_ptr(proofs) && is_device_ptr(seeded ? seeds : tape);
-    // (two equal chunks per lane instead of the tapered host schedule: no gain at batch 8192, slower at batch 1024)
-    const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)std::min(ctx->chunk, all_dev ? 4096 : std::min(4096, ctx->host_chunk)), lanes, !all_dev);
-    const uint32_t nchunks = (uint32_t)off.size() - 1;
-    const int used = (int)std::min<uint32_t>((uint32_t)lanes, nchunks);
-    std::atomic<uint32_t> next_chunk((uint32_t)used);
-    const bool trace = getenv("ZKA_TRACE") != nullptr;
-    const auto t_call = std::chrono::steady_clock::now();
-    auto ms_now = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_call).count(); };
-    // every lane starts with chunk `li` and then claims chunks from a shared counter: copy-in, kernels and copy-out of a chunk are sequential on the
-    // lane's stream; the copies of one lane overlap the kernels of the others
-    // the inputs of a lane's NEXT chunk travel on the copy-in stream (second set of staging buffers) while the current
-    // chunk computes; a chunk's kernels wait for its event only
-    struct VIn { const uint8_t* msg; const uint8_t* proofs; const uint32_t* plen; const uint8_t* tape; const uint8_t* seeds; const uint32_t* ring_of; };
-    auto stage_chunk = [&](Lane& ln, int slot, uint32_t kk) {
-      // ONE copy-in stream for all lanes of the call: the chunks' inputs cross PCIe in the order they were queued, each at
-      // full bandwidth (with a copy stream per lane the first chunks and the prefetched ones were all in flight at once).
-      std::lock_guard<std::mutex> copy_lock(ctx->copy_mu);
-      Stream& ci = ctx->cs_in;
-      Cursor in(ln.in[slot]);
-      DevBuf& rows_buf = in.next();   // first, like the prover's tape: the largest inputs share one buffer
-      const uint32_t b0 = off[kk];
-      const size_t Bc = off[kk + 1] - b0;
-      VIn v;
-      v.msg = stage_in(ci, in.next(), msg_hash ? msg_hash + (size_t)b0 * 32 : nullptr, Bc * 32);
-      if (is_device_ptr(proofs) || is_device_ptr(proof_len)) {
-        v.proofs = stage_in(ci, rows_buf, proofs + (size_t)b0 * proof_stride, Bc * proof_stride);
-      } else {
-        // host rows: only the bytes up to the longest proof of the chunk cross PCIe (rows are stride-padded;
-        // a length above the stride is rejected by VLayoutTask without reading the row)
-        size_t w = 0;
-        for (size_t i = 0; i < Bc; i++) w = std::max<size_t>(w, proof_len[b0 + i]);
-        w = std::min(proof_stride, (w + 15) & ~(size_t)15);
-        uint8_t* dp = rows_buf.get<uint8_t>(Bc * proof_stride);
-        copy_d2h_2d(ci, dp, proof_stride, proofs + (size_t)b0 * proof_stride, proof_stride, w, Bc);
-        v.proofs = dp;
-      }
-      v.plen = stage_in(ci, in.next(), proof_len + b0, Bc);
-      if (seeded) v.tape = in.next().get<uint8_t>(Bc * seed_stride);   // filled by SeedVerifyTapeTask
-      else v.tape = stage_in(ci, in.next(), tape + (size_t)b0 * tape_stride, Bc * tape_stride);
-      v.seeds = stage_in(ci, in.next(), seeded ? seeds + (size_t)b0 * 32 : nullptr, Bc * 32);
-      v.ring_of = stage_in(ci, in.next(), rp ? rp->ring_of + b0 : nullptr, Bc);
-      ev_record(ln.ev_small[slot], ci);
-      return v;
-    };
-    // the first chunk of every lane is queued here, in chunk order, before any lane prefetches its second one (otherwise a
-    // lane queues its first chunk and its prefetch back to back, and another lane's first inputs land late)
-    std::vector<VIn> first((size_t)used);
-    for (int li = 0; li < used; li++) first[(size_t)li] = stage_chunk(ctx->lane(li), 0, (uint32_t)li);
-    auto run_lane = [&](int li) {
-      Lane& ln = ctx->lane(li);
-      Stream& st = ln.st;
-      uint32_t k = (uint32_t)li;
-      if (k >= nchunks) return;
-      int slot = 0;
-      VIn cur = first[(size_t)li];
-      for (;;) {
-      // claim the next chunk now and send its inputs on their way (the other slot's buffers were last read by the chunk
-      // before this one, which ended with a stream synchronisation)
-      const uint32_t kn = next_chunk.fetch_add(1);
-      VIn nxt{};
-      if (kn < nchunks) nxt = stage_chunk(ln, slot ^ 1, kn);
-      ev_wait(st, ln.ev_small[slot]);
-      const uint32_t b0 = off[k];
-      const int Bc = (int)(off[k + 1] - b0);
-      const double t_begin = trace ? ms_now() : 0.0;
-      VerifyCtx c = verify_ctx(ctx, P, Bc, S, (int)N, n, K, mode);
-      c.q_ext = q_ext ? q_ext + (size_t)b0 * NP : nullptr;
-      c.msg_hash = cur.msg;
-      c.proofs = cur.proofs;
-      c.proof_stride = proof_stride;
-      c.proof_len = cur.plen;
-      c.tape = cur.tape;
-      c.tape_stride = seeded ? seed_stride : tape_stride;
-      c.ring_m = ring_m;
-      if (rp) {
-        c.ring_of = cur.ring_of;
-        c.ring_base = (const uint32_t*)rp->set->ring_base.p;
-      }
-      if (seeded) {
-        const SeedVerifyTapeTask vt{cur.seeds, const_cast<uint8_t*>(cur.tape), seed_stride, n, S, K};
-        launch(st, (long long)Bc * vt.slots(), vt);
-      }
-      double t_in = 0.0;
-      if (trace) { sync(st); t_in = ms_now(); }
-      const size_t ns = (size_t)Bc * K;
-      const int ET = c.ent_tom(), EN = c.ent_nist(), SG = c.segs();
-      const int ngk = 4 * n + 1;
-      Cursor w(ln.w);
-      c.rep_off = w.take<uint32_t>((size_t)Bc * S);
-      c.gk_off = w.take<uint32_t>(Bc);
-      c.tagbits = w.take<uint32_t>((size_t)Bc * 3);
-      c.chal = w.take<uint32_t>((size_t)Bc * 3);
-      c.gk_ok_len = w.take<uint8_t>(Bc);
-      c.r_aff = w.take<uint32_t>((size_t)Bc * 16);
-      c.q_aff = w.take<uint32_t>((size_t)Bc * 16);
-      c.q_inf = w.take<uint8_t>(Bc);
-      c.rpows = w.take<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
-      c.rrows = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_PROJ_WORDS);
-      c.rtab = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_AFF_WORDS);
-      c.samp_idx = w.take<uint32_t>(ns);
-      c.samp_draw = w.take<uint32_t>(ns);
-      c.sp_T = w.take<uint32_t>(ns * P256_PROJ_WORDS);
-      c.sp_T_aff = w.take<uint32_t>(ns * 16);
-      c.sp_T_inf = w.take<uint8_t>(ns);
-      c.ta_jv = w.take<uint32_t>(ns * 2 * 8);
-      c.ta_jr = w.take<uint32_t>(ns * 2 * 8);
-      c.ta_proj = w.take<uint32_t>(ns * 2 * TOM_E2_WORDS);
-      c.ta_aff = w.take<uint32_t>(ns * 2 * TOM_AFF_WORDS);
-      c.td_proj = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_PROJ_WORDS);
-      c.td_aff = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_AFF_WORDS);
-      c.td_bytes = w.take<uint8_t>(ns * DERS_PER_ITEM * BSTRIDE);
-      c.item_chal = w.take<uint32_t>(ns * HASHES_PER_ITEM * 3);
-      c.ent_scalar = w.take<uint32_t>((size_t)Bc * ET * 8);
-      c.ent_off = w.take<uint32_t>((size_t)Bc * ET);
-      c.ent_pre = w.take<uint32_t>((size_t)Bc * ET * TOM_PRE_WORDS);
-      c.ent_cnt = w.take<uint32_t>(ns);
-      c.part = w.take<uint32_t>(ns * V_PART_WORDS);
-      // the small per-proof arrays before the entries and windows: the prover of this lane has small arrays at the
-      // same places of the pool, so these share its buffers without growing them much
-      c.fx_jv = w.take<uint32_t>((size_t)Bc * 2 * 8);
-      c.fx_jr = w.take<uint32_t>((size_t)Bc * 2 * 8);
-      c.fx_proj = w.take<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
-      c.nfix = w.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
-      c.id_flags = w.take<uint8_t>((size_t)Bc * 3);
-      c.gk_tape_bad = w.take_if<uint8_t>(mode == 0, Bc);
-      c.nent_scalar = w.take<uint32_t>((size_t)Bc * EN * 8);
-      c.nent_aff = w.take<uint32_t>((size_t)Bc * EN * 16);
-      c.nent_skip = w.take<uint8_t>((size_t)Bc * EN);
-      c.gk_scalar = w.take<uint32_t>((size_t)Bc * ngk * 8);
-      c.gk_pre = w.take<uint32_t>((size_t)Bc * ngk * TOM_PRE_WORDS);
-      uint32_t* gk_offs = w.take<uint32_t>((size_t)Bc * ngk);
-      c.win_w = w.take<uint32_t>((size_t)Bc * SG * MSM_NWIN * 36);
-      c.win_g = w.take<uint32_t>((size_t)Bc * MSM_NWIN * 36);
-      c.win_n = w.take<uint32_t>((size_t)Bc * MSM_NWIN_N * P256_PROJ_WORDS);
-      c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * gk_blocks(n) * 8);
-      Cursor ob(ln.out[0]);
-      c.ok = oo.rows(ob.next(), b0, Bc);
-      c.status = so.rows(ob.next(), b0, Bc);
-
-      launch(st, Bc, VLayoutTask{c});
-      launch(st, (long long)Bc * (S + 1), VValidateTask{c});
-      {
-        // the per-proof tables of R (a 255-doubling chain per proof, rows, normalisation: no status writes) run beside the
-        // Fiat-Shamir hash of the repetitions (one thread per proof, 16 KB) unless per-kernel profiling is on
-        const bool fork = !st.profiling;
-        Stream& sr = fork ? ln.aux[0] : st;
-        if (fork) { ev_record(ln.ev_fork, st); ev_wait(sr, ln.ev_fork); }
-        launch(sr, Bc, P256PowsTask{c.r_aff, nullptr, c.rpows, Bc, RT_NWIN, RT_W});
-        launch(sr, (long long)Bc * RT_NWIN, P256RowsSignedTask{c.rpows, c.rrows});
-        launch_p256_norm(sr, c.rrows, c.rtab, nullptr, nullptr, (long long)Bc * RT_ENTRIES);
-        launch(st, Bc, VChallengeTask{c});
-        if (fork) { ev_record(ln.ev_join[0], sr); ev_wait(st, ln.ev_join[0]); }
-      }
-      // the Groth-Kohlweiss chain (ring polynomial, relations, offsets) only needs the layout: it runs on a side stream
-      // beside the sampled-repetition chain; its tape-range status is folded in by VReduceTask (same precedence)
-      const bool gk_fork = mode == 0 && !st.profiling;
-      if (gk_fork) {
-        ev_record(ln.ev_fork, st);
-        ev_wait(ln.aux[1], ln.ev_fork);
-        verify_gk(ln.aux[1], c, gk_offs);
-        ev_record(ln.ev_join[1], ln.aux[1]);
-      }
-      launch(st, (long long)ns, VSampleP256Task{c});
-      launch_p256_norm(st, c.sp_T, c.sp_T_aff, nullptr, c.sp_T_inf, (long long)(ns));
-      launch(st, (long long)ns, VSampleJobsTask{c});
-      launch(st, (long long)ns * 2, TomCommitTask{c.ta_jv, c.ta_jr, c.tg_tab, c.th_tab, c.ta_proj, c.tom_w, c.tom_nwin});
-      launch_tom_norm(st, c.ta_proj, c.ta_aff, nullptr, (long long)(ns * 2), 1);
-      launch(st, (long long)ns, VDerivedTask{c});
-      launch_tom_norm(st, c.td_proj, nullptr, c.td_bytes, (long long)(ns * DERS_PER_ITEM), 0);
-      launch(st, (long long)ns * HASHES_PER_ITEM, VItemHashTask{c});
-      dev_memset(st, c.ent_off, 0, (size_t)Bc * ET * 4);
-      launch(st, (long long)ns, VRelationsTask{c});
-      if (mode == 0) {
-        if (gk_fork) ev_wait(st, ln.ev_join[1]);
-        else verify_gk(st, c, gk_offs);
-      }
-      launch(st, Bc, VReduceTask{c});
-      launch(st, (long long)Bc * ET, VParseEntriesTask{c.proofs, proof_stride, c.ent_off, c.ent_pre, ET});
-      if (mode == 0) launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, proof_stride, gk_offs, c.gk_pre, ngk});
-      launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin, 1});
-      // chunk-wide aggregate check (zk_verify_agg.cuh): the sum over all proofs of the chunk of the three linear
-      // combinations, as ONE wide-window MSM per group; when both sums are the identity the per-proof MSMs below
-      // return at once
-      uint32_t* ctl = nullptr;
-      if (ctx->agg && mode == 0) {
-        Cursor A(ln.agg);
-        const int fgroups = (Bc * 2 + 63) / 64, ngroups = (Bc + 31) / 32, ngroups2 = (ngroups + 31) / 32;
-        ctl = A.take<uint32_t>(AGG_CTL_WORDS);
-#if !defined(ZKA_PG_WAR256)
-        uint32_t* tpart = A.take<uint32_t>((size_t)Bc * (K + 1) * 2 * PG_EXT_WORDS);
-#endif
-        uint32_t* fpart = A.take<uint32_t>((size_t)fgroups * 16);
-        uint32_t* fjv = A.take<uint32_t>(8);
-        uint32_t* fjr = A.take<uint32_t>(8);
-        uint32_t* fproj = A.take<uint32_t>(TOM_PROJ_WORDS);
-        uint32_t* npart = A.take<uint32_t>((size_t)ngroups * P256_PROJ_WORDS);
-        uint32_t* npart2 = A.take_if<uint32_t>(ngroups > 32, (size_t)ngroups2 * P256_PROJ_WORDS);
-        dev_memset(st, ctl, 0, AGG_CTL_WORDS * 4);
-        launch(st, Bc, AggGateTask{c, ctl});
-        const AggTomSrc tsrc{c.ent_scalar, c.ent_pre, c.ent_cnt, c.gk_scalar, c.gk_pre, Bc, ET, K, ngk};
-        const AggNistSrc nsrc{c.nent_scalar, c.nent_aff, c.nent_skip, Bc, EN};
-        // three independent chains from here to AggFinalTask: the tomEdwards256 MSM (this stream), the torsion guard and the
-        // P-256 MSM with its fixed parts (two side streams; with per-kernel profiling on, everything stays on one stream
-        // so that the event pairs time one kernel at a time).  A skip flag raised by the torsion guard may reach the MSM
-        // kernels late — they then only do work AggFinalTask discards.
-        const bool fork = !st.profiling;
-        Stream& sa = fork ? ln.aux[0] : st;
-        Stream& sb = fork ? ln.aux[1] : st;
-        if (fork) {
-          ev_record(ln.ev_fork, st);
-          ev_wait(sa, ln.ev_fork);
-          ev_wait(sb, ln.ev_fork);
-        }
-#if !defined(ZKA_PG_WAR256)
-        // cofactor 4: no small-order components, or the per-proof path decides
-        launch(sa, (long long)Bc * (K + 1) * 2, AggTorsionPartTask{tsrc, ctl, tpart});
-        launch(sa, Bc, AggTorsionTask{tpart, ctl, K});
-#endif
-        const AggPlan tp = agg_plan((double)Bc * (0.5 * K * V_ENT_PER_SAMPLE + 2 + ngk), ctx->agg_c);
-        const AggPlan np = agg_plan((double)Bc * EN, 0);
-        ctx->agg_c_last = tp.D.c;
-        const uint32_t *tA, *tB, *nA, *nB;
-        agg_msm(st, Cursor(ln.agg_tom), tsrc, tp, ctl, &tA, &tB);
-        agg_msm(sb, Cursor(ln.agg_nist), nsrc, np, ctl, &nA, &nB);
-        // fixed-base parts: one commitment for the summed tomEdwards256 scalars, a two-level sum of the P-256 points
-        launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, fpart, Bc});
-        launch(st, 1, AggFixSumTask{ctl, fpart, fjv, fjr, fgroups});
-        launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom_w, c.tom_nwin, 1});
-        launch(sb, ngroups, AggNistFixPartTask{ctl, c.nfix, npart, Bc});
-        int nleft = ngroups;            // second level: at most Bc / 1024 partial sums reach the final thread
-        const uint32_t* nsum = npart;
-        if (nleft > 32) {
-          launch(sb, ngroups2, AggNistFixPartTask{ctl, npart, npart2, nleft});
-          nsum = npart2;
-          nleft = ngroups2;
-        }
-        if (fork) {
-          ev_record(ln.ev_join[0], sa);
-          ev_record(ln.ev_join[1], sb);
-          ev_wait(st, ln.ev_join[0]);
-          ev_wait(st, ln.ev_join[1]);
-        }
-        launch(st, 33, AggFinalTask{ctl, tA, tB, fproj, tp.D.nwin, tp.D.c, nA, nB, nsum, np.D.nwin, np.D.c, nleft});
-        c.agg_ctl = ctl;
-      }
-      {
-        const int nW = Bc * SG * MSM_NWIN, nWp = (nW + 31) & ~31, nG = Bc * MSM_NWIN;
-        launch(st, (long long)nWp + nG,
-               MsmTomWindowBothTask{MsmTomWindowTask{c.ent_scalar, c.ent_pre, c.ent_cnt, ET, K, V_ENT_PER_SAMPLE, 2, V_SEG, SG, c.win_w},
-                                    MsmTomWindowTask{c.gk_scalar, c.gk_pre, nullptr, ngk, 0, 0, mode == 0 ? ngk : 0, V_SEG, 1, c.win_g}, nW, nWp, nG, ctl});
-      }
-      launch(st, (long long)Bc * MSM_NWIN_N, MsmP256WindowTask{c.nent_scalar, c.nent_aff, c.nent_skip, c.win_n, EN, ctl});
-      {
-        const int Bp = (Bc + 31) & ~31;
-        launch(st, 3ll * Bp, MsmCombineAllTask{MsmTomCombineTask{c.win_g, c.fx_proj, c.id_flags, 2, 0, 0},
-                                               MsmTomCombineTask{c.win_w, c.fx_proj, c.id_flags, 2, 1, 1, SG},
-                                               MsmP256CombineTask{c.win_n, c.nfix, c.id_flags}, Bc, Bp, ctl});
-      }
-      launch(st, Bc, VFinalTask{c});
-      oo.copy_back(st, b0, c.ok, Bc);
-      so.copy_back(st, b0, c.status, Bc);
-      uint32_t hctl[AGG_CTL_WORDS] = {0, 0, 0, 0};
-      if (ctl) copy_d2h(st, hctl, ctl, sizeof(hctl));
-      const double t_enq = trace ? ms_now() : 0.0;
-      sync(st);
-      if (trace)
-        fprintf(stderr, "VTRACE lane %d chunk %u rows %d begin %.2f inputs_on_device %.2f enqueued %.2f done %.2f\n", li, k, Bc, t_begin, t_in,
-                t_enq, ms_now());
-      if (ctl) {
-        std::lock_guard<std::mutex> g(ctx->stat_mu);
-        if (hctl[AGG_TOM_PASS] && hctl[AGG_NIST_PASS]) ctx->agg_pass++;
-        else ctx->agg_fail++;
-      }
-      if (kn >= nchunks) break;
-      k = kn;
-      cur = nxt;
-      slot ^= 1;
-    }
-    };
-    run_lanes(ctx, used, run_lane);
-    sync(ctx->cs_in);
-    return 0;
-  });
+  VerifyRows r(proofs, proof_stride, proof_len, ok, status);
+  r.msg_hash = msg_hash; r.ring_of = ring_of; r.seeds = seeds;
+  return verify_batch(ctx, P, B, r, RingSrc::pass(rings, 0), samples, 0);
 }
 
 // ------------------------------------------------------------------ stand-alone sub-proof verifiers
@@ -2207,7 +2203,7 @@ int zka_verify_exp_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const ui
   if (B == 0) return 0;
   return guarded(ctx, [&] {
     Stream& st = ctx->st;
-    DevBuf bufs[10];   // not the lane's staging buffers: verify_impl stages through those
+    DevBuf bufs[10];   // not the lane's staging buffers: verify_batch stages through those
     Cursor in(bufs);
     const uint8_t* d_base = stage_in(st, in.next(), base, (size_t)B * NP);
     const uint8_t* d_com = stage_in(st, in.next(), com, (size_t)B * NP);
@@ -2223,7 +2219,10 @@ int zka_verify_exp_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const ui
     const int pieces = (int)((row_stride + 63) / 64);
     launch(st, (long long)B * pieces, VAssembleTask{d_base, d_com, d_px, d_py, d_body, proof_stride, d_len, d_rows, row_stride, d_rlen, pieces});
     sync(st);
-    return verify_impl(ctx, P, B, nullptr, nullptr, 2, d_rows, row_stride, d_rlen, d_tape, tape_stride, ok, status, samples, 1, d_q);
+    VerifyRows r(d_rows, row_stride, d_rlen, ok, status);
+    r.tape = d_tape; r.tape_stride = tape_stride; r.q_ext = d_q;
+    // n = 1 sizes GK workspace (ngk = 4n + 1) that mode 1 never fills, keeping the lane pools' layout as it has been
+    return verify_batch(ctx, P, B, r, RingSrc::none(1), samples, 1);
   });
 }
 
