@@ -192,9 +192,10 @@ int zka_seed_tape(zka_ctx* ctx, int kind, uint32_t B, const uint8_t* seeds, uint
  *     must cover the largest ring the call uses (zka_prove_tape_len, zka_verify_tape_len_ex, zka_proof_max_len of it).
  *   - which[i] >= N_r gives the row status ZKA_ERR_BAD_INDEX, also inside the padding (N_r = 5, which = 6).
  *   - Any ring_of[i] >= R: the call returns ZKA_E_ARG before any work.
- *   - The call runs each maximal run of consecutive rows whose rings share a depth as one pass of the batched pipeline.
- *     Rows in any order give the same bytes; rows grouped by depth are fast (interleaved depths make many small passes).
- *   - zka_set_progress flags are not written by these calls. */
+ *   - The call is ONE pass of the batched pipeline whatever the order of ring depths in ring_of: its chunks are laid out for
+ *     the largest depth the rows use and every row follows its own.  Rows in any order give the same bytes, and need no
+ *     sorting or grouping to be fast.
+ *   - The chunk schedule and the zka_set_progress flags are those of the one-ring call over the same B (zka_chunk_schedule). */
 int zka_rings_create(zka_ctx* ctx, uint32_t R, const uint32_t* sizes /* R */, const uint8_t* keys /* sum(sizes) x 32 */,
                      zka_rings** out);
 void zka_rings_destroy(zka_rings* rings);

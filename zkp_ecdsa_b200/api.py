@@ -273,7 +273,8 @@ class Engine:
         return RingSet(self.lib.rings_create(sizes, keys), self.lib, [int(s) for s in sizes])
 
     def prove_batch_rings(self, params, rings: RingSet, ring_of, msg_hash, sig, pk, which, tape, proofs=None) -> ProveResult:
-        """prove_batch with row i against ring ring_of[i] of `rings`; tape rows as wide as the largest ring used needs."""
+        """prove_batch with row i against ring ring_of[i] of `rings`; tape rows as wide as the largest ring used needs.
+        Rows go in any order (rings.depths need not be grouped): the call is one pass of the pipeline."""
         B = msg_hash.shape[0]
         ring_of = np.ascontiguousarray(ring_of, np.uint32)
         stride = self.lib.proof_max_len(rings.largest(ring_of), params.sec_level)

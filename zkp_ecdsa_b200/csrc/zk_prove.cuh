@@ -27,7 +27,8 @@ struct ProveCtx {
   int B;        // proofs in this chunk
   int S;        // repetitions (SecLevel, <= 80)
   int N;        // ring size
-  int n;        // ceil(log2 N)
+  int n;        // the depth the chunk is laid out for (grids, workspace strides, slots per proof): ceil(log2 N), with a
+                //    ring set the largest depth the call uses; the depth of row b's own ring is n_row(b)
   int M;        // total 0-bit repetitions (items) in the chunk (valid after the scan)
   int tom_w, tom_nwin;
   int mode;                  // 0: proveSignatureList; 1: proveExp alone (exp.ts:126-231): R = `base`, s and Q are inputs,
@@ -50,7 +51,8 @@ struct ProveCtx {
                              //    ring of the set (zka_rings), ring r at entry ring_base[r]
   const uint32_t* ring_of;   // [B] ring-set calls: the ring of each row (null: every row uses ring_m, N entries)
   const uint32_t* ring_base; // [R] entry offset of each padded ring of the set
-  const uint32_t* ring_size; // [R] N_r (every ring of one pass has depth n)
+  const uint32_t* ring_size; // [R] N_r
+  const uint32_t* ring_depth;// [R] n_r = ceil(log2 N_r) <= n
   // parameters / tables
   const uint32_t* g_tab8;    // P-256 generator, w=8 affine table [32][256][16]
   const uint32_t* h_tab8;    // NistGroup.h, fixed-base affine table with h_w-bit windows
@@ -106,9 +108,10 @@ struct ProveCtx {
   uint32_t* secrets;   // [M][34][8] Montgomery mod tom.order
   uint32_t* item_chal; // [M][6][3]
   // GK
-  uint32_t* gk_dv;     // [B][n][8]  d(omega_w), Montgomery
+  uint32_t* gk_dv;     // [B][n][8]  d(omega_w), Montgomery (row b fills its first n_row(b))
   uint32_t* gk_part;   // [B][n][2^(n-k)][8] block sums of d(omega_w) when the ring is cut into blocks (n > k)
-  uint32_t* gk_lag;    // [n][n][8]  Lagrange matrix for nodes 0..n-1, Montgomery
+  uint32_t* gk_lag;    // [n][n][8]  Lagrange matrix for nodes 0..n-1, Montgomery; with a ring set the matrices of every
+                       //    depth 1..n, depth d at word gk_lag_off(d)
   uint32_t* gk_x;      // [B][3]
   // outputs
   uint8_t* proofs;     // [B][proof_stride]
@@ -118,6 +121,7 @@ struct ProveCtx {
 
   ZK_HD size_t s2_job(size_t item, int j) const { return item * JOBS_PER_ITEM + j; }
   ZK_HD size_t s2_der(size_t item, int j) const { return (size_t)M * JOBS_PER_ITEM + item * DERS_PER_ITEM + j; }
+  // GK commitment j of row b: cl ca cb cd fill the first 4 n_row(b) of the row's 4n slots, the rest are zero jobs
   ZK_HD size_t s2_gk(size_t b, int j) const { return (size_t)M * (JOBS_PER_ITEM + DERS_PER_ITEM) + b * 4 * n + j; }
   ZK_HD size_t s2_count() const { return (size_t)M * (JOBS_PER_ITEM + DERS_PER_ITEM) + (size_t)B * 4 * n; }
   ZK_HD size_t s1_pt(size_t b, int j) const { return b * (2 + 2 * S) + j; }  // 0 pkX, 1 pkY, 2+2i Tx_i, 3+2i Ty_i
@@ -125,6 +129,10 @@ struct ProveCtx {
   // the ring of row b (its 2^n padded entries) and its size
   ZK_HD const uint32_t* ring_of_row(int b) const { return ring_of ? ring_m + (size_t)8 * ring_base[ring_of[b]] : ring_m; }
   ZK_HD uint32_t ring_size_row(int b) const { return ring_of ? ring_size[ring_of[b]] : (uint32_t)N; }
+  // the depth of row b's ring, the n of its proof (gk.ts:94-195), and the Lagrange matrix of that depth
+  ZK_HD int n_row(int b) const { return ring_of ? (int)ring_depth[ring_of[b]] : n; }
+  ZK_HD static size_t gk_lag_off(int d) { return (size_t)8 * ((size_t)(d - 1) * d * (2 * d - 1) / 6); }   // 8 * sum of e^2, e < d
+  ZK_HD const uint32_t* gk_lag_row(int b) const { return ring_of ? gk_lag + gk_lag_off(n_row(b)) : gk_lag; }
 };
 
 // draw a scalar and check it is below the modulus (the host pre-filters, see include/zkattest.h)
@@ -454,7 +462,7 @@ struct ExpChallengeTask {
     }
     c.zcount[b] = z;
     c.gk_off[b] = off;
-    c.proof_len[b] = c.mode == 1 ? off : off + gk_len(c.n);
+    c.proof_len[b] = c.mode == 1 ? off : off + gk_len(c.n_row(b));
   }
 };
 // single-thread exclusive scan of zcount (B <= a few thousand per chunk)
@@ -832,9 +840,17 @@ ZK_HD int gk_draw0(const ProveCtx& c, int b) { return draws_before_items(c.S) + 
 struct GkJobsTask {
   ProveCtx c;
   ZK_HD void operator()(int t) const {
-    const int b = t / c.n, i = t % c.n;
-    const int d = gk_draw0(c, b) + DRAWS_PER_GK_ROUND * i;
+    const int b = t / c.n, i = t % c.n, n = c.n_row(b);
     uint32_t ri[8], ai[8], si[8], ti[8], v[8];
+    if (i >= n) {   // beyond the row's depth: the thread zeroes four of the row's unused slots [4 n, 4 c.n)
+      zero_n<8>(v);
+      for (int q = 0; q < 4; q++) {
+        const size_t j = c.s2_gk(b, 4 * i + q);
+        st8v(c.s2_jv + j * 8, v); st8v(c.s2_jr + j * 8, v);
+      }
+      return;
+    }
+    const int d = gk_draw0(c, b) + DRAWS_PER_GK_ROUND * i;
     draw_checked<FpP256>(ri, c, b, d + 0);
     draw_checked<FpP256>(ai, c, b, d + 1);
     draw_checked<FpP256>(si, c, b, d + 2);
@@ -844,9 +860,9 @@ struct GkJobsTask {
     v[0] = bit;
     size_t j = c.s2_gk(b, i);                        // cl_i
     st8v(c.s2_jv + j * 8, v); st8v(c.s2_jr + j * 8, ri);
-    j = c.s2_gk(b, c.n + i);                         // ca_i
+    j = c.s2_gk(b, n + i);                           // ca_i
     st8v(c.s2_jv + j * 8, ai); st8v(c.s2_jr + j * 8, si);
-    j = c.s2_gk(b, 2 * c.n + i);                     // cb_i
+    j = c.s2_gk(b, 2 * n + i);                       // cb_i
     if (bit) copy_n<8>(v, ai); else zero_n<8>(v);
     st8v(c.s2_jv + j * 8, v); st8v(c.s2_jr + j * 8, ti);
   }
@@ -860,10 +876,12 @@ struct GkPolyTask {     // one thread per (proof, w, ring block)
   ProveCtx c;
   ZK_HD void operator()(int t) const {
     using F = Tomq;
-    const int n = c.n, k = gk_block_bits(n);
+    const int gblk = 1 << (c.n - gk_block_bits(c.n));   // the grid: c.n points w and gblk blocks per proof
+    const int blk = t % gblk, bw = t / gblk;
+    const int b = bw / c.n, w = bw % c.n;
+    const int n = c.n_row(b), k = gk_block_bits(n);
     const int nblk = 1 << (n - k);
-    const int blk = t % nblk, bw = t / nblk;
-    const int b = bw / n, w = bw % n;
+    if (w >= n || blk >= nblk) return;
     const int d0 = gk_draw0(c, b);
     uint32_t f0[20][8], f1[20][8];
     uint32_t wm[8], wc[8];
@@ -893,11 +911,13 @@ struct GkPolyReduceTask {   // d(omega_w) = sum of the block sums (only launched
   ProveCtx c;
   ZK_HD void operator()(int bw) const {
     using F = Tomq;
-    const int nblk = 1 << (c.n - gk_block_bits(c.n));
+    const int gblk = 1 << (c.n - gk_block_bits(c.n));
+    const int n = c.n_row(bw / c.n), nblk = 1 << (n - gk_block_bits(n));
+    if (bw % c.n >= n || nblk == 1) return;   // no such point, or GkPolyTask wrote gk_dv itself
     uint32_t acc[8], v[8];
     zero_n<8>(acc);
     for (int i = 0; i < nblk; i++) {
-      ld<8>(v, c.gk_part + ((size_t)bw * nblk + i) * 8);
+      ld<8>(v, c.gk_part + ((size_t)bw * gblk + i) * 8);
       F::add(acc, acc, v);
     }
     st<8>(c.gk_dv + (size_t)bw * 8, acc);
@@ -958,17 +978,25 @@ struct GkLagrangeTask {
   }
 };
 
+// the matrices of the depths 1..count for a ring set, depth d at word ProveCtx::gk_lag_off(d).  One thread per depth.
+struct GkLagrangeSetTask {
+  uint32_t* lag;
+  ZK_HD void operator()(int t) const { GkLagrangeTask{lag + ProveCtx::gk_lag_off(t + 1), t + 1}(0); }
+};
+
 // cd_k = commit(d_k, rho_k), d = L * dv  (gk.ts:173-176).  One thread per (proof, k).
 struct GkCdJobsTask {
   ProveCtx c;
   ZK_HD void operator()(int t) const {
     using F = Tomq;
-    const int b = t / c.n, k = t % c.n;
+    const int b = t / c.n, k = t % c.n, n = c.n_row(b);
+    if (k >= n) return;
+    const uint32_t* lag = c.gk_lag_row(b);
     uint32_t acc[8];
     zero_n<8>(acc);
-    for (int i = 0; i < c.n; i++) {
+    for (int i = 0; i < n; i++) {
       uint32_t l[8], y[8], m[8];
-      ld<8>(l, c.gk_lag + ((size_t)k * c.n + i) * 8);
+      ld<8>(l, lag + ((size_t)k * n + i) * 8);
       ld<8>(y, c.gk_dv + ((size_t)b * c.n + i) * 8);
       F::mul(m, l, y);
       F::add(acc, acc, m);
@@ -976,7 +1004,7 @@ struct GkCdJobsTask {
     uint32_t v[8], rho[8];
     F::from_mont(v, acc);
     draw_checked<FpP256>(rho, c, b, gk_draw0(c, b) + DRAWS_PER_GK_ROUND * k + 4);
-    const size_t j = c.s2_gk(b, 3 * c.n + k);
+    const size_t j = c.s2_gk(b, 3 * n + k);
     st<8>(c.s2_jv + j * 8, v);
     st<8>(c.s2_jr + j * 8, rho);
   }
@@ -995,7 +1023,7 @@ struct GkEmitTask {
   };
   ZK_HD void operator()(int b) const {
     using F = Tomq;
-    const int n = c.n;
+    const int n = c.n_row(b);
     uint32_t c3[3], xc[8], xm[8];
     Src src{&c, b};
     hash_points80(c3, src, 4 * n);

@@ -113,16 +113,18 @@ ZK_HD bool prove_draw_mod_n(int k, int S) {
 }
 
 // Prover draws [d0, d0 + span) of every row: thread t = (row t / span, draw d0 + t % span), one 32-byte draw in two
-// 16-byte stores.  With zcount set, row b stops at prove_draws(zcount[b], n, S), the last draw its proof reads.
+// 16-byte stores.  With zcount set, row b stops at prove_draws(zcount[b], n_b, S), the last draw its proof reads; n_b is
+// the depth of the row's own ring when ring_of is set (a ring-set call, n then being the largest depth), else n.
 struct SeedProveTapeTask {
   const uint8_t* seeds;   // [B][32]
   uint8_t* tape;          // [B][tape_stride], 16-byte aligned rows
   size_t tape_stride;
   int S, n, d0, span;
   const uint32_t* zcount; // [B] or null
+  const uint32_t *ring_of, *ring_depth;   // [B], [R] or null
   ZK_HD void operator()(int t) const {
     const int b = t / span, k = d0 + t % span;
-    if (zcount && k >= prove_draws((int)zcount[b], n, S)) return;
+    if (zcount && k >= prove_draws((int)zcount[b], ring_of ? (int)ring_depth[ring_of[b]] : n, S)) return;
     uint32_t key[8], m[8], w[8];
     seed_key(key, seeds + (size_t)b * 32);
     seed_modulus(m, prove_draw_mod_n(k, S));
@@ -133,27 +135,30 @@ struct SeedProveTapeTask {
 
 // The verifier layout of every row (zk_verify.cuh): thread t = (row, slot).  Slots [0, 2n + 1 + 25K) are the 32-byte
 // draws in order (GK drains, then the packed exp drains behind the index area); the V_IDX_PAD / 16 slots after them
-// write the index area 16 bytes at a time (index bytes i < S - 2, zero padding behind).
+// write the index area 16 bytes at a time (index bytes i < S - 2, zero padding behind).  With ring_of set (a ring-set
+// call) a row has the layout of its own ring's depth n_b <= n, and the slots beyond it are idle.
 struct SeedVerifyTapeTask {
   const uint8_t* seeds;   // [B][32]
   uint8_t* tape;          // [B][tape_stride], 16-byte aligned rows
   size_t tape_stride;
   int n, S, K;
-  ZK_HD int draws() const { return 2 * n + 1 + 25 * K; }
-  ZK_HD int slots() const { return draws() + V_IDX_PAD / 16; }
+  const uint32_t *ring_of, *ring_depth;   // [B], [R] or null
+  ZK_HD int slots() const { return 2 * n + 1 + 25 * K + V_IDX_PAD / 16; }
   ZK_HD void operator()(int t) const {
-    const int b = t / slots(), s = t % slots(), g = 2 * n + 1;
+    const int b = t / slots(), s = t % slots();
+    const int g = 2 * (ring_of ? (int)ring_depth[ring_of[b]] : n) + 1, draws = g + 25 * K;
+    if (s >= draws + V_IDX_PAD / 16) return;
     uint32_t key[8], w[8];
     seed_key(key, seeds + (size_t)b * 32);
     uint8_t* row = tape + (size_t)b * tape_stride;
-    if (s < draws()) {
+    if (s < draws) {
       uint32_t m[8];
       seed_modulus(m, true);
       seed_draw32(w, key, SEED_DOM_VERIFY, (uint64_t)s, m);
       st8v(reinterpret_cast<uint32_t*>(row + (s < g ? (size_t)32 * s : (size_t)32 * s + V_IDX_PAD)), w);
       return;
     }
-    const int j = s - draws();
+    const int j = s - draws;
 #pragma unroll
     for (int q = 0; q < 4; q++) w[q] = 0;
     for (int q = 0; q < 16; q++) {

@@ -55,7 +55,7 @@ ZK_LAYOUT_FN size_t verify_tape_len(int n, int /*reps*/, int K = V_SAMPLES) {
 }
 
 struct VerifyCtx {
-  int B, S, N, n;
+  int B, S, N, n;              // n: the depth the chunk is laid out for (ProveCtx::n); n_row(b) is row b's own
   int K;                       // sampled repetitions (<= S)
   int mode;                    // 0: verifySignatureList; 1: verifyExp alone (exp.ts:233, no GK block, Q given or absent);
                                // 2: verifyMembership alone (gk.ts:197)
@@ -70,6 +70,7 @@ struct VerifyCtx {
   const uint32_t* ring_m;      // [2^n][8] Montgomery mod q (a ring set: all its rings, see ProveCtx)
   const uint32_t* ring_of;     // [B] ring-set calls: the ring of each row (null: ring_m for every row)
   const uint32_t* ring_base;   // [R] entry offset of each padded ring of the set
+  const uint32_t* ring_depth;  // [R] n_r = ceil(log2 N_r) <= n
   const uint32_t* g_tab8;
   const uint32_t* h_tab8;
   int h_w;
@@ -111,7 +112,7 @@ struct VerifyCtx {
   uint32_t* nent_aff;   // [B][21][16]
   uint8_t* nent_skip;   // [B][21]
   // GK
-  uint32_t* gk_scalar;  // [B][4n+1][8]
+  uint32_t* gk_scalar;  // [B][4n+1][8]        row b: cl ca cb cd com in its first 4 n_row(b) + 1, zero scalars behind them
   uint32_t* gk_part;    // [B][2^(n-k)][8] block sums of the ring polynomial (only when n > GK_BLOCK_BITS)
   uint32_t* gk_pre;     // [B][4n+1][32]
   // fixed-base parts: tom jobs [B][2] (0: GK, 1: W) and their points; P-256 fixed part
@@ -133,8 +134,10 @@ struct VerifyCtx {
   ZK_HD const uint8_t* proof_of(int b) const { return proofs + (size_t)b * proof_stride; }
   ZK_HD const uint8_t* tape_of(int b) const { return tape + (size_t)b * tape_stride; }
   ZK_HD const uint32_t* ring_of_row(int b) const { return ring_of ? ring_m + (size_t)8 * ring_base[ring_of[b]] : ring_m; }
-  ZK_HD size_t gk_tape_bytes() const { return mode == 1 ? 0 : (size_t)32 * (2 * n + 1); }
-  ZK_HD const uint8_t* exp_tape(int b) const { return tape_of(b) + gk_tape_bytes() + V_IDX_PAD; }
+  ZK_HD int n_row(int b) const { return ring_of ? (int)ring_depth[ring_of[b]] : n; }   // the depth of row b's ring
+  // a row's tape has the layout of its own ring: 2 n_row(b) + 1 GK drains, the index area, the exp drains
+  ZK_HD size_t gk_tape_bytes(int b) const { return mode == 1 ? 0 : (size_t)32 * (2 * n_row(b) + 1); }
+  ZK_HD const uint8_t* exp_tape(int b) const { return tape_of(b) + gk_tape_bytes(b) + V_IDX_PAD; }
   ZK_HD size_t ta_pt(size_t sample, int j) const { return sample * 2 + j; }   // 0 T1x, 1 T1y
   ZK_HD size_t td_pt(size_t sample, int j) const { return sample * DERS_PER_ITEM + j; }
 };
@@ -178,7 +181,7 @@ struct VLayoutTask {
     }
     st<3>(c.tagbits + (size_t)b * 3, tg);
     c.gk_off[b] = off;
-    c.gk_ok_len[b] = (!bad && (c.mode == 1 || ngk == c.n)) ? 1 : 0;
+    c.gk_ok_len[b] = (!bad && (c.mode == 1 || ngk == c.n_row(b))) ? 1 : 0;
     if (bad) {
       ZK_SET_STATUS(c.status + b, ZKA_ERR_MALFORMED);
       // park the offsets on the header so later stages read in-bounds garbage
@@ -293,7 +296,7 @@ struct VChallengeTask {
     // Knuth shuffle with the pre-filtered index bytes: j = rnd(limit - i) + i
     uint8_t perm[MAX_REPS];
     for (int i = 0; i < c.S; i++) perm[i] = (uint8_t)i;
-    const uint8_t* ib = c.tape_of(b) + c.gk_tape_bytes();
+    const uint8_t* ib = c.tape_of(b) + c.gk_tape_bytes(b);
     for (int i = 0; i < c.S - 2; i++) {
       uint32_t r = ib[i];
       if (r >= (uint32_t)(c.S - i)) { ZK_SET_STATUS(c.status + b, ZKA_ERR_TAPE_RANGE); r = 0; }
@@ -583,9 +586,10 @@ struct VGkSumTask {
   VerifyCtx c;
   ZK_HD void operator()(int t) const {
     using F = Tomq;
-    const int n = c.n, k = gk_block_bits(n);
-    const int nblk = 1 << (n - k);
-    const int b = t / nblk, blk = t % nblk;
+    const int gblk = 1 << (c.n - gk_block_bits(c.n));   // the grid: gblk blocks per proof
+    const int b = t / gblk, blk = t % gblk;
+    const int n = c.n_row(b), k = gk_block_bits(n);
+    if (n == k || blk >= 1 << (n - k)) return;   // VGkTask sums a ring of one block itself
     uint32_t acc[8];
     zero_n<8>(acc);
     if (c.gk_ok_len[b]) {
@@ -619,10 +623,11 @@ struct VGkTask {
   VerifyCtx c;
   ZK_HD void operator()(int b) const {
     using F = Tomq;
-    const int n = c.n;
+    const int n = c.n_row(b), per = 4 * c.n + 1;
     if (c.gk_tape_bad) c.gk_tape_bad[b] = 0;
+    // the slots behind the row's 4n + 1 entries (all of them when the length check fails) hold zero scalars
+    for (int k = c.gk_ok_len[b] ? 4 * n + 1 : 0; k < per; k++) { uint32_t z[8]; zero_n<8>(z); st<8>(c.gk_scalar + ((size_t)b * per + k) * 8, z); }
     if (!c.gk_ok_len[b]) {   // length check fails -> verifyMembership returns false before any draw
-      for (int k = 0; k < 4 * n + 1; k++) { uint32_t z[8]; zero_n<8>(z); st<8>(c.gk_scalar + ((size_t)b * (4 * n + 1) + k) * 8, z); }
       uint32_t z[8]; zero_n<8>(z);
       st<8>(c.fx_jv + (size_t)b * 2 * 8, z); st<8>(c.fx_jr + (size_t)b * 2 * 8, z);
       return;
@@ -645,7 +650,7 @@ struct VGkTask {
     zero_n<8>(gS); zero_n<8>(hS); zero_n<8>(z);
     uint32_t fm[20][8], omf[20][8];     // f_j and x - f_j (Montgomery)
     bool tape_ok = true;
-    uint32_t* sc = c.gk_scalar + (size_t)b * (4 * n + 1) * 8;
+    uint32_t* sc = c.gk_scalar + (size_t)b * per * 8;
     for (int i = 0; i < n; i++) {
       uint32_t f[8], za[8], zb[8];
       wscalar_parse(f, fs + (size_t)i * WS);  F::to_mont(fm[i], f);
@@ -673,7 +678,7 @@ struct VGkTask {
         uint32_t v[8];
         zero_n<8>(total);
         for (int i = 0; i < nblk; i++) {
-          ld<8>(v, c.gk_part + ((size_t)b * nblk + i) * 8);
+          ld<8>(v, c.gk_part + ((size_t)b * (1 << (c.n - gk_block_bits(c.n))) + i) * 8);
           F::add(total, total, v);
         }
       }
@@ -707,8 +712,8 @@ struct VGkOffsetsTask {   // byte offsets of cl, ca, cb, cd, com for VParseEntri
   uint32_t* off;          // [B][4n+1]
   ZK_HD void operator()(int t) const {
     const int per = 4 * c.n + 1;
-    const int b = t / per, k = t % per;
-    off[t] = c.gk_ok_len[b] ? (k < 4 * c.n ? c.gk_off[b] + 1 + (uint32_t)k * WP : (uint32_t)(2 * NP)) : (uint32_t)(2 * NP);
+    const int b = t / per, k = t % per;   // com and the zero-scalar slots behind it read keyXcom
+    off[t] = c.gk_ok_len[b] && k < 4 * c.n_row(b) ? c.gk_off[b] + 1 + (uint32_t)k * WP : (uint32_t)(2 * NP);
   }
 };
 

@@ -348,7 +348,8 @@ struct zka_rings {
   uint32_t R = 0;
   std::vector<uint32_t> size;              // N_r
   std::vector<int> depth;                  // n_r = ceil(log2 N_r)
-  DevBuf ring_m, ring_base, ring_size;     // [total][8], [R], [R]
+  DevBuf ring_m, ring_base, ring_size, ring_depth;   // [total][8], [R], [R], [R]
+  DevBuf lag;                              // the prover's GK Lagrange matrices of the depths 1 .. max n_r (GkLagrangeSetTask)
 };
 
 namespace {
@@ -674,21 +675,21 @@ struct VerifyRows {
   }
 };
 
-// Where the rows of a batched call find their ring: one ring of N keys for every row, or one pass of a set, whose rows
-// (ring_of) all have rings of depth n (a set call enters ring_passes as pass(set, 0)).  proveExp / verifyExp alone have
-// neither and keep N = 2.
+// Where the rows of a batched call find their ring: one ring of N keys for every row, or a set, whose rows (ring_of) each
+// have the ring and the depth of their own; n, the depth the chunks are laid out for, is then the largest depth the rows
+// use (a set call enters ring_passes as pass(set, 0)).  proveExp / verifyExp alone have neither and keep N = 2.
 struct RingSrc {
   const uint8_t* ring; uint32_t N;   // one ring, or
-  const zka_rings* set; int n;       // one pass of a set
+  const zka_rings* set; int n;       // a set
   static RingSrc one(const uint8_t* ring, uint32_t N) { return {ring, N, nullptr, ceil_log2(N)}; }
   static RingSrc pass(const zka_rings* set, int n) { return {nullptr, 0, set, n}; }
   static RingSrc none(int n) { return {nullptr, 2, nullptr, n}; }
   // the call's ring on the device and, for the prover, the Lagrange matrix: once per call, done before the lanes start
   const uint32_t* prepare(zka_ctx* ctx, bool lagrange) const {
     if (!set && !ring) return nullptr;
-    const uint32_t* ring_m = set ? (const uint32_t*)set->ring_m.p : prep_ring(ctx, ctx->st, ring, N, n, lagrange);
-    if (set && lagrange) prep_lagrange(ctx, ctx->st, n);
-    if (!set || lagrange) sync(ctx->st);   // (the verifier's pass of a set queues nothing)
+    if (set) return (const uint32_t*)set->ring_m.p;   // prepared by zka_rings_create, with the matrices of every depth
+    const uint32_t* ring_m = prep_ring(ctx, ctx->st, ring, N, n, lagrange);
+    sync(ctx->st);
     return ring_m;
   }
   // a chunk's ring fields; ring_of: the chunk's rows of it on the device
@@ -698,14 +699,18 @@ struct RingSrc {
     if (!set) return;
     c.ring_of = ring_of;
     c.ring_base = (const uint32_t*)set->ring_base.p;
-    if constexpr (std::is_same<Ctx, ProveCtx>::value) c.ring_size = (const uint32_t*)set->ring_size.p;
+    c.ring_depth = (const uint32_t*)set->ring_depth.p;
+    if constexpr (std::is_same<Ctx, ProveCtx>::value) {
+      c.ring_size = (const uint32_t*)set->ring_size.p;
+      c.gk_lag = (uint32_t*)set->lag.p;
+    }
   }
 };
 
-// A batched call after its null checks: its ring's checks, check(largest depth used), then pass(r0, count, ring) on rows
-// [r0, r0 + count): all B rows for one ring (or none), else each run of consecutive rows whose rings share a depth, as a
-// chunk's launch geometry (B n GK threads, 4n + 1 GK scalars per proof, the verify tape layout, the seeded spans) assumes
-// one n.  A set's ring_of is read on the host (4 bytes per row, copied when it is device memory).
+// A batched call after its null checks: its ring's checks, check(largest depth used), then ONE pass(ring) over all B rows.
+// For a set the chunks' launch geometry (B n GK threads, 4n + 1 GK scalars per proof, the tape row widths) takes the largest
+// depth the rows use and every row follows its own (n_row), whatever the order of depths in ring_of.  A set's ring_of is
+// read on the host (4 bytes per row, copied when it is device memory) to check the indices and find that depth.
 template <class Check, class Pass>
 int ring_passes(zka_ctx* ctx, const RingSrc& ring, const uint32_t* ring_of, uint32_t B, Check check, Pass pass) {
   if (ring.set && ring.set->ctx != ctx) return fail(ctx, ZKA_E_ARG, "ring set of another context");
@@ -715,9 +720,9 @@ int ring_passes(zka_ctx* ctx, const RingSrc& ring, const uint32_t* ring_of, uint
       // N = 1 makes hashPoints([]) throw in the reference (group.ts:223 reduce of an empty array)
       if (ring.N < 2 || ring.N > (1u << 20)) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
       const int rc = check(ring.n);
-      return rc ? rc : pass(0u, B, ring);
+      return rc ? rc : pass(ring);
     }
-    std::vector<uint32_t> h(B), start;
+    std::vector<uint32_t> h(B);
     if (is_device_ptr(ring_of)) {
       copy_d2h(ctx->st, h.data(), ring_of, (size_t)B * 4);
       sync(ctx->st);
@@ -728,14 +733,10 @@ int ring_passes(zka_ctx* ctx, const RingSrc& ring, const uint32_t* ring_of, uint
     int nmax = 0;
     for (uint32_t b = 0; b < B; b++) {
       if (h[b] >= ring.set->R) return fail(ctx, ZKA_E_ARG, "ring_of[i] >= number of rings in the set");
-      if (b == 0 || depth[h[b]] != depth[h[b - 1]]) start.push_back(b);
       nmax = std::max(nmax, depth[h[b]]);
     }
-    start.push_back(B);
-    if (const int rc = check(nmax)) return rc;
-    for (size_t k = 0; k + 1 < start.size(); k++)
-      if (const int rc = pass(start[k], start[k + 1] - start[k], RingSrc::pass(ring.set, depth[h[start[k]]]))) return rc;
-    return 0;
+    const int rc = check(nmax);
+    return rc ? rc : pass(RingSrc::pass(ring.set, nmax));
   });
 }
 
@@ -1123,11 +1124,16 @@ int zka_rings_create(zka_ctx* ctx, uint32_t R, const uint32_t* sizes, const uint
     uint32_t* d_off = obuf.get<uint32_t>(R);
     uint32_t* d_base = set->ring_base.get<uint32_t>(R);
     uint32_t* d_size = set->ring_size.get<uint32_t>(R);
+    uint32_t* d_depth = set->ring_depth.get<uint32_t>(R);
+    const std::vector<uint32_t> depth(set->depth.begin(), set->depth.end());
+    const int nmax = *std::max_element(set->depth.begin(), set->depth.end());
     uint32_t* ring_m = set->ring_m.get<uint32_t>((size_t)total * 8);
     copy_h2d(st, d_off, key_off.data(), (size_t)R * 4);
     copy_h2d(st, d_base, base.data(), (size_t)R * 4);
     copy_h2d(st, d_size, set->size.data(), (size_t)R * 4);
+    copy_h2d(st, d_depth, depth.data(), (size_t)R * 4);
     launch(st, (long long)total, RingSetPrepTask{d_keys, d_off, d_base, d_size, ring_m, (int)R});
+    launch(st, nmax, GkLagrangeSetTask{set->lag.get<uint32_t>(ProveCtx::gk_lag_off(nmax + 1))});
     sync(st);
     *out = set.release();
     return 0;
@@ -1487,9 +1493,10 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
       const bool tape_host = !seeded && ctx->tape_split && !is_device_ptr(rows.tape);
       sync(st);
       if (seeded) {
-        // the item and GK draws of each proof, up to the longest proof of the chunk (zmax = tot2[1])
+        // the item and GK draws of each proof, up to the longest a proof of the chunk can be (zmax = tot2[1], depth n)
         const int d1 = draws_before_items(S), span = prove_draws((int)tot2[1], n, S) - d1;
-        launch(st, (long long)Bc * span, SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, d1, span, c.zcount});
+        launch(st, (long long)Bc * span,
+               SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, d1, span, c.zcount, c.ring_of, c.ring_depth});
       } else if (tape_host) {
         // second part of the tape: draws [3 + 4S, 3 + 4S + 40 zmax + 5n) of every row in one strided copy
         // (zmax = the largest zero-bit count of the chunk)
@@ -1535,7 +1542,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
       launch(st, (long long)Bc * FIN_PARTS, FinalizeTask{c});
       // --- results: on the output stream, behind this chunk's last kernel
       ev_record(ln.ev_done[slot], st);
-      if (ctx->progress && !ring.set && k_this < ctx->progress_cap) notify_progress(st, ctx->progress + k_this);
+      if (ctx->progress && k_this < ctx->progress_cap) notify_progress(st, ctx->progress + k_this);
       if (!po.dev || !lo.dev || !so.dev) {
         Stream& co = ln.cs_out;
         ev_wait(co, ln.ev_done[slot]);
@@ -1564,7 +1571,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
   return 0;
 }
 
-// Every batched prove call: its argument checks (strides against the deepest ring used), then its prove_impl passes
+// Every batched prove call: its argument checks (strides against the deepest ring used), then its prove_impl pass
 static int prove_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const ProveRows& rows, const RingSrc& ring, int mode) {
   if (!ctx || !P || !rows.pk || (!rows.tape && !rows.seeds) || !rows.proofs || !rows.proof_len || !rows.status) return ZKA_E_ARG;
   if (mode == 0 && (!rows.msg_hash || !rows.sig || !rows.which || !(ring.set ? (const void*)rows.ring_of : ring.ring))) return ZKA_E_ARG;
@@ -1575,9 +1582,7 @@ static int prove_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prov
     if (rows.tape && rows.tape_stride < (size_t)32 * (mode == 0 ? prove_draws(0, n, S) : draws_before_items(S))) return fail(ctx, ZKA_E_ARG, "tape_stride too small");
     return 0;
   };
-  return ring_passes(ctx, ring, rows.ring_of, B, check, [&](uint32_t r0, uint32_t count, const RingSrc& pass) {
-    return prove_impl(ctx, P, count, rows.at(r0), pass, mode);
-  });
+  return ring_passes(ctx, ring, rows.ring_of, B, check, [&](const RingSrc& pass) { return prove_impl(ctx, P, B, rows, pass, mode); });
 }
 
 int zka_prove_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
@@ -1929,7 +1934,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
     c.tape_stride = seeded ? seed_stride : rows.tape_stride;
     ring.fill(c, ring_m, cur.ring_of);
     if (seeded) {
-      const SeedVerifyTapeTask vt{cur.seeds, const_cast<uint8_t*>(cur.tape), seed_stride, n, S, K};
+      const SeedVerifyTapeTask vt{cur.seeds, const_cast<uint8_t*>(cur.tape), seed_stride, n, S, K, c.ring_of, c.ring_depth};
       launch(st, (long long)Bc * vt.slots(), vt);
     }
     double t_in = 0.0;
@@ -2134,7 +2139,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
   return 0;
 }
 
-// Every batched verify call: its argument checks (tape stride against the deepest ring used), then its verify_impl passes
+// Every batched verify call: its argument checks (tape stride against the deepest ring used), then its verify_impl pass
 static int verify_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const VerifyRows& rows, const RingSrc& ring,
                         uint32_t samples, int mode) {
   if (!ctx || !P || !rows.proofs || !rows.proof_len || (!rows.tape && !rows.seeds) || !rows.ok || !rows.status) return ZKA_E_ARG;
@@ -2148,9 +2153,7 @@ static int verify_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const Ver
       return fail(ctx, ZKA_E_ARG, "tape_stride < zka_verify_tape_len");
     return 0;
   };
-  return ring_passes(ctx, ring, rows.ring_of, B, check, [&](uint32_t r0, uint32_t count, const RingSrc& pass) {
-    return verify_impl(ctx, P, count, rows.at(r0), pass, samples, mode);
-  });
+  return ring_passes(ctx, ring, rows.ring_of, B, check, [&](const RingSrc& pass) { return verify_impl(ctx, P, B, rows, pass, samples, mode); });
 }
 
 int zka_verify_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
