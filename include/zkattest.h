@@ -294,8 +294,17 @@ int zka_set_profiling(zka_ctx* ctx, int enable);
 int zka_profile_reset(zka_ctx* ctx);
 size_t zka_profile_json(zka_ctx* ctx, char* buf, size_t cap);
 /* tuning knobs read at zka_init from the environment (zka_config reports the first three):
- *   ZKA_TOM_W       window bits of the tomEdwards256 fixed-base tables, 2..24, default 22
- *                   (ceil(256/w) windows x 2^w entries x 128 B per base: 6.4 GB at 22, 134 MB at 16)
+ *   ZKA_TOM_NWIN    lookups per scalar of the tomEdwards256 fixed-base tables g and h, 11..128, default 11.  The 257 bits
+ *                   of a walk (256 of the scalar, 1 carry of the signed recoding) are cut into windows of
+ *                   w = floor(257 / n) bits and, on top of them, 257 - w n windows of w + 1 bits; a window of b bits holds
+ *                   2^(b-1) + 1 entries of 128 B.  11: 7 windows of 23 bits + 4 of 24 = 8.05 GB per base; 12: 7 of 21 + 5
+ *                   of 22 = 2.3 GB; 16: 15 of 16 + 1 of 17 = 71 MB.  If the tables do not fit in the device's free memory
+ *                   at zka_init, the context walks one lookup more (12 for the default) and says so: zka_config reports
+ *                   the shape in use, zka_stat "tom_fallback" is 1.
+ *   ZKA_TOM_W       instead: the same width for all windows, 2..24 ((256 + w) / w windows of 2^(w-1) + 1 entries: 3.2 GB
+ *                   per base at 22, 12 lookups; 11.8 GB at 24, 11 lookups).  Takes precedence; never replaced by a
+ *                   smaller table.  The only form the war256 build knows (default 22).
+ *   ZKA_TOM_TABLE_MAX  bytes: a tomEdwards256 table larger than this is treated as an allocation that failed
  *   ZKA_P256_HW     window bits of the P-256 G / NistGroup.h tables, 8..24, default 20 (872 MB per base)
  *   ZKA_CHUNK       largest chunk (proofs per pipeline pass) when all buffers are device memory, default 4096
  *   ZKA_HOST_CHUNK  largest chunk when buffers are host memory, default 2048; the schedule is tapered
@@ -318,7 +327,9 @@ int zka_set_option(zka_ctx* ctx, const char* key, long value);
  * sum over all proofs of the chunk of the reference's three linear combinations, multimult.ts:147-174, evaluated as one
  * wide-window MSM; every relation carries its own random scalar, so the sum is the identity iff (w.h.p.) every
  * per-proof combination is), "agg_fail" = chunks that went on to the per-proof evaluation (some proof invalid or
- * already rejected by the parsers; verdicts and statuses are then exactly the per-proof ones).  -1: unknown key.
+ * already rejected by the parsers; verdicts and statuses are then exactly the per-proof ones).  Not counters:
+ * "tom_n_lo" = how many of the tom_nwin windows zka_config reports have tom_w bits (the others have tom_w + 1),
+ * "tom_fallback" = 1 when the tables asked for did not fit and the context walks one lookup more.  -1: unknown key.
  * ZKA_AGG=0 disables the aggregate check, ZKA_AGG_C=4..16 fixes its window bits. */
 long long zka_stat(zka_ctx* ctx, const char* key);
 

@@ -214,7 +214,12 @@ class ZkaLib:
         w, nw, ch = C.c_int(), C.c_int(), C.c_int()
         self._check(self.lib.zka_config(self.ctx, C.byref(w), C.byref(nw), C.byref(ch)), 'zka_config')
         lanes = int(self.lib.zka_lanes(self.ctx)) if hasattr(self.lib, 'zka_lanes') else 1
-        return {'tom_w': w.value, 'tom_nwin': nw.value, 'chunk': ch.value, 'lanes': lanes}
+        cfg = {'tom_w': w.value, 'tom_nwin': nw.value, 'chunk': ch.value, 'lanes': lanes}
+        # the first tom_n_lo of the tom_nwin windows have tom_w bits, the others tom_w + 1 (ZKA_TOM_NWIN; all of them with
+        # ZKA_TOM_W); tom_fallback: the tables asked for did not fit and the context walks one lookup more
+        if hasattr(self.lib, 'zka_stat') and self.stat('tom_n_lo') >= 0:
+            cfg.update(tom_n_lo=self.stat('tom_n_lo'), tom_fallback=bool(self.stat('tom_fallback')))
+        return cfg
 
     def set_option(self, key: str, value: int):
         self._check(self.lib.zka_set_option(self.ctx, key.encode(), int(value)), f'zka_set_option({key})')

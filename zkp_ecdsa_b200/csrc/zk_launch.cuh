@@ -206,15 +206,28 @@ struct DevBuf {
   DevBuf(const DevBuf&) = delete;
   DevBuf& operator=(const DevBuf&) = delete;
   ~DevBuf() { dev_free(p); }
+  void release() {
+    dev_free(p);
+    p = nullptr;
+    cap = 0;
+  }
   template <class T>
   T* get(size_t count) {
     size_t bytes = count * sizeof(T);
     if (bytes > cap) {
-      dev_free(p);
+      release();   // stays empty if the allocation throws
       size_t want = bytes + bytes / 8 + 256;
       p = dev_alloc(want);
       cap = want;
     }
+    return reinterpret_cast<T*>(p);
+  }
+  // a buffer that will not grow (a multi-gigabyte table): no headroom
+  template <class T>
+  T* get_exact(size_t count) {
+    release();
+    p = dev_alloc(count * sizeof(T));
+    cap = count * sizeof(T);
     return reinterpret_cast<T*>(p);
   }
 };

@@ -238,14 +238,43 @@ ZK_HD uint32_t digit_w(const uint32_t* k, int pos, int w) {
 ZK_HD int fb_entries(int w) { return (1 << (w - 1)) + 1; }
 ZK_HD int fb_windows(int w) { return (256 + w) / w; }
 // digit j of k in signed form: returns |d_j| and its sign; `carry` is the running carry (start with 0)
-ZK_HD uint32_t signed_digit(const uint32_t* k, int j, int w, uint32_t& carry, bool& neg) {
-  const int pos = j * w;
+// the w-bit digit at bit `pos`
+ZK_HD uint32_t signed_digit_at(const uint32_t* k, int pos, int w, uint32_t& carry, bool& neg) {
   uint32_t d = carry;
   if (pos < 256) d += digit_w(k, pos, (256 - pos) < w ? (256 - pos) : w);
   const uint32_t half = 1u << (w - 1);
   neg = d > half;
   carry = neg ? 1u : 0u;
   return neg ? (1u << w) - d : d;
+}
+ZK_HD uint32_t signed_digit(const uint32_t* k, int j, int w, uint32_t& carry, bool& neg) {
+  return signed_digit_at(k, j * w, w, carry, neg);
+}
+
+// Shape of a positional signed-digit table whose windows are not all equally wide: the first n_lo of its nwin windows
+// have w bits, the others w + 1.  With one width the 257 bits of a walk (256 of the scalar and the recoding's carry)
+// take 12 windows at w = 22 and at w = 23, and 11 only at w = 24; seven windows of 23 bits and four of 24 cover exactly
+// 257 bits in 11 lookups with a third less memory than 11 x 24.  The wide windows are the top ones, so bit position and
+// entry offset of window j stay one multiply-add and one shift.  A uniform table is the case n_lo = nwin.
+struct FbShape {
+  int w, nwin, n_lo;
+  ZK_HD int wide(int j) const { return j > n_lo ? j - n_lo : 0; }   // wide windows below window j
+  ZK_HD int width(int j) const { return w + (j >= n_lo ? 1 : 0); }
+  ZK_HD int bitpos(int j) const { return j * w + wide(j); }
+  ZK_HD int bits() const { return bitpos(nwin); }
+  ZK_HD size_t entries(int j) const { return ((size_t)1 << (width(j) - 1)) + 1; }
+  ZK_HD size_t offset(int j) const { return (size_t)j * (size_t)fb_entries(w) + ((size_t)wide(j) << (w - 1)); }   // entries below window j
+  ZK_HD size_t total() const { return offset(nwin); }
+};
+ZK_HD FbShape fb_uniform(int w) { return FbShape{w, fb_windows(w), fb_windows(w)}; }
+// the shape that covers exactly 257 bits in nwin lookups (nwin < 257): w = floor(257 / nwin), 257 - w nwin wide windows
+ZK_HD FbShape fb_lookups(int nwin) {
+  const int w = 257 / nwin;
+  return FbShape{w, nwin, nwin - (257 - w * nwin)};
+}
+// digit j of k on a table of shape s, otherwise as above
+ZK_HD uint32_t signed_digit(const uint32_t* k, int j, const FbShape& s, uint32_t& carry, bool& neg) {
+  return signed_digit_at(k, s.bitpos(j), s.width(j), carry, neg);
 }
 
 // read a 32-byte big-endian tape draw into 8 limbs.  A 16-byte aligned draw (every row of the library's own tape
@@ -383,78 +412,77 @@ ZK_HD int item_job_of_gpart(int g) {
 // ===================================================================== tomEdwards256 tables
 struct TomPowsTask {
   const uint32_t* base_aff;  // [nbase][18] image-curve affine (x', y), Montgomery
-  uint32_t* pows;            // [nbase][nwin][36] extended (X,Y,T,Z)
-  int nbase, nwin, w;
+  uint32_t* pows;            // [nbase][nwin][36] extended (X,Y,T,Z): 2^bitpos(j) * base
+  int nbase;
+  FbShape sh;
   ZK_HD void operator()(int t) const {
     uint32_t x[9], y[9];
     ld<9>(x, base_aff + (size_t)t * TOM_AFF_WORDS);
     ld<9>(y, base_aff + (size_t)t * TOM_AFF_WORDS + 9);
     TomPt p;
     tom_from_affine(p, x, y);
-    for (int j = 0; j < nwin; j++) {
-      uint32_t* o = pows + ((size_t)t * nwin + j) * 36;
+    for (int j = 0; j < sh.nwin; j++) {
+      uint32_t* o = pows + ((size_t)t * sh.nwin + j) * 36;
       st<9>(o, p.x); st<9>(o + 9, p.y); st<9>(o + 18, p.t); st<9>(o + 27, p.z);
-      for (int k = 0; k < w; k++) tom_dbl(p, p);
+      for (int k = 0; k < sh.width(j); k++) tom_dbl(p, p);
     }
   }
 };
-// rows: proj store [(base*nwin + j) * 2^w + d][27] = d * pows[base][j]  (d = 0 is the identity)
+// The rows of ONE window are staged at a time (112 bytes per entry), so the staging buffer is bounded by the widest
+// window and not by the table.
+// rows of a window of w bits: proj store [d][27] = d * pow, d = 0 .. 2^(w-1)  (d = 0 is the identity)
 struct TomRowsTask {
-  const uint32_t* pows;
+  const uint32_t* pow;    // [36]
   uint32_t* rows;
   int w;
-  ZK_HD void operator()(int t) const {
+  ZK_HD void operator()(int) const {
     TomPt p, acc;
-    const uint32_t* s = pows + (size_t)t * 36;
-    ld<9>(p.x, s); ld<9>(p.y, s + 9); ld<9>(p.t, s + 18); ld<9>(p.z, s + 27);
+    ld<9>(p.x, pow); ld<9>(p.y, pow + 9); ld<9>(p.t, pow + 18); ld<9>(p.z, pow + 27);
     tom_set_identity(acc);
     const int ne = fb_entries(w);
-    uint32_t* out = rows + (size_t)t * ne * TOM_PROJ_WORDS;
     for (int d = 0; d < ne; d++) {
-      uint32_t* o = out + (size_t)d * TOM_PROJ_WORDS;
+      uint32_t* o = rows + (size_t)d * TOM_PROJ_WORDS;
       tom_st_xyz(o, acc.x, acc.y, acc.z);
       tom_add(acc, acc, p);
     }
   }
 };
-// Two-level construction of the same rows for wide windows (w > 8): first the 2^(w-8) "high"
-// multiples m * 2^8 * P_j (one thread per window), then one thread per (window, m) walks the
-// 256 entries below it.  2^(w-8) + 256 sequential additions instead of 2^w.
+// Two-level construction of the same rows for wide windows (w > 9): first the 2^(w-9) + 1 "high" multiples
+// m * 2^8 * P_j of every window (one thread per window), then, window by window, one thread per m walks the 256
+// entries above it (the last m = 2^(w-9) is the top entry 2^(w-1) * P_j alone).  2^(w-9) + 256 sequential additions
+// instead of 2^(w-1).
+ZK_HD size_t tom_hi_offset(const FbShape& sh, int j) { return ((sh.offset(j) - (size_t)j) >> 8) + (size_t)j; }   // sum of 2^(w_i - 9) + 1 over i < j
 struct TomRowsHiTask {
   const uint32_t* pows;   // [nwin][36]
-  uint32_t* hi;           // [nwin][2^(w-9)][36]
-  uint32_t* rows;         // the top entry 2^(w-1) * pows of every window is written here directly
-  int w;
+  uint32_t* hi;           // window j at tom_hi_offset(j): [2^(w_j-9) + 1][36]
+  FbShape sh;
   ZK_HD void operator()(int t) const {
     TomPt p, acc;
     const uint32_t* s = pows + (size_t)t * 36;
     ld<9>(p.x, s); ld<9>(p.y, s + 9); ld<9>(p.t, s + 18); ld<9>(p.z, s + 27);
     for (int k = 0; k < 8; k++) tom_dbl(p, p);
     tom_set_identity(acc);
-    const int nh = 1 << (w - 9);
-    for (int m = 0; m < nh; m++) {
-      uint32_t* o = hi + ((size_t)t * nh + m) * 36;
+    const int nh = 1 << (sh.width(t) - 9);
+    for (int m = 0; m <= nh; m++) {
+      uint32_t* o = hi + (tom_hi_offset(sh, t) + m) * 36;
       st<9>(o, acc.x); st<9>(o + 9, acc.y); st<9>(o + 18, acc.t); st<9>(o + 27, acc.z);
       tom_add(acc, acc, p);
     }
-    tom_st_xyz(rows + ((size_t)t * fb_entries(w) + ((size_t)1 << (w - 1))) * TOM_PROJ_WORDS, acc.x, acc.y, acc.z);
   }
 };
 struct TomRowsLoTask {
-  const uint32_t* pows;   // [nwin][36]
-  const uint32_t* hi;     // [nwin][2^(w-9)][36]
-  uint32_t* rows;         // [nwin][E][27]
-  int w;
-  ZK_HD void operator()(int t) const {
-    const int nh = 1 << (w - 9);
-    const int j = t / nh, m = t % nh;
+  const uint32_t* pow;    // [36]: the window's 2^bitpos * base
+  const uint32_t* hi;     // [nh + 1][36]: the window's high multiples
+  uint32_t* rows;         // [256 nh + 1][27]
+  int nh;
+  ZK_HD void operator()(int m) const {
     TomPt p, acc;
-    const uint32_t* s = pows + (size_t)j * 36;
-    ld<9>(p.x, s); ld<9>(p.y, s + 9); ld<9>(p.t, s + 18); ld<9>(p.z, s + 27);
-    const uint32_t* h = hi + (size_t)t * 36;
+    ld<9>(p.x, pow); ld<9>(p.y, pow + 9); ld<9>(p.t, pow + 18); ld<9>(p.z, pow + 27);
+    const uint32_t* h = hi + (size_t)m * 36;
     ld<9>(acc.x, h); ld<9>(acc.y, h + 9); ld<9>(acc.t, h + 18); ld<9>(acc.z, h + 27);
-    uint32_t* out = rows + ((size_t)j * fb_entries(w) + ((size_t)m << 8)) * TOM_PROJ_WORDS;
-    for (int d = 0; d < 256; d++) {
+    uint32_t* out = rows + ((size_t)m << 8) * TOM_PROJ_WORDS;
+    const int n = m < nh ? 256 : 1;
+    for (int d = 0; d < n; d++) {
       uint32_t* o = out + (size_t)d * TOM_PROJ_WORDS;
       tom_st_xyz(o, acc.x, acc.y, acc.z);
       tom_add(acc, acc, p);
@@ -602,9 +630,9 @@ struct TomNormTask {
   }
 };
 
-// entry |d| of window j of a signed-digit E2 table [nwin][ne][32], negated for a negative digit
-ZK_HD void tom2_ld_entry(TomPre& q, const uint32_t* tab, int j, size_t ne, uint32_t d, bool neg) {
-  tom_ld_pre(q, tab + ((size_t)j * ne + d) * TOM_PRE_WORDS);
+// entry |d| of window j of a signed-digit E2 table of shape sh ([total][32]), negated for a negative digit
+ZK_HD void tom2_ld_entry(TomPre& q, const uint32_t* tab, const FbShape& sh, int j, uint32_t d, bool neg) {
+  tom_ld_pre(q, tab + (sh.offset(j) + d) * TOM_PRE_WORDS);
   tom2_pre_neg(q, neg);
 }
 
@@ -615,30 +643,29 @@ ZK_HD void tom2_ld_entry(TomPre& q, const uint32_t* tab, int j, size_t ne, uint3
 struct TomCommitTask {
   const uint32_t* jv;    // [count][8] canonical value scalars (mod tom.order)
   const uint32_t* jr;    // [count][8] canonical blinders
-  const uint32_t* gtab;  // [nwin][2^w][32]
+  const uint32_t* gtab;  // [sh.total()][32]
   const uint32_t* htab;
   uint32_t* proj;        // [count][TOM_E2_WORDS] (E, F, G, H) -> TomNormTask{e2 = 1}; xyz: [count][TOM_PROJ_WORDS]
-  int w, nwin;
+  FbShape sh;
   int xyz = 0;           // 1: a full last addition, E2 (W : V : Z) for readers other than the normaliser (pg_fixed_to_msm)
   ZK_HD void operator()(int t) const {
     uint32_t v[8], r[8];
     ld<8>(v, jv + (size_t)t * 8);
     ld<8>(r, jr + (size_t)t * 8);
-    const size_t ne = (size_t)fb_entries(w);
     uint32_t cv = 0, cr = 0;
     bool nv, nr;
     TomPre q;
-    uint32_t dv = signed_digit(v, 0, w, cv, nv);
-    tom2_ld_entry(q, gtab, 0, ne, dv, nv);
+    uint32_t dv = signed_digit(v, 0, sh, cv, nv);
+    tom2_ld_entry(q, gtab, sh, 0, dv, nv);
     TomPt acc;
     tom2_from_pre(acc, q);
     for (int j = 0;; j++) {
-      const uint32_t dr = signed_digit(r, j, w, cr, nr);
-      tom2_ld_entry(q, htab, j, ne, dr, nr);
-      if (j == nwin - 1) break;
+      const uint32_t dr = signed_digit(r, j, sh, cr, nr);
+      tom2_ld_entry(q, htab, sh, j, dr, nr);
+      if (j == sh.nwin - 1) break;
       tom2_madd<true>(acc, acc, q);     // a = -1 image curve E2: 7M per lookup
-      dv = signed_digit(v, j + 1, w, cv, nv);
-      tom2_ld_entry(q, gtab, j + 1, ne, dv, nv);
+      dv = signed_digit(v, j + 1, sh, cv, nv);
+      tom2_ld_entry(q, gtab, sh, j + 1, dv, nv);
       tom2_madd<true>(acc, acc, q);
     }
     if (xyz) {
@@ -656,23 +683,22 @@ struct TomCommitGTask {   // one thread per (item, g-part): K = v*g as an extend
   const uint32_t* jv;     // [items*34][8]
   const uint32_t* gtab;
   uint32_t* ext;          // [items*28][36]
-  int w, nwin;
+  FbShape sh;
   ZK_HD void operator()(int t) const {
     const int item = t / GJOBS_PER_ITEM, g = t % GJOBS_PER_ITEM;
     uint32_t v[8];
     ld<8>(v, jv + ((size_t)item * JOBS_PER_ITEM + item_job_of_gpart(g)) * 8);
-    const size_t ne = (size_t)fb_entries(w);
     uint32_t carry = 0;
     bool neg;
     TomPre q;
-    const uint32_t d0 = signed_digit(v, 0, w, carry, neg);
-    tom2_ld_entry(q, gtab, 0, ne, d0, neg);
+    const uint32_t d0 = signed_digit(v, 0, sh, carry, neg);
+    tom2_ld_entry(q, gtab, sh, 0, d0, neg);
     TomPt acc;
     tom2_from_pre<TompCommit>(acc, q);
 #pragma unroll 1
-    for (int j = 1; j < nwin; j++) {
-      const uint32_t d = signed_digit(v, j, w, carry, neg);
-      tom2_ld_entry(q, gtab, j, ne, d, neg);
+    for (int j = 1; j < sh.nwin; j++) {
+      const uint32_t d = signed_digit(v, j, sh, carry, neg);
+      tom2_ld_entry(q, gtab, sh, j, d, neg);
       tom2_madd<true, TompCommit>(acc, acc, q);
     }
     uint32_t* o = ext + (size_t)t * TOM_EXT_WORDS;
@@ -684,7 +710,7 @@ struct TomCommitHTask {   // one thread per job: C = K + r*h, ending in tom2_mad
   const uint32_t* htab;
   const uint32_t* ext;    // [items*28][36]
   uint32_t* proj;         // [items*34][TOM_E2_WORDS]  (E, F, G, H) -> TomNormTask{e2 = 1}
-  int w, nwin;
+  FbShape sh;
   ZK_HD void operator()(int t) const {
     const int item = t / JOBS_PER_ITEM, jb = t % JOBS_PER_ITEM;
     uint32_t r[8];
@@ -692,18 +718,17 @@ struct TomCommitHTask {   // one thread per job: C = K + r*h, ending in tom2_mad
     TomPt acc;
     const uint32_t* s = ext + ((size_t)item * GJOBS_PER_ITEM + item_gpart_of_job(jb)) * TOM_EXT_WORDS;
     ld<9>(acc.x, s); ld<9>(acc.y, s + 9); ld<9>(acc.t, s + 18); ld<9>(acc.z, s + 27);
-    const size_t ne = (size_t)fb_entries(w);
     uint32_t carry = 0;
     bool neg;
     TomPre q;
 #pragma unroll 1
-    for (int j = 0; j < nwin - 1; j++) {
-      const uint32_t d = signed_digit(r, j, w, carry, neg);
-      tom2_ld_entry(q, htab, j, ne, d, neg);
+    for (int j = 0; j < sh.nwin - 1; j++) {
+      const uint32_t d = signed_digit(r, j, sh, carry, neg);
+      tom2_ld_entry(q, htab, sh, j, d, neg);
       tom2_madd<true, TompCommit>(acc, acc, q);
     }
-    const uint32_t d = signed_digit(r, nwin - 1, w, carry, neg);
-    tom2_ld_entry(q, htab, nwin - 1, ne, d, neg);
+    const uint32_t d = signed_digit(r, sh.nwin - 1, sh, carry, neg);
+    tom2_ld_entry(q, htab, sh, sh.nwin - 1, d, neg);
     TomEfgh e;
     tom2_madd_end<TompCommit>(e, acc, q);
     tom_st_efgh(proj + (size_t)t * TOM_E2_WORDS, e);

@@ -90,7 +90,7 @@ struct TomCommitTask {
   const uint32_t* gtab;  // [nwin][E][16]
   const uint32_t* htab;
   uint32_t* proj;        // [count][24]
-  int w, nwin;
+  FbShape sh;             // always uniform in this build: sh.w bits in every window
   int xyz = 0;           // the tomEdwards256 build's output-form flag; the output here is always (X, Y, Z)
   ZK_HD void operator()(int t) const {
     uint32_t v[8], r[8];
@@ -98,8 +98,8 @@ struct TomCommitTask {
     ld<8>(r, jr + (size_t)t * 8);
     WarJac aj;
     war_set_identity_jac(aj);
-    war_accum_fixed_jac(aj, gtab, v, w);
-    war_accum_fixed_jac(aj, htab, r, w);
+    war_accum_fixed_jac(aj, gtab, v, sh.w);
+    war_accum_fixed_jac(aj, htab, r, sh.w);
     WarPt acc;
     war_jac_to_hom(acc, aj);
     war_st_proj(proj + (size_t)t * TOM_PROJ_WORDS, acc);
@@ -110,14 +110,14 @@ struct TomCommitGTask {   // one thread per (item, g-part): K = v*g
   const uint32_t* jv;     // [items*34][8]
   const uint32_t* gtab;
   uint32_t* ext;          // [items*28][24]
-  int w, nwin;
+  FbShape sh;             // always uniform in this build: sh.w bits in every window
   ZK_HD void operator()(int t) const {
     const int item = t / GJOBS_PER_ITEM, g = t % GJOBS_PER_ITEM;
     uint32_t v[8];
     ld<8>(v, jv + ((size_t)item * JOBS_PER_ITEM + item_job_of_gpart(g)) * 8);
     WarJac aj;
     war_set_identity_jac(aj);
-    war_accum_fixed_jac(aj, gtab, v, w);
+    war_accum_fixed_jac(aj, gtab, v, sh.w);
     WarPt acc;
     war_jac_to_hom(acc, aj);
     war_st_proj(ext + (size_t)t * TOM_EXT_WORDS, acc);
@@ -128,14 +128,14 @@ struct TomCommitHTask {   // one thread per job: C = K + r*h
   const uint32_t* htab;
   const uint32_t* ext;    // [items*28][24]
   uint32_t* proj;         // [items*34][24]
-  int w, nwin;
+  FbShape sh;             // always uniform in this build: sh.w bits in every window
   ZK_HD void operator()(int t) const {
     const int item = t / JOBS_PER_ITEM, jb = t % JOBS_PER_ITEM;
     uint32_t r[8];
     ld<8>(r, jr + (size_t)t * 8);
     WarPt acc;
     war_ld_proj(acc, ext + ((size_t)item * GJOBS_PER_ITEM + item_gpart_of_job(jb)) * TOM_EXT_WORDS);
-    war_accum_fixed(acc, htab, r, w);
+    war_accum_fixed(acc, htab, r, sh.w);
     war_st_proj(proj + (size_t)t * TOM_PROJ_WORDS, acc);
   }
 };

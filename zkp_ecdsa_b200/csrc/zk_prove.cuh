@@ -30,7 +30,7 @@ struct ProveCtx {
   int n;        // the depth the chunk is laid out for (grids, workspace strides, slots per proof): ceil(log2 N), with a
                 //    ring set the largest depth the call uses; the depth of row b's own ring is n_row(b)
   int M;        // total 0-bit repetitions (items) in the chunk (valid after the scan)
-  int tom_w, tom_nwin;
+  FbShape tom;                 // shape of the proof group's two fixed-base tables (g, h)
   int mode;                  // 0: proveSignatureList; 1: proveExp alone (exp.ts:126-231): R = `base`, s and Q are inputs,
                              //    the row holds the repetitions only (no header, no GK block)
   int head_len;              // bytes before the first repetition (HEAD_LEN, or 0 in mode 1)

@@ -60,7 +60,7 @@ struct VerifyCtx {
   int mode;                    // 0: verifySignatureList; 1: verifyExp alone (exp.ts:233, no GK block, Q given or absent);
                                // 2: verifyMembership alone (gk.ts:197)
   const uint8_t* q_ext;        // mode 1: [B][65] Q points (all-zero = identity) or null (no Q: T1 = g*z)
-  int tom_w, tom_nwin;
+  FbShape tom;                 // shape of the proof group's two fixed-base tables (g, h)
   const uint8_t* msg_hash;     // [B][32]
   const uint8_t* proofs;       // [B][proof_stride]
   size_t proof_stride;

@@ -308,7 +308,14 @@ struct zka_ctx : Lane {
   int nlanes = 3;             // ZKA_LANES
   DevBuf ring_in, ring_m;     // the ring of the current call (shared by all lanes, read-only while they run)
   Lane& lane(int i) { return i == 0 ? *this : *extra[i - 1]; }
-  int tom_w = 22, tom_nwin = 12;   // per base: 12 windows x (2^21 + 1) signed-digit entries x 128 B = 3.2 GB of HBM (ZKA_TOM_W)
+#if defined(ZKA_PG_WAR256)
+  FbShape tom = fb_uniform(22);   // shape of the proof group's fixed-base tables g and h (ZKA_TOM_W)
+#else
+  FbShape tom = fb_lookups(11);   // 7 windows of 23 bits + 4 of 24: 7 (2^22 + 1) + 4 (2^23 + 1) signed-digit entries x 128 B =
+                                  // 8.05 GB of HBM per base (ZKA_TOM_NWIN, ZKA_TOM_W)
+#endif
+  size_t tom_table_max = 0;       // a proof-group table above this many bytes counts as an allocation that failed (ZKA_TOM_TABLE_MAX)
+  bool tom_fallback = false;      // the tables of the shape asked for did not fit: this context walks one lookup more (zka_stat)
   int chunk = 4096;       // largest chunk of a call whose buffers are all device memory (ZKA_CHUNK)
   int host_chunk = 2048;  // chunk size when proofs return to host memory: copies of one chunk overlap the next
   volatile uint32_t* progress = nullptr;   // zka_set_progress: flags[k] = 1 when chunk k of the running prove call is complete
@@ -472,16 +479,23 @@ void build_p256_tab(zka_ctx* ctx, const uint32_t* base_aff_dev, FixedTable& out,
   launch_p256_norm(st, d_rows, out.tab, nullptr, nullptr, (long long)(count));
   sync(st);
 }
+// memory of one proof-group table of shape ctx->tom; throws when it exceeds ZKA_TOM_TABLE_MAX or the device has no room
+uint32_t* alloc_tom_tab(zka_ctx* ctx, DevBuf& buf) {
+  const size_t words = ctx->tom.total() * TOM_PRE_WORDS;
+  if (ctx->tom_table_max && words * sizeof(uint32_t) > ctx->tom_table_max)
+    throw std::runtime_error("proof-group fixed-base table of " + std::to_string(words * sizeof(uint32_t)) + " bytes exceeds ZKA_TOM_TABLE_MAX");
+  return buf.get_exact<uint32_t>(words);
+}
 #if defined(ZKA_PG_WAR256)
 // war256 positional table [fb_windows(w)][fb_entries(w)] of affine points from one affine base (16 words, device)
 void build_tom_tab(zka_ctx* ctx, const uint32_t* base_aff_dev, FixedTable& out) {
   Stream& st = ctx->st;
-  const int w = ctx->tom_w, nwin = fb_windows(w);
+  const int w = ctx->tom.w, nwin = ctx->tom.nwin;
   const size_t E = (size_t)fb_entries(w), count = (size_t)nwin * E;
   DevBuf pows, rows;
   uint32_t* d_pows = pows.get<uint32_t>((size_t)nwin * P256_PROJ_WORDS);
   uint32_t* d_rows = rows.get<uint32_t>(count * P256_PROJ_WORDS);
-  out.tab = out.buf.get<uint32_t>(count * TOM_PRE_WORDS);
+  out.tab = alloc_tom_tab(ctx, out.buf);
   launch(st, 1, WarPowsTask{base_aff_dev, nullptr, d_pows, 1, nwin, w});
   if (w > 9) {
     DevBuf hi;
@@ -500,28 +514,35 @@ void build_tom_tab(zka_ctx* ctx, const uint32_t* base_aff_dev, FixedTable& out) 
   sync(st);
 }
 #else
-// tomEdwards256 positional table [nwin][fb_entries(w)] from one image-curve affine base (18 words, device)
+// tomEdwards256 positional table of shape ctx->tom from one image-curve affine base (18 words, device).  Built window
+// by window through one staging buffer of projective rows, which is therefore as large as the widest window (0.94 GB
+// at 24 bits) and not as the table.
 void build_tom_tab(zka_ctx* ctx, const uint32_t* base_aff_dev, FixedTable& out) {
   Stream& st = ctx->st;
-  const int w = ctx->tom_w, nwin = ctx->tom_nwin;
-  const size_t ne = (size_t)fb_entries(w), count = (size_t)nwin * ne;
-  DevBuf pows, rows;
-  uint32_t* d_pows = pows.get<uint32_t>((size_t)nwin * 36);
-  uint32_t* d_rows = rows.get<uint32_t>(count * TOM_PROJ_WORDS);
-  out.tab = out.buf.get<uint32_t>(count * TOM_PRE_WORDS);
-  launch(st, 1, TomPowsTask{base_aff_dev, d_pows, 1, nwin, w});
-  if (w > 9) {
-    DevBuf hi;
-    const int nh = 1 << (w - 9);
-    uint32_t* d_hi = hi.get<uint32_t>((size_t)nwin * nh * 36);
-    launch(st, nwin, TomRowsHiTask{d_pows, d_hi, d_rows, w});
-    launch(st, (long long)nwin * nh, TomRowsLoTask{d_pows, d_hi, d_rows, w});
-    sync(st);   // hi is freed at the end of this block, before the normalisation
-  } else {
-    launch(st, nwin, TomRowsTask{d_pows, d_rows, w});
+  const FbShape sh = ctx->tom;
+  out.tab = alloc_tom_tab(ctx, out.buf);
+  DevBuf pows, rows, hi;
+  uint32_t* d_pows = pows.get<uint32_t>((size_t)sh.nwin * 36);
+  uint32_t* d_rows = rows.get<uint32_t>(sh.entries(sh.nwin - 1) * TOM_PROJ_WORDS);
+  launch(st, 1, TomPowsTask{base_aff_dev, d_pows, 1, sh});
+  const bool two_level = sh.w > 9;
+  uint32_t* d_hi = nullptr;
+  if (two_level) {
+    d_hi = hi.get<uint32_t>(tom_hi_offset(sh, sh.nwin) * 36);
+    launch(st, sh.nwin, TomRowsHiTask{d_pows, d_hi, sh});
   }
-  // rows (E1 projective) -> entries of the prover's a = -1 image curve (v - w, v + w, 2 d2 w v)
-  launch(st, (long long)(count + 15) / 16, TomTabE2Task{d_rows, out.tab, (int)count});
+  for (int j = 0; j < sh.nwin; j++) {
+    const size_t ne = sh.entries(j);
+    const uint32_t* pw = d_pows + (size_t)j * 36;
+    if (two_level) {
+      const int nh = 1 << (sh.width(j) - 9);
+      launch(st, nh + 1, TomRowsLoTask{pw, d_hi + tom_hi_offset(sh, j) * 36, d_rows, nh});
+    } else {
+      launch(st, 1, TomRowsTask{pw, d_rows, sh.width(j)});
+    }
+    // rows (E1 projective) -> entries of the prover's a = -1 image curve (v - w, v + w, 2 d2 w v)
+    launch(st, (long long)(ne + 15) / 16, TomTabE2Task{d_rows, out.tab + sh.offset(j) * TOM_PRE_WORDS, (int)ne});
+  }
   sync(st);
 }
 
@@ -747,7 +768,7 @@ ProveCtx prove_ctx(const zka_ctx* ctx, const zka_params* P, int B, int S, int N,
   ProveCtx c;
   memset(&c, 0, sizeof(c));
   c.B = B; c.S = S; c.N = N; c.n = n;
-  c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
+  c.tom = ctx->tom;
   c.g_tab8 = ctx->g8.tab; c.h_tab8 = P->h8.tab; c.h_w = P->h_w;
   c.g_tabw = ctx->gw.tab; c.g_w = ctx->p256_hw;
   c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
@@ -760,7 +781,7 @@ VerifyCtx verify_ctx(const zka_ctx* ctx, const zka_params* P, int B, int S, int 
   VerifyCtx c;
   memset(&c, 0, sizeof(c));
   c.B = B; c.S = S; c.N = N; c.n = n; c.K = K; c.mode = mode;
-  c.tom_w = ctx->tom_w; c.tom_nwin = ctx->tom_nwin;
+  c.tom = ctx->tom;
   c.g_tab8 = ctx->g8.tab; c.h_tab8 = P->h8.tab; c.h_w = P->h_w;
   c.tg_tab = ctx->tg.tab; c.th_tab = P->th.tab;
   c.tg_bytes = (const uint8_t*)ctx->tg_bytes.p;
@@ -771,7 +792,7 @@ VerifyCtx verify_ctx(const zka_ctx* ctx, const zka_params* P, int B, int S, int 
 void prove_store1(Stream& st, const ProveCtx& c) {
   const long long n1 = (long long)c.B * (2 + 2 * c.S);
   launch(st, n1, JobsATask{c});
-  launch(st, n1, TomCommitTask{c.s1_jv, c.s1_jr, c.tg_tab, c.th_tab, c.s1_proj, c.tom_w, c.tom_nwin});
+  launch(st, n1, TomCommitTask{c.s1_jv, c.s1_jr, c.tg_tab, c.th_tab, c.s1_proj, c.tom});
   launch_tom_norm(st, c.s1_proj, c.s1_aff, c.s1_bytes, n1, 1);
 }
 // The c.M items of the 0-bit repetitions (pointAdd.ts:92-163 each), from their secrets to their bytes in the proof rows,
@@ -795,12 +816,11 @@ void prove_items_gk(Stream& st, const ProveCtx& c, uint32_t* gext, bool items, b
     launch(st, Bn, GkCdJobsTask{c});
   }
   if (items) {   // item jobs: g-parts once per distinct committed value, then r*h on top (TomCommitG/HTask)
-    launch(st, M * GJOBS_PER_ITEM, TomCommitGTask{c.s2_jv, c.tg_tab, gext, c.tom_w, c.tom_nwin});
-    launch(st, nj, TomCommitHTask{c.s2_jr, c.th_tab, gext, c.s2_proj, c.tom_w, c.tom_nwin});
+    launch(st, M * GJOBS_PER_ITEM, TomCommitGTask{c.s2_jv, c.tg_tab, gext, c.tom});
+    launch(st, nj, TomCommitHTask{c.s2_jr, c.th_tab, gext, c.s2_proj, c.tom});
   }
   if (gk)
-    launch(st, ng, TomCommitTask{c.s2_jv + g0 * 8, c.s2_jr + g0 * 8, c.tg_tab, c.th_tab, c.s2_proj + g0 * TOM_E2_WORDS, c.tom_w,
-                                 c.tom_nwin});
+    launch(st, ng, TomCommitTask{c.s2_jv + g0 * 8, c.s2_jr + g0 * 8, c.tg_tab, c.th_tab, c.s2_proj + g0 * TOM_E2_WORDS, c.tom});
   if (items) {
     // only T1x, T1y (jobs 0, 1 of each item) are needed again as points (DerivedTask)
     launch_tom_norm(st, c.s2_proj, c.s2_aff, c.s2_bytes, nj, 1, JOBS_PER_ITEM, 2);
@@ -900,6 +920,8 @@ long long zka_stat(zka_ctx* ctx, const char* key) {
   if (k == "agg_pass") return (long long)ctx->agg_pass;
   if (k == "agg_fail") return (long long)ctx->agg_fail;
   if (k == "agg_c") return (long long)ctx->agg_c_last;        // window bits of the last tomEdwards256 aggregate MSM
+  if (k == "tom_n_lo") return (long long)ctx->tom.n_lo;
+  if (k == "tom_fallback") return ctx->tom_fallback ? 1 : 0;
   return -1;
 }
 size_t zka_profile_json(zka_ctx* ctx, char* buf, size_t cap) {
@@ -963,8 +985,8 @@ int zka_chunk_schedule(zka_ctx* ctx, uint32_t B, int host_buffers, uint32_t* off
 int zka_lanes(const zka_ctx* ctx) { return ctx ? ctx->nlanes : 0; }
 int zka_config(const zka_ctx* ctx, int* tom_w, int* tom_nwin, int* chunk) {
   if (!ctx) return ZKA_E_ARG;
-  if (tom_w) *tom_w = ctx->tom_w;
-  if (tom_nwin) *tom_nwin = ctx->tom_nwin;
+  if (tom_w) *tom_w = ctx->tom.w;
+  if (tom_nwin) *tom_nwin = ctx->tom.nwin;
   if (chunk) *chunk = ctx->chunk;
   return 0;
 }
@@ -987,11 +1009,19 @@ int zka_init(int device, zka_ctx** out) {
     ZK_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->st.s, cudaStreamNonBlocking));
 #endif
     ctx->device = device;
+    // shape of the proof-group tables: ZKA_TOM_W pins one width for all windows; otherwise ZKA_TOM_NWIN lookups
+    [[maybe_unused]] bool tom_pinned = false;
     if (const char* e = getenv("ZKA_TOM_W")) {
       int w = atoi(e);
-      if (w >= 2 && w <= 24) ctx->tom_w = w;
+      if (w >= 2 && w <= 24) { ctx->tom = fb_uniform(w); tom_pinned = true; }
     }
-    ctx->tom_nwin = fb_windows(ctx->tom_w);
+#if !defined(ZKA_PG_WAR256)
+    if (const char* e = tom_pinned ? nullptr : getenv("ZKA_TOM_NWIN")) {
+      int n = atoi(e);
+      if (n >= 11 && n <= 128) ctx->tom = fb_lookups(n);
+    }
+#endif
+    if (const char* e = getenv("ZKA_TOM_TABLE_MAX")) ctx->tom_table_max = (size_t)strtoull(e, nullptr, 10);
     if (const char* e = getenv("ZKA_CHUNK")) {
       int c = atoi(e);
       if (c >= 1) ctx->chunk = c;
@@ -1036,7 +1066,28 @@ int zka_init(int device, zka_ctx** out) {
     launch(ctx->st, 1, GenAffTask{d_gen, d_gen + 16});
     build_p256_tab(ctx.get(), d_gen, ctx->g8, 8);
     build_p256_tab(ctx.get(), d_gen, ctx->gw, ctx->p256_hw);
+#if defined(ZKA_PG_WAR256)
     build_tom_tab(ctx.get(), d_gen + 16, ctx->tg);
+#else
+    // g and every h table share one shape, so it is settled here: a shape given by its lookups is kept when the g table
+    // and one table more (the first parameter set's h) can be allocated; otherwise (other work may hold the card's
+    // memory) what was taken is freed and the context walks one lookup more, 12 for the default: 2.3 GB per base.  A
+    // width pinned with ZKA_TOM_W is not replaced: it fails.
+    try {
+      DevBuf room;
+      alloc_tom_tab(ctx.get(), room);
+      build_tom_tab(ctx.get(), d_gen + 16, ctx->tg);
+    } catch (const std::exception&) {
+      if (tom_pinned || ctx->tom.nwin >= 128) throw;
+#if !defined(ZKA_HOSTSIM)
+      cudaGetLastError();   // the failed allocation is handled here
+#endif
+      ctx->tg.buf.release();
+      ctx->tom = fb_lookups(ctx->tom.nwin + 1);
+      ctx->tom_fallback = true;
+      build_tom_tab(ctx.get(), d_gen + 16, ctx->tg);
+    }
+#endif
     // encoding of g (C_14 = params.g in pi_8, pointAdd.ts:144,220): normalise the table entry 1*g
     DevBuf proj, aff;
     uint32_t* d_proj = proj.get<uint32_t>(TOM_PROJ_WORDS);
@@ -1170,7 +1221,7 @@ int zka_tom_commit_batch(zka_ctx* ctx, const zka_params* P, uint32_t count, cons
     const Output<uint8_t> o(out, WP);
     uint8_t* packed = o.rows(ob.next(), 0, count);
     launch(st, count, CommitConvTask{dv, dr, jv, jr});
-    launch(st, count, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, proj, ctx->tom_w, ctx->tom_nwin});
+    launch(st, count, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, proj, ctx->tom});
     launch_tom_norm(st, proj, aff, bytes, (long long)(count), 1);
     launch(st, count, PackTomTask{bytes, packed});
     o.copy_back(st, 0, packed, count);
@@ -1274,7 +1325,7 @@ int zka_params_generate(zka_ctx* ctx, const uint8_t rnd[64], uint8_t h_nist[65],
     copy_h2d(st, d_rnd, rnd + 32, 32);
     launch(st, 1, GenConvTask{d_rnd, jv, jr});
     // v*g + 0*g: use the g table for both bases
-    launch(st, 1, TomCommitTask{jv, jr, ctx->tg.tab, ctx->tg.tab, proj, ctx->tom_w, ctx->tom_nwin});
+    launch(st, 1, TomCommitTask{jv, jr, ctx->tg.tab, ctx->tg.tab, proj, ctx->tom});
     launch_tom_norm(st, proj, aff, bytes, (long long)(1), 1);
     copy_d2h(st, h_proof, bytes, WP);
     sync(st);
@@ -1751,7 +1802,7 @@ static int prove_sub(zka_ctx* ctx, const zka_params* P, int kind, uint32_t B, co
       uint8_t* d_prf = po.rows(ob.next(), b0, Bc);
       int32_t* d_st = so.rows(ob.next(), b0, Bc);
       launch(st, Bc, SubProveJobsTask{kind, d_sc, d_tape, tape_stride, jv, jr, d_st});
-      launch(st, (long long)nj, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, proj, ctx->tom_w, ctx->tom_nwin});
+      launch(st, (long long)nj, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, proj, ctx->tom});
       launch_tom_norm(st, proj, nullptr, bytes, (long long)nj, 1);
       launch(st, Bc, SubProveEmitTask{kind, d_sc, d_tape, tape_stride, jr, bytes, d_com, d_prf, d_st});
       co.copy_back(st, b0, d_com, Bc);
@@ -2020,7 +2071,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
     launch(st, (long long)ns, VSampleP256Task{c});
     launch_p256_norm(st, c.sp_T, c.sp_T_aff, nullptr, c.sp_T_inf, (long long)(ns));
     launch(st, (long long)ns, VSampleJobsTask{c});
-    launch(st, (long long)ns * 2, TomCommitTask{c.ta_jv, c.ta_jr, c.tg_tab, c.th_tab, c.ta_proj, c.tom_w, c.tom_nwin});
+    launch(st, (long long)ns * 2, TomCommitTask{c.ta_jv, c.ta_jr, c.tg_tab, c.th_tab, c.ta_proj, c.tom});
     launch_tom_norm(st, c.ta_proj, c.ta_aff, nullptr, (long long)(ns * 2), 1);
     launch(st, (long long)ns, VDerivedTask{c});
     launch_tom_norm(st, c.td_proj, nullptr, c.td_bytes, (long long)(ns * DERS_PER_ITEM), 0);
@@ -2034,7 +2085,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
     launch(st, Bc, VReduceTask{c});
     launch(st, (long long)Bc * ET, VParseEntriesTask{c.proofs, c.proof_stride, c.ent_off, c.ent_pre, ET});
     if (mode == 0) launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, c.proof_stride, gk_offs, c.gk_pre, ngk});
-    launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin, 1});
+    launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom, 1});
     // chunk-wide aggregate check (zk_verify_agg.cuh): the sum over all proofs of the chunk of the three linear
     // combinations, as ONE wide-window MSM per group; when both sums are the identity the per-proof MSMs below
     // return at once
@@ -2082,7 +2133,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
       // fixed-base parts: one commitment for the summed tomEdwards256 scalars, a two-level sum of the P-256 points
       launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, fpart, Bc});
       launch(st, 1, AggFixSumTask{ctl, fpart, fjv, fjr, fgroups});
-      launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom_w, c.tom_nwin, 1});
+      launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom, 1});
       launch(sb, ngroups, AggNistFixPartTask{ctl, c.nfix, npart, Bc});
       int nleft = ngroups;            // second level: at most Bc / 1024 partial sums reach the final thread
       const uint32_t* nsum = npart;
@@ -2281,7 +2332,7 @@ int zka_verify_membership_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, c
       dev_memset(st, c.fx_jr, 0, (size_t)Bc * 2 * 8 * 4);
       verify_gk(st, c, gk_offs);
       launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, row_stride, gk_offs, c.gk_pre, ngk});
-      launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom_w, c.tom_nwin, 1});
+      launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom, 1});
       launch(st, (long long)Bc * MSM_NWIN, MsmTomWindowTask{c.gk_scalar, c.gk_pre, nullptr, ngk, 0, 0, ngk, V_SEG, 1, c.win_g});
       launch(st, Bc, MsmTomCombineTask{c.win_g, c.fx_proj, c.id_flags, 2, 0, 0});
       launch(st, Bc, VGkOnlyFinalTask{c});
@@ -2327,7 +2378,7 @@ static int verify_sub(zka_ctx* ctx, const zka_params* P, int kind, uint32_t B, c
       launch(st, Bc, VSubProofTask{kind, rows, stride, d_tape, tape_stride, (const uint8_t*)ctx->tg_bytes.p, ent_scalar, ent_off,
                                    fx_jv, fx_jr, d_st, d_ok});
       launch(st, (long long)Bc * SUB_ENT_MAX, VParseEntriesTask{rows, stride, ent_off, ent_pre, SUB_ENT_MAX});
-      launch(st, (long long)Bc * 2, TomCommitTask{fx_jv, fx_jr, ctx->tg.tab, P->th.tab, fx_proj, ctx->tom_w, ctx->tom_nwin, 1});
+      launch(st, (long long)Bc * 2, TomCommitTask{fx_jv, fx_jr, ctx->tg.tab, P->th.tab, fx_proj, ctx->tom, 1});
       launch(st, (long long)Bc * MSM_NWIN, MsmTomWindowTask{ent_scalar, ent_pre, nullptr, SUB_ENT_MAX, 0, 0, ne, V_SEG, 1, win});
       launch(st, Bc, MsmTomCombineTask{win, fx_proj, flags, 2, 1, 1});
       launch(st, Bc, VSubFinalTask{d_st, flags, d_ok});
