@@ -86,6 +86,14 @@ enum {
   ZKA_ERR_MALFORMED = 9,         /* proof bytes do not parse (deserializePoint / deserializeScalar throw) */
   ZKA_ERR_PARAMS_NOT_FOUND = 10  /* exp.ts:270,302 */
 };
+/* Precedence: a row with several defects gets the code of the one the reference meets first.
+ *   verify (zka_verify_batch*, zka_verify_exp_batch):  ZKA_ERR_MALFORMED (the whole proof is parsed first, so it wins over
+ *     everything below), ZKA_ERR_R_INFINITY, a Groth-Kohlweiss draw out of range (ZKA_ERR_TAPE_RANGE); then a membership
+ *     proof that fails gives ok = 0 with status 0, whatever the repetitions carry; then a generateIndices byte out of
+ *     range (ZKA_ERR_TAPE_RANGE); then the sampled repetitions in sample order (generateIndices on the tape), the first
+ *     one with a defect deciding: ZKA_ERR_PARAMS_NOT_FOUND, its first draw out of range, ZKA_ERR_T_INFINITY /
+ *     ZKA_ERR_T1_INFINITY, its later draws out of range.
+ *   prove: ZKA_ERR_INVALID_PK, ZKA_ERR_BAD_INDEX, then the repetitions in order. */
 
 enum {
   ZKA_E_ARG = -1,     /* bad argument */

@@ -21,6 +21,8 @@ namespace zk {
 
 #if defined(__CUDA_ARCH__)
 #define ZK_SET_STATUS(ptr, code) atomicCAS((int*)(ptr), 0, (int)(code))
+// the smallest key wins, whichever thread or kernel posts it first (the verifier's exp-side status keys, zk_verify.cuh)
+#define ZK_POST_MIN(ptr, key) atomicMin((int*)(ptr), (int)(key))
 // first error wins, except that `code` also replaces the later-stage error `over` (used when the two
 // stages run side by side in one grid: the outcome equals running this stage first)
 #define ZK_SET_STATUS_OVER(ptr, code, over) \
@@ -36,6 +38,10 @@ namespace zk {
 #define ZK_SET_STATUS(ptr, code) \
   do {                           \
     if (*(ptr) == 0) *(ptr) = (code); \
+  } while (0)
+#define ZK_POST_MIN(ptr, key)             \
+  do {                                    \
+    if ((int)(key) < *(ptr)) *(ptr) = (int)(key); \
   } while (0)
 #endif
 

@@ -49,6 +49,17 @@ enum : int {
   AGG_CTL_WORDS = 4,
 };
 
+// Status precedence of a row (include/zkattest.h): the reference throws at the first defect it meets, so a row with several
+// defects reports that one.  status[] takes, first writer wins (ZK_SET_STATUS, in launch order), what is thrown before
+// verifyExp: a proof that does not parse (VLayoutTask, VValidateTask), then R at infinity (VChallengeTask), then a GK draw
+// out of range (VReduceTask).  verifyExp's own throws (exp.ts:253-345) come from several kernels, and from concurrent
+// threads of one proof, but the reference meets them in sample order: each writer posts a key to vkey[] with
+// ZK_POST_MIN and VFinalTask keeps the smallest.  A key is (sample + 1) << 8 | phase << 4 | code, sample -1 being the
+// generateIndices draws; inside one sample the phases follow verifyExp: 'params not found', the first draw (relA), T / T1
+// at infinity, the later draws.
+enum : int { VK_NONE = 0x7fffffff, VK_PARAMS = 0, VK_FIRST_DRAW = 1, VK_T_INF = 2, VK_DRAWS = 3 };
+ZK_HD int vkey(int sample, int phase, int code) { return ((sample + 1) << 8) | (phase << 4) | code; }
+
 // K = number of sampled repetitions (verifyExp's secparam, exp.ts:233-262): 20 in verifySignatureList
 ZK_LAYOUT_FN size_t verify_tape_len(int n, int /*reps*/, int K = V_SAMPLES) {
   return (size_t)32 * (2 * n + 1) + V_IDX_PAD + (size_t)32 * 25 * K;
@@ -123,6 +134,7 @@ struct VerifyCtx {
   uint32_t* win_g;      // [B][MSM_NWIN][36]
   uint32_t* win_n;      // [B][MSM_NWIN_N][24]
   uint8_t* id_flags;    // [B][3]  gk, W, N identity
+  int32_t* vkey;        // [B] smallest exp-side status key (vkey()), VK_NONE if none
   const uint32_t* agg_ctl;  // aggregate verdicts of the chunk (AGG_*), or null
   // outputs
   uint8_t* ok;          // [B]
@@ -151,6 +163,7 @@ struct VLayoutTask {
     using Fn = P256n;
     using Fp = P256p;
     c.status[b] = ZKA_OK;
+    c.vkey[b] = VK_NONE;
     c.ok[b] = 0;
     const uint8_t* pr = c.proof_of(b);
     const uint32_t len = c.proof_len[b];
@@ -194,7 +207,7 @@ struct VLayoutTask {
     bool okR = bad ? true : p256_parse(R, rinf, pr);
     if (bad) p256_set_generator(R);
     if (!okR) { ZK_SET_STATUS(c.status + b, ZKA_ERR_MALFORMED); p256_set_generator(R); }
-    if (rinf) ZK_SET_STATUS(c.status + b, ZKA_ERR_R_INFINITY);   // zkpAttestList.ts:158-160
+    // R at infinity is reported by VChallengeTask, behind every deserialisation error of the proof
     p256_st_aff(c.r_aff + (size_t)b * 16, R);
     if (c.mode == 1) {   // Q is an input (or absent): no statement to derive it from
       P256Aff Qa;
@@ -286,6 +299,11 @@ struct VChallengeTask {
   VerifyCtx c;
   ZK_HD void operator()(int b) const {
     const uint8_t* pr = c.proof_of(b);
+    // 'R is at infinity' (zkpAttestList.ts:158-160) is thrown once the whole proof has parsed (readJson): after
+    // VValidateTask, so that a proof with both reports ZKA_ERR_MALFORMED.  The identity is the all-zero slot (p256_parse).
+    bool rinf = true;
+    for (int k = 0; k < NP; k++) rinf = rinf && pr[k] == 0;
+    if (rinf) ZK_SET_STATUS(c.status + b, ZKA_ERR_R_INFINITY);
     Sha256 h;
     h.init();
     h.update(pr + 2 * NP, 2 * WP);
@@ -297,9 +315,10 @@ struct VChallengeTask {
     uint8_t perm[MAX_REPS];
     for (int i = 0; i < c.S; i++) perm[i] = (uint8_t)i;
     const uint8_t* ib = c.tape_of(b) + c.gk_tape_bytes(b);
+    int key = VK_NONE;
     for (int i = 0; i < c.S - 2; i++) {
       uint32_t r = ib[i];
-      if (r >= (uint32_t)(c.S - i)) { ZK_SET_STATUS(c.status + b, ZKA_ERR_TAPE_RANGE); r = 0; }
+      if (r >= (uint32_t)(c.S - i)) { key = vkey(-1, 0, ZKA_ERR_TAPE_RANGE); r = 0; }
       const int j = (int)r + i;
       const uint8_t k = perm[i];
       perm[i] = perm[j];
@@ -312,11 +331,12 @@ struct VChallengeTask {
       const int i = perm[j];
       const uint32_t bit = (c3[i >> 5] >> (i & 31)) & 1u;
       const uint32_t tag = (tg[i >> 5] >> (i & 31)) & 1u;
-      if (bit != tag) ZK_SET_STATUS(c.status + b, ZKA_ERR_PARAMS_NOT_FOUND);   // exp.ts:269-271,301-303
+      if (bit != tag && key == VK_NONE) key = vkey(j, VK_PARAMS, ZKA_ERR_PARAMS_NOT_FOUND);   // exp.ts:269-271,301-303
       c.samp_idx[(size_t)b * c.K + j] = (uint32_t)i;
       c.samp_draw[(size_t)b * c.K + j] = draw;
       draw += bit ? 3 : 25;
     }
+    if (key != VK_NONE) ZK_POST_MIN(c.vkey + b, key);
   }
 };
 
@@ -361,7 +381,7 @@ struct VSampleJobsTask {
       st<8>(c.ta_jv + c.ta_pt(t, xy) * 8, v);
       st<8>(c.ta_jr + c.ta_pt(t, xy) * 8, r);
     }
-    if (c.sp_T_inf[t]) ZK_SET_STATUS(c.status + b, rep[0] ? ZKA_ERR_T_INFINITY : ZKA_ERR_T1_INFINITY);  // exp.ts:283,323
+    if (c.sp_T_inf[t]) ZK_POST_MIN(c.vkey + b, vkey(t % c.K, VK_T_INF, rep[0] ? ZKA_ERR_T_INFINITY : ZKA_ERR_T1_INFINITY));  // exp.ts:283,323
   }
 };
 
@@ -433,7 +453,7 @@ struct VRelationsTask {
     f.tape_ok = true;
     // --- multiN: relA (exp.ts:273-279 / 306-316)
     uint32_t rho[8], rm[8], s[8], sm[8], t0[8], t1[8];
-    f.tape_ok = vdraw(rho, dr, true) && f.tape_ok;
+    const bool first_ok = vdraw(rho, dr, true);
     Fn::to_mont(rm, rho);
     nscalar_parse(s, body);            // alpha | z
     Fn::to_mont(sm, s);
@@ -491,7 +511,7 @@ struct VRelationsTask {
       out.put_m(e0 + 1, in[5], offTy);
       c.ent_cnt[t] = V_ENT_PER_SAMPLE;
     }
-    if (!f.tape_ok) ZK_SET_STATUS(c.status + b, ZKA_ERR_TAPE_RANGE);
+    if (!first_ok || !f.tape_ok) ZK_POST_MIN(c.vkey + b, vkey(j, first_ok ? VK_DRAWS : VK_FIRST_DRAW, ZKA_ERR_TAPE_RANGE));
     st<8>(part, f.gW); st<8>(part + 8, f.hW); st<8>(part + 16, pX); st<8>(part + 24, pY);
     st<8>(part + 32, sR); st<8>(part + 40, sH); st<8>(part + 48, sC);
     // multiN variable point A_i
@@ -510,7 +530,7 @@ struct VReduceTask {
   ZK_HD void operator()(int b) const {
     using F = Tomq;
     using Fn = P256n;
-    if (c.gk_tape_bad && c.gk_tape_bad[b]) ZK_SET_STATUS(c.status + b, ZKA_ERR_TAPE_RANGE);   // after every exp-side status
+    if (c.gk_tape_bad && c.gk_tape_bad[b]) ZK_SET_STATUS(c.status + b, ZKA_ERR_TAPE_RANGE);   // behind MALFORMED, R at infinity
     uint32_t gW[8], hW[8], pX[8], pY[8], sR[8], sH[8], sC[8];
     zero_n<8>(gW); zero_n<8>(hW); zero_n<8>(pX); zero_n<8>(pY); zero_n<8>(sR); zero_n<8>(sH); zero_n<8>(sC);
     for (int j = 0; j < c.K; j++) {
@@ -1229,16 +1249,15 @@ struct VFinalTask {
     // the aggregate check of the chunk stands for every per-proof identity test of its group (zk_verify_agg.cuh)
     const bool tom_pass = c.agg_ctl && c.agg_ctl[AGG_TOM_PASS], nist_pass = c.agg_ctl && c.agg_ctl[AGG_NIST_PASS];
     const bool f[3] = {tom_pass || fl[0], tom_pass || fl[1], nist_pass || fl[2]};
-    const int st = c.status[b];
     const bool gk = c.gk_ok_len[b] && f[0];
-    if (st == ZKA_ERR_MALFORMED || st == ZKA_ERR_R_INFINITY) { c.ok[b] = 0; return; }
-    if (!gk) {
-      // verifyMembership returned false before verifyExp could throw: not an error
-      if (st != ZKA_ERR_TAPE_RANGE) c.status[b] = ZKA_OK;
-      c.ok[b] = 0;
-      return;
-    }
-    c.ok[b] = (st == ZKA_OK && f[1] && f[2]) ? 1 : 0;
+    c.ok[b] = 0;
+    // MALFORMED, R at infinity, a GK draw out of range: thrown before verifyMembership can return false
+    if (c.status[b] != ZKA_OK) return;
+    // verifyMembership returned false before verifyExp could throw: not an error
+    if (!gk) return;
+    const int key = c.vkey[b];
+    if (key != VK_NONE) c.status[b] = key & 15;
+    else c.ok[b] = (f[1] && f[2]) ? 1 : 0;
   }
 };
 

@@ -171,7 +171,7 @@ struct AggGateTask {
   VerifyCtx c;
   uint32_t* ctl;
   ZK_HD void operator()(int b) const {
-    if (c.status[b] != ZKA_OK || (c.mode == 0 && !c.gk_ok_len[b])) ctl[AGG_SKIP] = 1;
+    if (c.status[b] != ZKA_OK || c.vkey[b] != VK_NONE || (c.mode == 0 && !c.gk_ok_len[b])) ctl[AGG_SKIP] = 1;
   }
 };
 

@@ -2031,6 +2031,7 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
     c.nfix = w.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
     c.id_flags = w.take<uint8_t>((size_t)Bc * 3);
     c.gk_tape_bad = w.take_if<uint8_t>(mode == 0, Bc);
+    c.vkey = w.take<int32_t>(Bc);
     c.nent_scalar = w.take<uint32_t>((size_t)Bc * EN * 8);
     c.nent_aff = w.take<uint32_t>((size_t)Bc * EN * 16);
     c.nent_skip = w.take<uint8_t>((size_t)Bc * EN);
