@@ -148,10 +148,13 @@ int zka_prove_batch(zka_ctx* ctx, const zka_params* params, uint32_t B,
  * ok[i] = 1 iff the reference would return true.  The verifier tape holds, per proof, the
  * random relation scalars of Relation.drain (multimult.ts:168-173) and the 78 index draws of
  * generateIndices (exp.ts:95-109); layout in zk_verify.cuh.
- * Evaluation order (verdicts do not depend on it): every relation of every proof has its own random scalar, so the SUM
- * over a chunk of proofs of the reference's three linear combinations is checked first, as one wide-window MSM; only a
- * chunk whose sum is not the identity — some proof wrong, rejected by the parsers, or (tomEdwards256, cofactor 4)
- * carrying a small-order component — is evaluated proof by proof with the same scalars (zka_stat). */
+ * Evaluation order (verdicts do not depend on it): a WEIGHTED sum over a chunk of proofs of the reference's three
+ * linear combinations is checked first, as one wide-window MSM per group; each combination of each row is scaled by a
+ * 128-bit weight from SHA-256 over the row's index in the call, ring index, message, tape row and the proof bytes the
+ * verifier reads, so rows that share a tape row (or a seed), or a prover who knows the tape, cannot pick residuals that
+ * cancel against the weights — the tape needs no property beyond the reference's own (limits: zk_verify_agg.cuh).
+ * Only a chunk whose sum is not the identity — some proof wrong, rejected by the parsers, or (tomEdwards256, cofactor 4)
+ * carrying a small-order component — is evaluated proof by proof with the reference's scalars (zka_stat). */
 int zka_verify_batch(zka_ctx* ctx, const zka_params* params, uint32_t B,
                      const uint8_t* msg_hash /* B x 32 */, const uint8_t* ring /* N x 32 */, uint32_t N,
                      const uint8_t* proofs /* B x proof_stride */, size_t proof_stride,

@@ -154,8 +154,7 @@ struct Sha256 {
       if (j < nf) put4(t[j]);
     for (int k = 0; k < (n & 3); k++) put((uint8_t)(t[16] >> (8 * k)));   // n in [64,68): the tail lives in t[16]
   }
-  // digest[0..9] as (hi16, lo64): challenge = hi16 * 2^64 + lo64
-  ZK_HD void final80(uint32_t* c3) {  // c3[0] = low 32, c3[1] = mid 32, c3[2] = top 16 bits
+  ZK_HD void pad() {
     const uint64_t bits = total * 8;
     put(0x80);
     while ((fill & 3) != 0) put(0);
@@ -167,6 +166,16 @@ struct Sha256 {
     push_word((uint32_t)(bits >> 32));
     push_word((uint32_t)bits);
     compress();
+  }
+  // the whole digest as eight big-endian words
+  ZK_HD void final256(uint32_t* d8) {
+    pad();
+#pragma unroll
+    for (int i = 0; i < 8; i++) d8[i] = h[i];
+  }
+  // digest[0..9] as (hi16, lo64): challenge = hi16 * 2^64 + lo64
+  ZK_HD void final80(uint32_t* c3) {  // c3[0] = low 32, c3[1] = mid 32, c3[2] = top 16 bits
+    pad();
     // digest bytes 0..9 = h0 (4) h1 (4) top half of h2 (2)  -> 80-bit big-endian integer
     uint32_t top16 = h[0] >> 16;
     uint32_t mid = (h[0] << 16) | (h[1] >> 16);

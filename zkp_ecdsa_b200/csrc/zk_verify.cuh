@@ -44,9 +44,12 @@ enum : int {
   MSM_NWIN_N = 65,             // 65 windows cover the 257 bits of k + offset (msm_digit4)
   // control words of the chunk-wide aggregate check (zk_verify_agg.cuh)
   AGG_SKIP = 0,                // != 0: some proof of the chunk is not eligible, the aggregate kernels return at once
-  AGG_TOM_PASS = 1,            // != 0: sum_b (GK_b + W_b) is the identity -> the per-proof tomEdwards256 MSMs are skipped
-  AGG_NIST_PASS = 2,           // != 0: sum_b N_b is the identity -> the per-proof P-256 MSMs are skipped
+  AGG_TOM_PASS = 1,            // != 0: sum_b (wG_b GK_b + wW_b W_b) is the identity -> the per-proof tomEdwards256 MSMs are skipped
+  AGG_NIST_PASS = 2,           // != 0: sum_b wN_b N_b is the identity -> the per-proof P-256 MSMs are skipped
   AGG_CTL_WORDS = 4,
+  // the aggregate's weights of a row (zk_verify_agg.cuh): one per combination, in the order of the fixed-base jobs
+  // (0: GK, 1: multiW), then multiN
+  AGG_W_GK = 0, AGG_W_W = 1, AGG_W_N = 2, AGG_WT = 3,
 };
 
 // Status precedence of a row (include/zkattest.h): the reference throws at the first defect it meets, so a row with several
@@ -93,6 +96,7 @@ struct VerifyCtx {
   uint32_t* gk_off;     // [B]
   uint32_t* tagbits;    // [B][3] tag of each repetition (bit i)
   uint32_t* chal;       // [B][3]
+  uint32_t* chal_full;  // [B][8] or null: the whole SHA-256 of the exp challenge (the aggregate's weights)
   uint8_t* gk_ok_len;   // [B] 1 if the GK length check passes (gk.ts:208-218)
   uint8_t* gk_tape_bad; // [B] or null: a GK draw was out of range — recorded here and folded into status[] by VReduceTask when
                         //     the GK chain runs beside the exp chain (same precedence as running it after), else written at once
@@ -129,6 +133,7 @@ struct VerifyCtx {
   // fixed-base parts: tom jobs [B][2] (0: GK, 1: W) and their points; P-256 fixed part
   uint32_t *fx_jv, *fx_jr, *fx_proj;   // [B*2]
   uint32_t* nfix;       // [B][24] projective sR*R + shN*h
+  uint32_t* nfix_k;     // [B][2][8] or null: sR, shN of nfix (canonical mod n) for the aggregate's weighted copy
   // MSM window sums and verdicts
   uint32_t* win_w;      // [B][MSM_NWIN][36]
   uint32_t* win_g;      // [B][MSM_NWIN][36]
@@ -311,6 +316,7 @@ struct VChallengeTask {
     uint32_t c3[3];
     h.final80(c3);
     st<3>(c.chal + (size_t)b * 3, c3);
+    if (c.chal_full) st<8>(c.chal_full + (size_t)b * 8, h.h);
     // Knuth shuffle with the pre-filtered index bytes: j = rnd(limit - i) + i
     uint8_t perm[MAX_REPS];
     for (int i = 0; i < c.S; i++) perm[i] = (uint8_t)i;
@@ -568,6 +574,10 @@ struct VReduceTask {
     p256_accum_rtab(acc, c.rtab + (size_t)b * RT_ENTRIES * P256_AFF_WORDS, kR);
     p256_accum_fixed(acc, c.h_tab8, kH, c.h_w);
     p256_st_proj(c.nfix + (size_t)b * P256_PROJ_WORDS, acc);
+    if (c.nfix_k) {   // for the aggregate's weighted copy (AggNistFixWeightTask); the per-proof path reads nfix
+      st<8>(c.nfix_k + (size_t)b * 16, kR);
+      st<8>(c.nfix_k + (size_t)b * 16 + 8, kH);
+    }
   }
 };
 

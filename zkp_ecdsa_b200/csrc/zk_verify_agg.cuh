@@ -1,14 +1,26 @@
 // zk_verify_agg.cuh — chunk-wide aggregate check of the verifier ("all proofs of the chunk at once").
 //
 // verifySignatureList (/root/reference/src/zkpAttestList.ts:147-184) answers `isIdentity()` of three linear
-// combinations per proof (GK, multiW, multiN; /root/reference/src/curves/multimult.ts:147-174 gives every relation its
-// own uniformly random scalar).  Because every relation of every proof carries an INDEPENDENT random scalar, the sum
-// of the combinations of all proofs of a chunk is itself a random linear combination of all their relations:
+// combinations per proof (GK, multiW, multiN; /root/reference/src/curves/multimult.ts:147-174 gives every relation of a
+// proof its own random scalar drawn from the verify tape).  The tape is an input: rows of one call may share a tape row
+// or a seed, and a prover may know it, so the tape scalars of DIFFERENT rows (or of GK and multiW of one row) need not be
+// independent — two rejected rows whose residuals cancel would pass an unweighted sum.  Each combination of each row is
+// therefore scaled by a weight of its own before the sums (AggWeightTask):
 //
-//     sum_b (GK_b + W_b) == O  and  sum_b N_b == O      <=>  (w.h.p.)  every single combination is O.
+//     sum_b (wG_b GK_b + wW_b W_b) == O  and  sum_b wN_b N_b == O      <=>  (w.h.p.)  every single combination is O.
+//
+// The weights are 128-bit values from SHA-256 over the row's index in the call, the index of its ring, its message, its
+// tape row and the proof bytes the verifier reads.  They change with every proof byte a residual depends on, so a
+// prover cannot pick one row's residual after seeing that row's weight, and the index separates rows that share
+// everything else; the argument needs no property of the tape beyond the reference's own.  Two limits: a weight
+// depends on its own row only, so a prover who knows the tapes and controls k rows of a chunk can search for rows whose
+// weighted residuals sum to O (a k-list birthday problem, about k 2^(256 / (1 + lg k)) hashes: 2^36 for k = 256) —
+// but with a known tape it can forge each row against the reference's own per-row check directly, so this adds no
+// weakness beyond the reference's; and the ring's keys, like the tape, are the verifier's input and are not hashed.
+// The weights are odd (non-zero mod both prime orders) and the per-proof path never sees them.
 //
 // The per-proof evaluation (zk_verify.cuh: one thread per (proof, 6-bit window), 43 x (n_b + 64) point operations with
-// n_b ~ 375) is therefore needed only when the sum is NOT the identity.  The sum itself is ONE multi-scalar
+// n_b ~ 375) is therefore needed only when a sum is NOT the identity.  Each sum is ONE multi-scalar
 // multiplication over all variable points of the chunk (~1.5 M tomEdwards256 points for 4096 proofs), evaluated with
 // wide windows: signed c-bit digits (c = 12..16), counting sort of the entries by bucket, one thread per (window,
 // bucket) summing its entries in registers, and a tree of weighted running sums over the buckets:
@@ -18,8 +30,8 @@
 //   fail (some proof is wrong, or some proof was already rejected by the parsers): the per-proof kernels run
 //          exactly as before, so every verdict and status is the one the per-proof path gives.
 // The verdict of a VALID batch is unchanged; for an invalid proof the per-proof path decides, under the same tape.
-// tomEdwards256 has cofactor 4: a chunk in which some proof's points carry a small-order component also goes to the
-// per-proof path (AggTorsionTask), because such components of two proofs could cancel in the sum.
+// tomEdwards256 has cofactor 4: a chunk in which some combination of some proof keeps a small-order component also goes
+// to the per-proof path (AggTorsionTask), because the sums only vouch for the prime-order parts.
 #pragma once
 #include <string.h>
 
@@ -39,6 +51,89 @@ enum : int {
   AGG_SEG = 256,      // buckets per segment of the prefix sum
   AGG_MAX_LEVELS = 6,
   AGG_FAN_BITS = 3,   // log2 of the largest fan-in of a reduction level (short latency chains: 7 x 3 additions)
+  AGG_PIECE = 2048,   // bytes of tape per leaf of a row's digest tree
+};
+
+// ---- the rows' weights ---------------------------------------------------------------------------------------------
+// A row's combinations depend on its message, ring and tape row and on the proof bytes the verifier reads: the header,
+// the tag bits, every repetition's A, Tx, Ty (only through the exp challenge, whose full SHA-256 VChallengeTask keeps),
+// the sampled repetitions and the GK block.  A row's digest is SHA-256 over a domain tag, its index in the call, its
+// ring, its message, its tag bits, the challenge digest, its header and the digests of the pieces: AGG_PIECE-byte pieces
+// of its tape row, each sampled repetition, the GK block (a two-level tree: the pieces hash in parallel).  Bytes the
+// verifier never reads (the unsampled repetitions' responses) cannot move a residual and are left out.  Weight j = the
+// first 128 bits of SHA-256(digest || j), made odd, in Montgomery form mod the group order of its combination: odd and
+// below 2^128, so non-zero mod tom.order and mod p256.n.
+ZK_HD int agg_tape_pieces(size_t tape_len) { return (int)((tape_len + AGG_PIECE - 1) / AGG_PIECE); }
+struct AggPieceTask {   // one thread per (row, piece): tp tape pieces, K sampled repetitions, the GK block
+  VerifyCtx c;
+  size_t tape_len;
+  int tp, np;           // np = tp + K + 1
+  uint32_t* dig;        // [B][np][8]
+  ZK_HD void operator()(int t) const {
+    const int b = t / np, j = t % np;
+    const uint32_t plen = c.proof_len[b] < c.proof_stride ? c.proof_len[b] : (uint32_t)c.proof_stride;
+    const uint8_t* p;
+    long lo, hi;
+    if (j < tp) {
+      p = c.tape_of(b);
+      lo = (long)j * AGG_PIECE;
+      hi = lo + AGG_PIECE < (long)tape_len ? lo + AGG_PIECE : (long)tape_len;
+    } else {
+      // a row the parsers rejected never reaches the aggregate: its offsets (parked at 0) only have to stay in bounds
+      p = c.proof_of(b);
+      if (j < tp + c.K) {
+        const int i = (int)c.samp_idx[(size_t)b * c.K + (j - tp)];
+        const uint32_t tag = (c.tagbits[(size_t)b * 3 + (i >> 5)] >> (i & 31)) & 1u;
+        lo = c.rep_off[(size_t)b * c.S + i];
+        hi = lo + (tag ? REP1_LEN : REP0_LEN);
+      } else {
+        lo = c.gk_off[b];
+        hi = plen;
+      }
+      if (hi > (long)plen) hi = plen;
+      if (lo > hi) lo = hi;
+    }
+    Sha256 h;
+    h.init();
+    h.update(p + lo, (int)(hi - lo));
+    h.final256(dig + (size_t)t * 8);
+  }
+};
+struct AggWeightTask {  // one thread per row
+  VerifyCtx c;
+  const uint32_t *chal_full, *dig;
+  uint32_t row0;        // index in the call of the chunk's first row
+  int np;
+  uint32_t* wt;         // [B][AGG_WT][8]
+  ZK_HD void operator()(int b) const {
+    const uint32_t head[4] = {0x5741475au /* "ZGAW" */, row0 + (uint32_t)b, c.ring_of ? c.ring_of[b] : 0u, c.proof_len[b]};
+    Sha256 h;
+    h.init();
+    h.update(reinterpret_cast<const uint8_t*>(head), (int)sizeof(head));
+    h.update(c.msg_hash + (size_t)b * 32, 32);
+    h.update(reinterpret_cast<const uint8_t*>(c.tagbits + (size_t)b * 3), 12);
+    h.update(reinterpret_cast<const uint8_t*>(chal_full + (size_t)b * 8), 32);
+    h.update(c.proof_of(b), c.proof_stride < HEAD_LEN ? (int)c.proof_stride : HEAD_LEN);
+    h.update(reinterpret_cast<const uint8_t*>(dig + (size_t)b * np * 8), np * 32);
+    uint32_t d[9];
+    h.final256(d);
+    for (int j = 0; j < AGG_WT; j++) {
+      d[8] = (uint32_t)j;
+      Sha256 g;
+      g.init();
+      g.update(reinterpret_cast<const uint8_t*>(d), 36);
+      uint32_t o[8], w[8];
+      g.final256(o);
+      zero_n<8>(w);
+      w[0] = o[3] | 1u;
+      w[1] = o[2];
+      w[2] = o[1];
+      w[3] = o[0];
+      if (j == AGG_W_N) P256n::to_mont(o, w);
+      else Tomq::to_mont(o, w);
+      st<8>(wt + ((size_t)b * AGG_WT + j) * 8, o);
+    }
+  }
 };
 
 // signed c-bit digits of a 256-bit scalar without a carry chain (see msm_digit6): with offs = sum_j 2^(c-1) 2^(c j)
@@ -118,6 +213,7 @@ inline AggPlan agg_plan(double entries, int c_forced) {
 struct AggTomSrc {
   const uint32_t *ent_scalar, *ent_pre, *ent_cnt, *gk_scalar, *gk_pre;
   int B, ET, K, ngk;   // slots [0, B*ET): multiW entries (K samples x 34 + keyXcom, keyYcom); then B*ngk GK entries
+  const uint32_t* wt;  // [B][AGG_WT][8] the rows' weights (AggWeightTask)
   using Pt = TomPt;
   enum { PTW = PG_EXT_WORDS };
   ZK_HD int slots() const { return B * (ET + ngk); }
@@ -129,6 +225,15 @@ struct AggTomSrc {
   }
   ZK_HD const uint32_t* scalar(int s) const {
     return s < B * ET ? ent_scalar + (size_t)s * 8 : gk_scalar + (size_t)(s - B * ET) * 8;
+  }
+  // the scalar the aggregate MSM uses: times the weight of the slot's row and combination (multiW or GK)
+  ZK_HD void load(uint32_t* k, int s) const {
+    ld<8>(k, scalar(s));
+    const bool w = s < B * ET;
+    const int b = w ? s / ET : (s - B * ET) / ngk;
+    uint32_t m[8];
+    ld<8>(m, wt + ((size_t)b * AGG_WT + (w ? AGG_W_W : AGG_W_GK)) * 8);
+    Tomq::mul(k, k, m);
   }
   ZK_HD void accumulate(Pt& acc, int s, bool neg) const {
     TomPre pt;
@@ -147,11 +252,18 @@ struct AggNistSrc {
   const uint32_t *scalar_, *aff;
   const uint8_t* skip;
   int B, EN;
+  const uint32_t* wt;
   using Pt = P256Pt;
   enum { PTW = 24 };
   ZK_HD int slots() const { return B * EN; }
   ZK_HD bool used(int s) const { return skip[s] == 0; }
   ZK_HD const uint32_t* scalar(int s) const { return scalar_ + (size_t)s * 8; }
+  ZK_HD void load(uint32_t* k, int s) const {
+    ld<8>(k, scalar(s));
+    uint32_t m[8];
+    ld<8>(m, wt + ((size_t)(s / EN) * AGG_WT + AGG_W_N) * 8);
+    P256n::mul(k, k, m);
+  }
   ZK_HD void accumulate(Pt& acc, int s, bool neg) const {
     P256Aff q;
     p256_ld_aff(q, aff + (size_t)s * P256_AFF_WORDS);
@@ -178,18 +290,21 @@ struct AggGateTask {
 #if !defined(ZKA_PG_WAR256)
 // A0b — tomEdwards256 has cofactor 4, and deserializePoint (edwards.ts:70-86) only checks the curve equation.  Points
 // with a small-order component make the reference's own verdict depend on its randomizers (a component of order 2
-// survives a relation iff its scalar is odd); two such proofs in one chunk could cancel each other's components in the
-// SUM although neither per-proof combination is the identity.  The aggregate verdict is therefore used only when no
-// proof of the chunk carries such a component:  with tau the projection onto E[4],  tau(sum_e s_e P_e) =
-// sum_e (s_e mod 4) tau(P_e) = tau(W_b)  for  W_b = sum_e (s_e mod 4) P_e  (fixed-base parts are multiples of g, h:
-// prime order), and  q W_b = (q mod 4) tau(W_b) = -tau(W_b)  (q = p256.p = 3 mod 4).  ~n_b mixed additions and 256
-// doublings per proof; q = 2^256 - 2^224 + 2^192 + 2^96 - 1 costs four more additions.
-// Two steps: partial sums per (proof, sampled repetition) — the last part takes keyXcom, keyYcom and the GK points —
-// then one thread per proof for the 2 (K + 1) additions and the doubling chain.
+// survives a relation iff its scalar is odd).  The weighted sums only vouch for the prime-order parts of the
+// combinations, so the aggregate verdict is used only when no combination of any proof keeps a small-order component
+// under the reference's OWN scalars (the unweighted ones: a weighted scalar is reduced mod q, which changes it mod 4).
+// With tau the projection onto E[4],  tau(C) = sum_e (s_e mod 4) tau(P_e) = tau(W)  for  W = sum_e (s_e mod 4) P_e
+// (fixed-base parts are multiples of g, h: prime order), and  q W = (q mod 4) tau(W) = -tau(W)  (q = p256.p = 3 mod 4).
+// GK and multiW are checked apart: the reference rejects a row whose GK keeps a component that its multiW cancels.
+// Then for every row  C = pi(C)  (pi: the prime-order part), and a weighted sum that is O has every pi(C) = O (w.h.p.).
+// ~n_b mixed additions and 256 doublings per combination; q = 2^256 - 2^224 + 2^192 + 2^96 - 1 costs four more
+// additions.  Two steps: partial sums per (proof, part) — parts 0..K-1 the sampled repetitions, part K keyXcom and
+// keyYcom (multiW), part K + 1 the GK points — then one thread per (proof, combination) for the additions and the
+// doubling chain.
 struct AggTorsionPartTask {   // one thread per (proof, part, bit of s mod 4): ONE accumulator per thread (two spilled)
   AggTomSrc src;
   const uint32_t* ctl;
-  uint32_t* part;    // [B][K + 1][2][PG_EXT_WORDS]: sums of the points with bit 0 / bit 1 of (s mod 4) set
+  uint32_t* part;    // [B][K + 2][2][PG_EXT_WORDS]: sums of the points with bit 0 / bit 1 of (s mod 4) set
   ZK_HD void add_range(TomPt& a, uint32_t mask, int s0, int cnt) const {
     for (int e = 0; e < cnt; e++) {
       const int s = s0 + e;
@@ -200,50 +315,49 @@ struct AggTorsionPartTask {   // one thread per (proof, part, bit of s mod 4): O
   ZK_HD void operator()(int t) const {
     if (ctl[AGG_SKIP]) return;
     const int bit = t & 1, bj = t >> 1;
-    const int b = bj / (src.K + 1), j = bj % (src.K + 1);
+    const int b = bj / (src.K + 2), j = bj % (src.K + 2);
     const uint32_t mask = 1u << bit;
     TomPt a;
     tom_set_identity(a);
-    if (j < src.K) {
-      add_range(a, mask, b * src.ET + j * V_ENT_PER_SAMPLE, V_ENT_PER_SAMPLE);
-    } else {
-      add_range(a, mask, b * src.ET + src.K * V_ENT_PER_SAMPLE, src.ET - src.K * V_ENT_PER_SAMPLE);
-      add_range(a, mask, src.B * src.ET + b * src.ngk, src.ngk);
-    }
+    if (j < src.K) add_range(a, mask, b * src.ET + j * V_ENT_PER_SAMPLE, V_ENT_PER_SAMPLE);
+    else if (j == src.K) add_range(a, mask, b * src.ET + src.K * V_ENT_PER_SAMPLE, src.ET - src.K * V_ENT_PER_SAMPLE);
+    else add_range(a, mask, src.B * src.ET + b * src.ngk, src.ngk);
     bk_store(reinterpret_cast<U4*>(part + (size_t)t * PG_EXT_WORDS), a);
   }
 };
-struct AggTorsionTask {
+struct AggTorsionTask {   // one thread per (proof, combination): t = 2 b + (0: GK, 1: multiW)
   const uint32_t* part;
   uint32_t* ctl;
   int K;
-  ZK_HD void operator()(int b) const {
+  ZK_HD void operator()(int t) const {
     if (ctl[AGG_SKIP]) return;
+    const int b = t >> 1;
+    const int j0 = (t & 1) ? 0 : K + 1, j1 = (t & 1) ? K : K + 1;
     TomPt a1, a2, p;
     tom_set_identity(a1);
     tom_set_identity(a2);
-    for (int j = 0; j <= K; j++) {
-      const uint32_t* o = part + ((size_t)b * (K + 1) + j) * 2 * PG_EXT_WORDS;
+    for (int j = j0; j <= j1; j++) {
+      const uint32_t* o = part + ((size_t)b * (K + 2) + j) * 2 * PG_EXT_WORDS;
       bk_load(p, reinterpret_cast<const U4*>(o));
       tom_add(a1, a1, p);
       bk_load(p, reinterpret_cast<const U4*>(o + PG_EXT_WORDS));
       tom_add(a2, a2, p);
     }
-    TomPt w, t, r;
+    TomPt w, r;
     tom_dbl(a2, a2);
-    tom_add(w, a1, a2);           // W_b
-    t = w;
-    for (int i = 0; i < 96; i++) tom_dbl(t, t);
+    tom_add(w, a1, a2);           // W
+    TomPt tt = w;
+    for (int i = 0; i < 96; i++) tom_dbl(tt, tt);
     tom_neg(r, w);
-    tom_add(r, r, t);             // 2^96 W - W
-    for (int i = 96; i < 192; i++) tom_dbl(t, t);
-    tom_add(r, r, t);             // + 2^192 W
-    for (int i = 192; i < 224; i++) tom_dbl(t, t);
+    tom_add(r, r, tt);            // 2^96 W - W
+    for (int i = 96; i < 192; i++) tom_dbl(tt, tt);
+    tom_add(r, r, tt);            // + 2^192 W
+    for (int i = 192; i < 224; i++) tom_dbl(tt, tt);
     TomPt n;
-    tom_neg(n, t);
+    tom_neg(n, tt);
     tom_add(r, r, n);             // - 2^224 W
-    for (int i = 224; i < 256; i++) tom_dbl(t, t);
-    tom_add(r, r, t);             // + 2^256 W
+    for (int i = 224; i < 256; i++) tom_dbl(tt, tt);
+    tom_add(r, r, tt);            // + 2^256 W
     if (!pg_is_identity(r)) ctl[AGG_SKIP] = 1;
   }
 };
@@ -259,7 +373,7 @@ struct AggHistTask {
   ZK_HD void operator()(int s) const {
     if (ctl[AGG_SKIP] || !src.used(s)) return;
     uint32_t k[8], kp[10];
-    ld<8>(k, src.scalar(s));
+    src.load(k, s);
     agg_kp(kp, k, D);
     for (int w = 0; w < D.nwin; w++) {
       const int d = agg_digit(kp, w, D.c);
@@ -328,7 +442,7 @@ struct AggScatterTask {
   ZK_HD void operator()(int s) const {
     if (ctl[AGG_SKIP] || !src.used(s)) return;
     uint32_t k[8], kp[10];
-    ld<8>(k, src.scalar(s));
+    src.load(k, s);
     agg_kp(kp, k, D);
     for (int w = 0; w < D.nwin; w++) {
       const int d = agg_digit(kp, w, D.c);
@@ -425,10 +539,11 @@ ZK_HD void agg_horner(typename Src::Pt& acc, const uint32_t* rootA, const uint32
 }
 
 // ---- fixed-base parts -------------------------------------------------------------------------------------------
-// tomEdwards256: sum_b (v_b0 g + r_b0 h + v_b1 g + r_b1 h) = (sum v) g + (sum r) h — the SCALARS are summed (mod the
-// group order) and ONE fixed-base commitment is evaluated for the whole chunk.
+// tomEdwards256: sum_b (wG_b (v_b0 g + r_b0 h) + wW_b (v_b1 g + r_b1 h)) = (sum w v) g + (sum w r) h — the weighted
+// SCALARS are summed (mod the group order) and ONE fixed-base commitment is evaluated for the whole chunk.
 struct AggFixPartTask {   // one thread per group of 32 proofs
-  const uint32_t *ctl, *fx_jv, *fx_jr;   // [B*2][8] canonical mod q
+  const uint32_t *ctl, *fx_jv, *fx_jr;   // [B*2][8] canonical mod q (job 0: GK, job 1: multiW)
+  const uint32_t* wt;                    // [B][AGG_WT][8]
   uint32_t* part;                        // [groups][2][8]
   int B;
   ZK_HD void operator()(int g) const {
@@ -437,9 +552,11 @@ struct AggFixPartTask {   // one thread per group of 32 proofs
     uint32_t sv[8], sr[8], t[8];
     zero_n<8>(sv);
     zero_n<8>(sr);
+    uint32_t m[8];
     for (int i = g * 64; i < (g + 1) * 64 && i < B * 2; i++) {
-      ld<8>(t, fx_jv + (size_t)i * 8); F::add(sv, sv, t);
-      ld<8>(t, fx_jr + (size_t)i * 8); F::add(sr, sr, t);
+      ld<8>(m, wt + ((size_t)(i >> 1) * AGG_WT + (i & 1)) * 8);   // job i & 1 = weight AGG_W_GK / AGG_W_W
+      ld<8>(t, fx_jv + (size_t)i * 8); F::mul(t, t, m); F::add(sv, sv, t);
+      ld<8>(t, fx_jr + (size_t)i * 8); F::mul(t, t, m); F::add(sr, sr, t);
     }
     st<8>(part + (size_t)g * 16, sv);
     st<8>(part + (size_t)g * 16 + 8, sr);
@@ -462,7 +579,27 @@ struct AggFixSumTask {
     st<8>(jr, sr);
   }
 };
-// P-256: sum_b (sR_b R_b + shN_b h) — R differs per proof, so the POINTS are summed: a tree of 32-way partial sums
+// P-256: sum_b wN_b (sR_b R_b + shN_b h) — R differs per proof, so the POINTS are summed: each row's weighted fixed part
+// from its weighted scalars (the per-proof path keeps the unweighted nfix), then a tree of 32-way partial sums
+struct AggNistFixWeightTask {   // one thread per proof
+  const uint32_t *ctl, *k, *wt, *rtab, *h_tab8;   // k: [B][2][8] sR, shN (VReduceTask)
+  int h_w;
+  uint32_t* out;                                  // [B][24]
+  ZK_HD void operator()(int b) const {
+    if (ctl[AGG_SKIP]) return;
+    uint32_t m[8], kR[8], kH[8];
+    ld<8>(m, wt + ((size_t)b * AGG_WT + AGG_W_N) * 8);
+    ld<8>(kR, k + (size_t)b * 16);
+    ld<8>(kH, k + (size_t)b * 16 + 8);
+    P256n::mul(kR, kR, m);
+    P256n::mul(kH, kH, m);
+    P256Pt acc;
+    p256_set_identity(acc);
+    p256_accum_rtab(acc, rtab + (size_t)b * RT_ENTRIES * P256_AFF_WORDS, kR);
+    p256_accum_fixed(acc, h_tab8, kH, h_w);
+    p256_st_proj(out + (size_t)b * P256_PROJ_WORDS, acc);
+  }
+};
 struct AggNistFixPartTask {
   const uint32_t *ctl, *in;     // [count][24]
   uint32_t* part;               // [ceil(count / 32)][24]

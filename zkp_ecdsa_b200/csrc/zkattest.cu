@@ -287,7 +287,7 @@ struct Lane {
   // run side by side)
   DevBuf w[51];
   DevBuf in[2][10], out[2][3];
-  DevBuf agg[8], agg_tom[5 + 2 * AGG_MAX_LEVELS], agg_nist[5 + 2 * AGG_MAX_LEVELS];
+  DevBuf agg[9], agg_tom[5 + 2 * AGG_MAX_LEVELS], agg_nist[5 + 2 * AGG_MAX_LEVELS];
   std::string err;
   ~Lane() {
     for (int i = 0; i < 2; i++) {
@@ -2042,6 +2042,13 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
     c.win_g = w.take<uint32_t>((size_t)Bc * MSM_NWIN * 36);
     c.win_n = w.take<uint32_t>((size_t)Bc * MSM_NWIN_N * P256_PROJ_WORDS);
     c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * gk_blocks(n) * 8);
+    const bool agg = ctx->agg && mode == 0;
+    const size_t agg_tape_len = verify_tape_len(n, S, K);
+    const int agg_tp = agg_tape_pieces(agg_tape_len), agg_np = agg_tp + K + 1;
+    uint32_t* agg_wt = w.take_if<uint32_t>(agg, (size_t)Bc * AGG_WT * 8);
+    uint32_t* agg_dig = w.take_if<uint32_t>(agg, (size_t)Bc * agg_np * 8);
+    c.chal_full = w.take_if<uint32_t>(agg, (size_t)Bc * 8);
+    c.nfix_k = w.take_if<uint32_t>(agg, (size_t)Bc * 16);
     Cursor ob(ln.out[0]);
     c.ok = oo.rows(ob.next(), b0, Bc);
     c.status = so.rows(ob.next(), b0, Bc);
@@ -2066,6 +2073,15 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
     if (gk_fork) {
       ev_record(ln.ev_fork, st);
       ev_wait(ln.aux[1], ln.ev_fork);
+    }
+    if (agg) {
+      // the aggregate's weights (zk_verify_agg.cuh) need the layout, the sampled repetitions and the exp challenge: they
+      // hash ahead of the GK chain on its side stream (joined before VReduceTask)
+      Stream& sw = gk_fork ? ln.aux[1] : st;
+      launch(sw, (long long)Bc * agg_np, AggPieceTask{c, agg_tape_len, agg_tp, agg_np, agg_dig});
+      launch(sw, Bc, AggWeightTask{c, c.chal_full, agg_dig, b0, agg_np, agg_wt});
+    }
+    if (gk_fork) {
       verify_gk(ln.aux[1], c, gk_offs);
       ev_record(ln.ev_join[1], ln.aux[1]);
     }
@@ -2091,23 +2107,24 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
     // combinations, as ONE wide-window MSM per group; when both sums are the identity the per-proof MSMs below
     // return at once
     uint32_t* ctl = nullptr;
-    if (ctx->agg && mode == 0) {
+    if (agg) {
       Cursor A(ln.agg);
       const int fgroups = (Bc * 2 + 63) / 64, ngroups = (Bc + 31) / 32, ngroups2 = (ngroups + 31) / 32;
       ctl = A.take<uint32_t>(AGG_CTL_WORDS);
 #if !defined(ZKA_PG_WAR256)
-      uint32_t* tpart = A.take<uint32_t>((size_t)Bc * (K + 1) * 2 * PG_EXT_WORDS);
+      uint32_t* tpart = A.take<uint32_t>((size_t)Bc * (K + 2) * 2 * PG_EXT_WORDS);
 #endif
       uint32_t* fpart = A.take<uint32_t>((size_t)fgroups * 16);
       uint32_t* fjv = A.take<uint32_t>(8);
       uint32_t* fjr = A.take<uint32_t>(8);
       uint32_t* fproj = A.take<uint32_t>(TOM_PROJ_WORDS);
+      uint32_t* nfix_w = A.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
       uint32_t* npart = A.take<uint32_t>((size_t)ngroups * P256_PROJ_WORDS);
       uint32_t* npart2 = A.take_if<uint32_t>(ngroups > 32, (size_t)ngroups2 * P256_PROJ_WORDS);
       dev_memset(st, ctl, 0, AGG_CTL_WORDS * 4);
       launch(st, Bc, AggGateTask{c, ctl});
-      const AggTomSrc tsrc{c.ent_scalar, c.ent_pre, c.ent_cnt, c.gk_scalar, c.gk_pre, Bc, ET, K, ngk};
-      const AggNistSrc nsrc{c.nent_scalar, c.nent_aff, c.nent_skip, Bc, EN};
+      const AggTomSrc tsrc{c.ent_scalar, c.ent_pre, c.ent_cnt, c.gk_scalar, c.gk_pre, Bc, ET, K, ngk, agg_wt};
+      const AggNistSrc nsrc{c.nent_scalar, c.nent_aff, c.nent_skip, Bc, EN, agg_wt};
       // three independent chains from here to AggFinalTask: the tomEdwards256 MSM (this stream), the torsion guard and the
       // P-256 MSM with its fixed parts (two side streams; with per-kernel profiling on, everything stays on one stream
       // so that the event pairs time one kernel at a time).  A skip flag raised by the torsion guard may reach the MSM
@@ -2122,8 +2139,8 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
       }
 #if !defined(ZKA_PG_WAR256)
       // cofactor 4: no small-order components, or the per-proof path decides
-      launch(sa, (long long)Bc * (K + 1) * 2, AggTorsionPartTask{tsrc, ctl, tpart});
-      launch(sa, Bc, AggTorsionTask{tpart, ctl, K});
+      launch(sa, (long long)Bc * (K + 2) * 2, AggTorsionPartTask{tsrc, ctl, tpart});
+      launch(sa, (long long)Bc * 2, AggTorsionTask{tpart, ctl, K});
 #endif
       const AggPlan tp = agg_plan((double)Bc * (0.5 * K * V_ENT_PER_SAMPLE + 2 + ngk), ctx->agg_c);
       const AggPlan np = agg_plan((double)Bc * EN, 0);
@@ -2131,11 +2148,13 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
       const uint32_t *tA, *tB, *nA, *nB;
       agg_msm(st, Cursor(ln.agg_tom), tsrc, tp, ctl, &tA, &tB);
       agg_msm(sb, Cursor(ln.agg_nist), nsrc, np, ctl, &nA, &nB);
-      // fixed-base parts: one commitment for the summed tomEdwards256 scalars, a two-level sum of the P-256 points
-      launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, fpart, Bc});
+      // fixed-base parts: one commitment for the summed weighted tomEdwards256 scalars, a two-level sum of the weighted
+      // P-256 points
+      launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, agg_wt, fpart, Bc});
       launch(st, 1, AggFixSumTask{ctl, fpart, fjv, fjr, fgroups});
       launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom, 1});
-      launch(sb, ngroups, AggNistFixPartTask{ctl, c.nfix, npart, Bc});
+      launch(sb, Bc, AggNistFixWeightTask{ctl, c.nfix_k, agg_wt, c.rtab, c.h_tab8, c.h_w, nfix_w});
+      launch(sb, ngroups, AggNistFixPartTask{ctl, nfix_w, npart, Bc});
       int nleft = ngroups;            // second level: at most Bc / 1024 partial sums reach the final thread
       const uint32_t* nsum = npart;
       if (nleft > 32) {
