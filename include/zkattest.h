@@ -54,6 +54,26 @@
  * pk = s1 * R - Q: the signer is deanonymised.  The domains keep a seed's prover and verifier streams apart; they do not
  * make reuse safe.  Draw seeds from the OS CSPRNG.
  *
+ * Hedged seeds (zka_prove_batch_hedged, zka_prove_batch_rings_hedged, zka_hedge_seeds[_rings]).  The seed of each row is
+ * derived on the GPU from the caller's seed, the statement and the signature (as RFC 6979 and its hedged variants derive
+ * a signature nonce), and then expanded by the seeded rule above.  Byte strings, || = concatenation:
+ *   params digest  SHA-256("ZKAttest/hedge/params/v1" || proof-group name, NUL-padded to 16 bytes || h_nist (65) ||
+ *                  h_proof (point_bytes) || le32(sec_level)), computed once by zka_params_create.
+ *   ring digest    of a ring of N entries, depth n = ceil(log2 N): e_j = ring[j] mod the proof-group order as 32 bytes
+ *                  big-endian for j < 2^n, the padding entries being e_0 (gk.ts:75-86); leaf k = SHA-256(e_{1024k} || ... ||
+ *                  e_{1024k+1023}), one leaf of all 2^n entries when 2^n <= 1024; digest = SHA-256("ZKAttest/hedge/ring/v1" ||
+ *                  le32(N) || le32(n) || leaf_0 || leaf_1 || ...).  Computed on the GPU once per one-ring call, and for every
+ *                  ring of a set once by zka_rings_create.
+ *   row seed       SHA-256("ZKAttest/hedge/prove/v1" || params digest || ring digest of the row's ring || seed_b (32, or 32
+ *                  zero bytes when seeds == NULL) || msg_hash_b (32) || sig_b (64) || pk_b (65) || le32(which_b)).
+ * Neither the row's index in the call nor its neighbours are hashed: rows in any order give the same bytes.  A hedged call
+ * is byte-identical (proofs, proof_len, status and its precedence) to the seeded call on the seeds zka_hedge_seeds returns.
+ * Two rows share randomness only if every hashed input is equal; they then prove the same statement with the same witness,
+ * and their proof bytes are identical.  So a caller seed that repeats (a broken CSPRNG, a VM restored from a snapshot, a
+ * forked worker, a reused buffer) no longer deanonymises the signer.  With seeds == NULL the proofs are deterministic and
+ * their randomness rests on the secrecy of the signature alone: (r, s) with the message recovers the public key, so the
+ * signature is as secret as the witness.  Derived seeds stay in library workspace; only zka_hedge_seeds copies them out.
+ *
  * Pointers may be host or CUDA device pointers (detected per argument); host buffers are
  * staged through the library's stream.  The caller owns every buffer.
  * Return value: 0 on success, negative on a fatal (argument/CUDA) error — see zka_last_error.
@@ -225,6 +245,28 @@ int zka_verify_batch_rings_seeded(zka_ctx* ctx, const zka_params* params, const 
                                   uint32_t B, const uint8_t* msg_hash, const uint8_t* proofs, size_t proof_stride,
                                   const uint32_t* proof_len, const uint8_t* seeds /* B x 32 */, uint32_t samples, uint8_t* ok,
                                   int32_t* status);
+
+/* ---- hedged seeds (rule under "Hedged seeds" above) ----
+ * zka_prove_batch_hedged / zka_prove_batch_rings_hedged: zka_prove_batch_seeded / zka_prove_batch_rings_seeded on the hedged
+ * seed of every row instead of `seeds`; every other argument, check, status and the chunk schedule are theirs, except that
+ * seeds may be NULL (deterministic proofs; the schedule then counts the seeds as device memory).  A ring-set row gets the
+ * seed, and so the proof bytes, of the one-ring hedged call on its ring.
+ * zka_hedge_seeds / zka_hedge_seeds_rings: the B x 32 seeds such a call derives, into `out` (host or device).  This is the
+ * audit hook of the rule: ITS OUTPUT IS AS SECRET AS THE WITNESS. */
+int zka_prove_batch_hedged(zka_ctx* ctx, const zka_params* params, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
+                           const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N,
+                           const uint8_t* seeds /* B x 32 or NULL */, uint8_t* proofs, size_t proof_stride,
+                           uint32_t* proof_len, int32_t* status);
+int zka_prove_batch_rings_hedged(zka_ctx* ctx, const zka_params* params, const zka_rings* rings, const uint32_t* ring_of,
+                                 uint32_t B, const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which,
+                                 const uint8_t* seeds /* B x 32 or NULL */, uint8_t* proofs, size_t proof_stride,
+                                 uint32_t* proof_len, int32_t* status);
+int zka_hedge_seeds(zka_ctx* ctx, const zka_params* params, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
+                    const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N,
+                    const uint8_t* seeds /* B x 32 or NULL */, uint8_t* out /* B x 32 */);
+int zka_hedge_seeds_rings(zka_ctx* ctx, const zka_params* params, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
+                          const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which,
+                          const uint8_t* seeds /* B x 32 or NULL */, uint8_t* out /* B x 32 */);
 
 /* ---- stand-alone sub-proof verifiers: the surface of the reference's own unit tests and benches ----
  * verifyExp(paramsNIST, paramsWario, Clambda, Px, Py, pi, secparam, Q?)   /root/reference/src/exp/exp.ts:233-349

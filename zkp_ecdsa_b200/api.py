@@ -261,6 +261,36 @@ class Engine:
                                      samples, ok, status)
         return ok, status
 
+    def _hedge_seeds_arg(self, B, seeds, deterministic):
+        if deterministic:
+            if seeds is not None:
+                raise ValueError('give either seeds or deterministic=True')
+            return None
+        return _seed_rows(os.urandom(32 * B), B) if seeds is None else seeds
+
+    def prove_batch_hedged(self, params, msg_hash, sig, pk, which, ring, seeds=None, deterministic: bool = False,
+                           proofs=None) -> ProveResult:
+        """prove_batch_seeded with each row's seed derived on the GPU from `seeds`, the statement and the signature
+        (include/zkattest.h, "Hedged seeds"): a repeated seed no longer deanonymises the signer.  Default: os.urandom(32 * B);
+        deterministic=True passes no seeds (the randomness then rests on the secrecy of the signature alone)."""
+        B = msg_hash.shape[0]
+        N = ring.shape[0]
+        seeds = self._hedge_seeds_arg(B, seeds, deterministic)
+        stride = self.lib.proof_max_len(N, params.sec_level)
+        if proofs is None:
+            proofs = np.zeros((B, stride), np.uint8)
+        plen = np.zeros(B, np.uint32)
+        status = np.zeros(B, np.int32)
+        self.lib.prove_batch_hedged(params.handle, B, msg_hash, sig, pk, which, ring, N, seeds, proofs, proofs.shape[1], plen, status)
+        return ProveResult(proofs, plen, status)
+
+    def hedge_seeds(self, params, msg_hash, sig, pk, which, ring, seeds=None, deterministic: bool = False) -> np.ndarray:
+        """The B x 32 seeds prove_batch_hedged derives from the same arguments (as secret as the witness; an audit hook).
+        With seeds=None and deterministic=False a fresh os.urandom draw is used, as prove_batch_hedged would."""
+        B = msg_hash.shape[0]
+        seeds = self._hedge_seeds_arg(B, seeds, deterministic)
+        return self.lib.hedge_seeds(params.handle, B, msg_hash, sig, pk, which, ring, ring.shape[0], seeds)
+
     # ------------------------------------------------------------------ ring sets: one batch, many rings
     def load_rings(self, rings: Sequence) -> RingSet:
         """Upload R rings (each a sequence of ints, like `keys`, or an N x 32 uint8 array of entries) as one device set.
@@ -298,6 +328,22 @@ class Engine:
         plen = np.zeros(B, np.uint32)
         status = np.zeros(B, np.int32)
         self.lib.prove_batch_rings_seeded(params.handle, rings.handle, ring_of, B, msg_hash, sig, pk, which, seeds, proofs,
+                                          proofs.shape[1], plen, status)
+        return ProveResult(proofs, plen, status)
+
+    def prove_batch_rings_hedged(self, params, rings: RingSet, ring_of, msg_hash, sig, pk, which, seeds=None,
+                                 deterministic: bool = False, proofs=None) -> ProveResult:
+        """prove_batch_rings_seeded with hedged seeds (see prove_batch_hedged); row i gets the bytes of the one-ring hedged
+        call on ring ring_of[i]."""
+        B = msg_hash.shape[0]
+        ring_of = np.ascontiguousarray(ring_of, np.uint32)
+        seeds = self._hedge_seeds_arg(B, seeds, deterministic)
+        stride = self.lib.proof_max_len(rings.largest(ring_of), params.sec_level)
+        if proofs is None:
+            proofs = np.zeros((B, stride), np.uint8)
+        plen = np.zeros(B, np.uint32)
+        status = np.zeros(B, np.int32)
+        self.lib.prove_batch_rings_hedged(params.handle, rings.handle, ring_of, B, msg_hash, sig, pk, which, seeds, proofs,
                                           proofs.shape[1], plen, status)
         return ProveResult(proofs, plen, status)
 

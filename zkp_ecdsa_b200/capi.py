@@ -31,7 +31,8 @@ SYMBOLS = [
     'zka_prove_equality_batch', 'zka_prove_mult_batch', 'zka_prove_pointadd_batch', 'zka_stat', 'zka_proof_group', 'zka_set_progress', 'zka_chunk_schedule',
     'zka_prove_batch_seeded', 'zka_verify_batch_seeded', 'zka_seed_tape',
     'zka_rings_create', 'zka_rings_destroy', 'zka_prove_batch_rings', 'zka_prove_batch_rings_seeded', 'zka_verify_batch_rings',
-    'zka_verify_batch_rings_seeded',
+    'zka_verify_batch_rings_seeded', 'zka_prove_batch_hedged', 'zka_prove_batch_rings_hedged', 'zka_hedge_seeds',
+    'zka_hedge_seeds_rings',
 ]
 
 STATUS_MESSAGES = {
@@ -173,6 +174,11 @@ class ZkaLib:
             L.zka_verify_batch_rings_seeded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
                                                         C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
                                                         C.c_void_p]
+        if hasattr(L, 'zka_hedge_seeds'):
+            L.zka_prove_batch_hedged.argtypes = L.zka_prove_batch_seeded.argtypes
+            L.zka_prove_batch_rings_hedged.argtypes = L.zka_prove_batch_rings_seeded.argtypes
+            L.zka_hedge_seeds.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 5 + [C.c_uint32, C.c_void_p, C.c_void_p]
+            L.zka_hedge_seeds_rings.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 6
         ctx = C.c_void_p()
         rc = L.zka_init(device, C.byref(ctx))
         if rc != 0 or not ctx:
@@ -349,6 +355,31 @@ class ZkaLib:
         self._check(self.lib.zka_verify_batch_rings_seeded(self.ctx, params, rings, _ptr(ring_of), B, _ptr(msg_hash), _ptr(proofs),
                                                            proof_stride, _ptr(proof_len), _ptr(seeds), samples, _ptr(ok), _ptr(status)),
                     'zka_verify_batch_rings_seeded')
+
+    # ------------------------------------------------------------------ hedged seeds (seeds may be None: NULL)
+    def prove_batch_hedged(self, params, B, msg_hash, sig, pk, which, ring, N, seeds, proofs, proof_stride, proof_len, status):
+        self._check(self.lib.zka_prove_batch_hedged(self.ctx, params, B, _ptr(msg_hash), _ptr(sig), _ptr(pk), _ptr(which), _ptr(ring),
+                                                    N, _ptr(seeds), _ptr(proofs), proof_stride, _ptr(proof_len), _ptr(status)),
+                    'zka_prove_batch_hedged')
+
+    def prove_batch_rings_hedged(self, params, rings, ring_of, B, msg_hash, sig, pk, which, seeds, proofs, proof_stride, proof_len,
+                                 status):
+        self._check(self.lib.zka_prove_batch_rings_hedged(self.ctx, params, rings, _ptr(ring_of), B, _ptr(msg_hash), _ptr(sig), _ptr(pk),
+                                                          _ptr(which), _ptr(seeds), _ptr(proofs), proof_stride, _ptr(proof_len),
+                                                          _ptr(status)), 'zka_prove_batch_rings_hedged')
+
+    def hedge_seeds(self, params, B, msg_hash, sig, pk, which, ring, N, seeds, out=None) -> np.ndarray:
+        """The B x 32 seeds a hedged call derives (as secret as the witness)."""
+        out = np.zeros((B, 32), np.uint8) if out is None else out
+        self._check(self.lib.zka_hedge_seeds(self.ctx, params, B, _ptr(msg_hash), _ptr(sig), _ptr(pk), _ptr(which), _ptr(ring), N,
+                                             _ptr(seeds), _ptr(out)), 'zka_hedge_seeds')
+        return out
+
+    def hedge_seeds_rings(self, params, rings, ring_of, B, msg_hash, sig, pk, which, seeds, out=None) -> np.ndarray:
+        out = np.zeros((B, 32), np.uint8) if out is None else out
+        self._check(self.lib.zka_hedge_seeds_rings(self.ctx, params, rings, _ptr(ring_of), B, _ptr(msg_hash), _ptr(sig), _ptr(pk),
+                                                   _ptr(which), _ptr(seeds), _ptr(out)), 'zka_hedge_seeds_rings')
+        return out
 
     # ------------------------------------------------------------------ stand-alone sub-proof verifiers
     def verify_exp_batch(self, params, base, com, px, py, q, proofs, proof_len, tape, samples):

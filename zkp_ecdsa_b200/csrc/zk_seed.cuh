@@ -169,4 +169,105 @@ struct SeedVerifyTapeTask {
   }
 };
 
+// ---- hedged seeds (include/zkattest.h, "Hedged seeds"; restated in tests/hedge_rule.py) ----------------------------
+//   ring digest  SHA-256("ZKAttest/hedge/ring/v1" || le32(N) || le32(n) || leaf_0 || leaf_1 || ...), leaf k = SHA-256 of
+//                the 32-byte big-endian entries [1024 k, 1024 k + 1024) of the ring reduced and padded to 2^n entries
+//                (all 2^n of them when 2^n <= 1024)
+//   row seed     SHA-256("ZKAttest/hedge/prove/v1" || params digest || ring digest || seed (or 32 zero bytes) ||
+//                msg_hash || sig || pk || le32(which))
+// The seed of a row then feeds SeedProveTapeTask unchanged.
+enum : int { HEDGE_LEAF_BITS = 10 };
+
+ZK_HD void sha_tag(Sha256& h, const char* s) {
+  while (*s) h.put((uint8_t)*s++);
+}
+// the digest as its 32 bytes in memory order (16-byte aligned destination)
+ZK_HD void sha_store(Sha256& h, uint8_t* out) {
+  uint32_t d[8];
+  h.final256(d);
+#pragma unroll
+  for (int i = 0; i < 8; i++) d[i] = bswap32(d[i]);
+  st8v(reinterpret_cast<uint32_t*>(out), d);
+}
+ZK_HD uint32_t hedge_leaves(int n) { return n > HEDGE_LEAF_BITS ? 1u << (n - HEDGE_LEAF_BITS) : 1u; }
+
+// The ring digest of R rings, two launches: leaf (thread = one leaf of one ring) then root (thread = one ring).  The
+// entries are read from the prepared rings (RingPrepTask / RingSetPrepTask: reduced, padded, Montgomery form), so the
+// digest covers exactly the ring the proof is made against.  One ring: ring_base / ring_size / ring_depth / leaf_off
+// null, R = 1, size N and depth n.
+struct RingDigestTask {
+  const uint32_t* ring_m;      // [entries][8]
+  const uint32_t *ring_base, *ring_size, *ring_depth, *leaf_off;   // [R], [R], [R], [R + 1] or null
+  uint32_t N, n, R;
+  uint8_t* leaves;             // [total leaves][32]
+  uint8_t* digest;             // [R][32]
+  bool root;
+  ZK_HD void operator()(int t) const {
+    if (root) {
+      const uint32_t r = (uint32_t)t, d = ring_depth ? ring_depth[r] : n;
+      const uint8_t* lv = leaves + (size_t)32 * (leaf_off ? leaf_off[r] : 0u);
+      Sha256 h;
+      h.init();
+      sha_tag(h, "ZKAttest/hedge/ring/v1");
+      h.put4(ring_size ? ring_size[r] : N);
+      h.put4(d);
+      for (uint32_t k = 0; k < hedge_leaves((int)d); k++) h.update(lv + (size_t)32 * k, 32);
+      sha_store(h, digest + (size_t)32 * r);
+      return;
+    }
+    uint32_t r = 0;
+    if (leaf_off) {   // the last ring whose first leaf is <= t
+      uint32_t lo = 0, hi = R - 1;
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (leaf_off[mid] <= (uint32_t)t) lo = mid; else hi = mid - 1;
+      }
+      r = lo;
+    }
+    const uint32_t d = ring_depth ? ring_depth[r] : n;
+    const uint32_t k = (uint32_t)t - (leaf_off ? leaf_off[r] : 0u);
+    const uint32_t count = d > HEDGE_LEAF_BITS ? 1u << HEDGE_LEAF_BITS : 1u << d;
+    const uint32_t* e = ring_m + (size_t)8 * ((ring_base ? ring_base[r] : 0u) + (k << HEDGE_LEAF_BITS));
+    Sha256 h;
+    h.init();
+    for (uint32_t j = 0; j < count; j++) {
+      uint32_t m[8], v[8];
+      ld<8>(m, e + (size_t)8 * j);
+      Tomq::from_mont(v, m);
+#pragma unroll
+      for (int w = 7; w >= 0; w--) h.put4(bswap32(v[w]));   // big-endian: the most significant limb first
+    }
+    sha_store(h, leaves + (size_t)32 * t);
+  }
+};
+
+// One thread per row: the row's hedged seed into out[b] (16-byte aligned rows of 32 bytes).  ring_of null: one ring.
+struct SeedHedgeTask {
+  uint32_t params_digest[8];   // the 32 bytes of zka_params' digest as little-endian words
+  const uint8_t* ring_digest;  // [R][32]
+  const uint32_t* ring_of;     // [B] or null
+  const uint8_t *seeds, *msg_hash, *sig, *pk;   // seeds may be null (32 zero bytes)
+  const uint32_t* which;
+  uint8_t* out;                // [B][32]
+  ZK_HD void operator()(int b) const {
+    Sha256 h;
+    h.init();
+    sha_tag(h, "ZKAttest/hedge/prove/v1");
+#pragma unroll
+    for (int i = 0; i < 8; i++) h.put4(params_digest[i]);
+    h.update(ring_digest + (size_t)32 * (ring_of ? ring_of[b] : 0u), 32);
+    if (seeds) {
+      h.update(seeds + (size_t)32 * b, 32);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; i++) h.put4(0u);
+    }
+    h.update(msg_hash + (size_t)32 * b, 32);
+    h.update(sig + (size_t)64 * b, 64);
+    h.update(pk + (size_t)65 * b, 65);
+    h.put4(which[b]);
+    sha_store(h, out + (size_t)32 * b);
+  }
+};
+
 }  // namespace zk

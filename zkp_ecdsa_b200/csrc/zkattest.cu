@@ -285,7 +285,7 @@ struct Lane {
   // workspace (grow-only pools, see Cursor): one chunk pass, the input and output staging buffers of each slot, and the
   // verifier's chunk-wide aggregate check (zk_verify_agg.cuh: its fixed parts, and one pool per MSM as the two MSMs
   // run side by side)
-  DevBuf w[51];
+  DevBuf w[52];
   DevBuf in[2][10], out[2][3];
   DevBuf agg[9], agg_tom[5 + 2 * AGG_MAX_LEVELS], agg_nist[5 + 2 * AGG_MAX_LEVELS];
   std::string err;
@@ -307,6 +307,7 @@ struct zka_ctx : Lane {
   std::vector<std::unique_ptr<Lane>> extra;   // lanes 1 .. nlanes-1 (lane 0 is the context itself)
   int nlanes = 3;             // ZKA_LANES
   DevBuf ring_in, ring_m;     // the ring of the current call (shared by all lanes, read-only while they run)
+  DevBuf ring_leaves, ring_digest;   // its hedge digest (RingDigestTask) when the call is hedged
   Lane& lane(int i) { return i == 0 ? *this : *extra[i - 1]; }
 #if defined(ZKA_PG_WAR256)
   FbShape tom = fb_uniform(22);   // shape of the proof group's fixed-base tables g and h (ZKA_TOM_W)
@@ -346,6 +347,7 @@ struct zka_params {
   FixedTable th;          // ProofGroup.h table
   uint8_t h_nist[65];
   uint8_t h_proof[WP];
+  uint8_t hedge_digest[32];   // the params digest of the hedged seeds (include/zkattest.h)
 };
 
 // R rings on the device (zka_rings_create): ring r is reduced mod the proof-group order and padded to 2^n_r entries with
@@ -357,6 +359,7 @@ struct zka_rings {
   std::vector<int> depth;                  // n_r = ceil(log2 N_r)
   DevBuf ring_m, ring_base, ring_size, ring_depth;   // [total][8], [R], [R], [R]
   DevBuf lag;                              // the prover's GK Lagrange matrices of the depths 1 .. max n_r (GkLagrangeSetTask)
+  DevBuf ring_digest;                      // [R][32] the hedge digest of each ring (RingDigestTask)
 };
 
 namespace {
@@ -650,22 +653,33 @@ void prep_lagrange(zka_ctx* ctx, Stream& st, int n) {
     ctx->lag_n = n;
   }
 }
-// The ring of a call on the device (RingPrepTask) and, for the prover, the Lagrange matrix.
-const uint32_t* prep_ring(zka_ctx* ctx, Stream& st, const uint8_t* ring, uint32_t N, int n, bool lagrange) {
+// The ring of a call on the device (RingPrepTask), for the prover the Lagrange matrix, and for a hedged call the ring's
+// digest into ctx->ring_digest (RingDigestTask: leaves, then root).
+const uint32_t* prep_ring(zka_ctx* ctx, Stream& st, const uint8_t* ring, uint32_t N, int n, bool lagrange, bool digest = false) {
   const uint8_t* d_ring = stage_in(st, ctx->ring_in, ring, (size_t)N * 32);
   uint32_t* ring_m = ctx->ring_m.get<uint32_t>(((size_t)1 << n) * 8);
   launch(st, 1ll << n, RingPrepTask{d_ring, ring_m, (int)N});
   if (lagrange) prep_lagrange(ctx, st, n);
+  if (digest) {
+    const uint32_t nl = hedge_leaves(n);
+    RingDigestTask t{ring_m, nullptr, nullptr, nullptr, nullptr, N, (uint32_t)n, 1u, ctx->ring_leaves.get<uint8_t>((size_t)32 * nl),
+                     ctx->ring_digest.get<uint8_t>(32), false};
+    launch(st, nl, t);
+    t.root = true;
+    launch(st, 1, t);
+  }
   return ring_m;
 }
 
-// The per-row arguments of a batched prove call (host or device), exactly one of tape / seeds set.  proveExp alone reads
+// The per-row arguments of a batched prove call (host or device), exactly one of tape / seeds set, or hedge (seeds then
+// optional: each row's seed is derived from them, the statement and the signature, SeedHedgeTask).  proveExp alone reads
 // base / s_in / q_in instead of msg_hash / sig / which; ring_of is set for a ring-set call.
 struct ProveRows {
   const uint8_t *msg_hash{}, *sig{}, *pk{}, *base{}, *s_in{}, *q_in{}, *tape{}, *seeds{};
   const uint32_t *which{}, *ring_of{};
   size_t tape_stride{}, proof_stride{};
   uint8_t* proofs{}; uint32_t* proof_len{}; int32_t* status{};
+  bool hedge = false;
   ProveRows() = default;
   ProveRows(uint8_t* proofs, size_t stride, uint32_t* len, int32_t* status) : proof_stride(stride), proofs(proofs), proof_len(len), status(status) {}
   // the rows from r0 on, null pointers left null (the one place that knows each row's width)
@@ -705,14 +719,17 @@ struct RingSrc {
   static RingSrc one(const uint8_t* ring, uint32_t N) { return {ring, N, nullptr, ceil_log2(N)}; }
   static RingSrc pass(const zka_rings* set, int n) { return {nullptr, 0, set, n}; }
   static RingSrc none(int n) { return {nullptr, 2, nullptr, n}; }
-  // the call's ring on the device and, for the prover, the Lagrange matrix: once per call, done before the lanes start
-  const uint32_t* prepare(zka_ctx* ctx, bool lagrange) const {
+  // the call's ring on the device, for the prover the Lagrange matrix and for a hedged call the ring digest: once per
+  // call, done before the lanes start
+  const uint32_t* prepare(zka_ctx* ctx, bool lagrange, bool digest = false) const {
     if (!set && !ring) return nullptr;
-    if (set) return (const uint32_t*)set->ring_m.p;   // prepared by zka_rings_create, with the matrices of every depth
-    const uint32_t* ring_m = prep_ring(ctx, ctx->st, ring, N, n, lagrange);
+    if (set) return (const uint32_t*)set->ring_m.p;   // prepared by zka_rings_create, with the matrices and digests
+    const uint32_t* ring_m = prep_ring(ctx, ctx->st, ring, N, n, lagrange, digest);
     sync(ctx->st);
     return ring_m;
   }
+  // [R][32] ring digests (one ring: R = 1), after prepare(.., digest = true)
+  const uint8_t* digests(const zka_ctx* ctx) const { return (const uint8_t*)(set ? set->ring_digest.p : ctx->ring_digest.p); }
   // a chunk's ring fields; ring_of: the chunk's rows of it on the device
   template <class Ctx>
   void fill(Ctx& c, const uint32_t* ring_m, const uint32_t* ring_of) const {
@@ -954,12 +971,13 @@ size_t zka_profile_json(zka_ctx* ctx, char* buf, size_t cap) {
   }
   return j.size() + 1;
 }
-int zka_proof_group(char* name, size_t cap, int* point_bytes, int* scalar_bytes) {
 #if defined(ZKA_PG_WAR256)
-  const char* n = "war256";
+static const char* const PROOF_GROUP = "war256";
 #else
-  const char* n = "tomEdwards256";
+static const char* const PROOF_GROUP = "tomEdwards256";
 #endif
+int zka_proof_group(char* name, size_t cap, int* point_bytes, int* scalar_bytes) {
+  const char* n = PROOF_GROUP;
   if (name && cap) {
     strncpy(name, n, cap - 1);
     name[cap - 1] = 0;
@@ -1119,6 +1137,20 @@ int zka_params_create(zka_ctx* ctx, const uint8_t h_nist[65], const uint8_t h_pr
     P->h_w = ctx->p256_hw;
     memcpy(P->h_nist, h_nist, 65);
     memcpy(P->h_proof, h_proof, WP);
+    {   // SHA-256("ZKAttest/hedge/params/v1" || group name NUL-padded to 16 || h_nist || h_proof || le32(sec_level))
+      uint8_t name[16] = {};
+      memcpy(name, PROOF_GROUP, strlen(PROOF_GROUP));
+      Sha256 h;
+      h.init();
+      sha_tag(h, "ZKAttest/hedge/params/v1");
+      h.update(name, 16);
+      h.update(h_nist, 65);
+      h.update(h_proof, WP);
+      h.put4(sec_level);
+      alignas(16) uint8_t d[32];
+      sha_store(h, d);
+      memcpy(P->hedge_digest, d, 32);
+    }
     DevBuf bn, bt, an, at, bad, inf;
     uint8_t* d_bn = bn.get<uint8_t>(65);
     uint8_t* d_bt = bt.get<uint8_t>(WP);
@@ -1185,6 +1217,17 @@ int zka_rings_create(zka_ctx* ctx, uint32_t R, const uint32_t* sizes, const uint
     copy_h2d(st, d_depth, depth.data(), (size_t)R * 4);
     launch(st, (long long)total, RingSetPrepTask{d_keys, d_off, d_base, d_size, ring_m, (int)R});
     launch(st, nmax, GkLagrangeSetTask{set->lag.get<uint32_t>(ProveCtx::gk_lag_off(nmax + 1))});
+    // the hedge digest of every ring (RingDigestTask), for the hedged prove calls
+    std::vector<uint32_t> leaf_off(R + 1, 0);
+    for (uint32_t r = 0; r < R; r++) leaf_off[r + 1] = leaf_off[r] + hedge_leaves(set->depth[r]);
+    DevBuf lbuf, leaves;
+    uint32_t* d_leaf_off = lbuf.get<uint32_t>(R + 1);
+    copy_h2d(st, d_leaf_off, leaf_off.data(), (size_t)(R + 1) * 4);
+    RingDigestTask dt{ring_m, d_base, d_size, d_depth, d_leaf_off, 0u, 0u, R, leaves.get<uint8_t>((size_t)32 * leaf_off[R]),
+                      set->ring_digest.get<uint8_t>((size_t)32 * R), false};
+    launch(st, leaf_off[R], dt);
+    dt.root = true;
+    launch(st, R, dt);
     sync(st);
     *out = set.release();
     return 0;
@@ -1360,19 +1403,23 @@ int zka_key_to_int(zka_ctx* ctx, uint32_t count, const uint8_t* pk, uint8_t* x_o
 // mode 0: proveSignatureList.  mode 1: proveExp alone (exp.ts:126-231) — base / s_in / q_in are the statement,
 // msg_hash / sig / which are unused, the rows hold the repetitions only.
 // seeds (B x 32, mode 0 only) instead of a tape: every lane expands its chunk's draws into its own tape buffer
-// (SeedProveTapeTask), the draws before the challenge first, the item and GK draws after the scan.
+// (SeedProveTapeTask), the draws before the challenge first, the item and GK draws after the scan.  hedge: the seeds
+// SeedProveTapeTask reads are first derived per row (SeedHedgeTask) into a lane buffer; rows.seeds may then be null.
 static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const ProveRows& rows, const RingSrc& ring, int mode) {
   const int S = (int)P->sec_level, n = ring.n;
-  const bool seeded = rows.seeds != nullptr;
+  const bool hedge = rows.hedge, seeded = rows.seeds != nullptr || hedge;
   // seeded: the library's tape rows hold every draw a proof can read (a multiple of 32 bytes, so 16-byte aligned rows)
   const int seed_draws = prove_draws(S, n, S);
-  const uint32_t* ring_m = ring.prepare(ctx, true);
+  const uint32_t* ring_m = ring.prepare(ctx, true, hedge);
+  const uint8_t* ring_digest = hedge ? ring.digests(ctx) : nullptr;
   const Output<uint8_t> po(rows.proofs, rows.proof_stride);
   const Output<uint32_t> lo(rows.proof_len, 1);
   const Output<int32_t> so(rows.status, 1);
   const int lanes = ctx->nlanes;
   const size_t dev_tape_stride = (rows.tape_stride + 15) & ~(size_t)15;   // row pitch of a host tape staged on the device
-  const bool all_dev = po.dev && is_device_ptr(seeded ? rows.seeds : rows.tape);
+  // (hedged calls without caller seeds count as device memory: no randomness crosses PCIe)
+  const uint8_t* rnd_in = seeded ? rows.seeds : rows.tape;
+  const bool all_dev = po.dev && (!rnd_in || is_device_ptr(rnd_in));
   const std::vector<uint32_t> off = chunk_schedule(B, (uint32_t)(all_dev ? ctx->chunk : std::min(ctx->chunk, ctx->host_chunk)), lanes, !all_dev);
   const uint32_t nchunks = (uint32_t)off.size() - 1;
   const int used = (int)std::min<uint32_t>((uint32_t)lanes, nchunks);
@@ -1491,6 +1538,8 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
       c.which_s = w.take<uint32_t>(Bc);
       uint32_t* base_aff = w.take_if<uint32_t>(mode == 1, (size_t)Bc * 16);
       c.base_aff = mode == 0 ? c.pk_aff : base_aff;
+      uint8_t* hedged = w.take_if<uint8_t>(hedge, (size_t)Bc * 32);
+      const uint8_t* seeds = hedge ? hedged : cin[slot].seeds;   // what SeedProveTapeTask expands
       c.proof_stride = rows.proof_stride;
       Cursor ob(ln.out[slot]);
       c.proofs = po.rows(ob.next(), b0, Bc);
@@ -1524,9 +1573,14 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
       }
       // --- phase A (first consumer of the tape) and R = u1*G + u2*pk side by side
       ev_wait(st, ln.ev_tape[slot]);
+      if (hedge) {
+        SeedHedgeTask ht{{}, ring_digest, cin[slot].ring_of, cin[slot].seeds, c.msg_hash, c.sig, c.pk, c.which, hedged};
+        memcpy(ht.params_digest, P->hedge_digest, 32);
+        launch(st, Bc, ht);
+      }
       if (seeded) {
         const int d1 = draws_before_items(S);
-        launch(st, (long long)Bc * d1, SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, 0, d1, nullptr});
+        launch(st, (long long)Bc * d1, SeedProveTapeTask{seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, 0, d1, nullptr});
       }
       {
         const int nAp = (int)((nA + 31) & ~(size_t)31);
@@ -1547,7 +1601,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
         // the item and GK draws of each proof, up to the longest a proof of the chunk can be (zmax = tot2[1], depth n)
         const int d1 = draws_before_items(S), span = prove_draws((int)tot2[1], n, S) - d1;
         launch(st, (long long)Bc * span,
-               SeedProveTapeTask{cin[slot].seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, d1, span, c.zcount, c.ring_of, c.ring_depth});
+               SeedProveTapeTask{seeds, const_cast<uint8_t*>(c.tape), c.tape_stride, S, n, d1, span, c.zcount, c.ring_of, c.ring_depth});
       } else if (tape_host) {
         // second part of the tape: draws [3 + 4S, 3 + 4S + 40 zmax + 5n) of every row in one strided copy
         // (zmax = the largest zero-bit count of the chunk)
@@ -1624,7 +1678,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
 
 // Every batched prove call: its argument checks (strides against the deepest ring used), then its prove_impl pass
 static int prove_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, const ProveRows& rows, const RingSrc& ring, int mode) {
-  if (!ctx || !P || !rows.pk || (!rows.tape && !rows.seeds) || !rows.proofs || !rows.proof_len || !rows.status) return ZKA_E_ARG;
+  if (!ctx || !P || !rows.pk || (!rows.tape && !rows.seeds && !rows.hedge) || !rows.proofs || !rows.proof_len || !rows.status) return ZKA_E_ARG;
   if (mode == 0 && (!rows.msg_hash || !rows.sig || !rows.which || !(ring.set ? (const void*)rows.ring_of : ring.ring))) return ZKA_E_ARG;
   if (mode == 1 && (!rows.base || !rows.s_in)) return ZKA_E_ARG;
   const int S = (int)P->sec_level;
@@ -1667,6 +1721,63 @@ int zka_prove_batch_rings_seeded(zka_ctx* ctx, const zka_params* P, const zka_ri
   ProveRows r(proofs, proof_stride, proof_len_out, status);
   r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.ring_of = ring_of; r.seeds = seeds;
   return prove_batch(ctx, P, B, r, RingSrc::pass(rings, 0), 0);
+}
+
+// ---- hedged seeds: the seeded calls with each row's seed derived on the device (SeedHedgeTask, rule in zk_seed.cuh)
+int zka_prove_batch_hedged(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
+                           const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* seeds,
+                           uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status) {
+  ProveRows r(proofs, proof_stride, proof_len_out, status);
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.seeds = seeds; r.hedge = true;
+  return prove_batch(ctx, P, B, r, RingSrc::one(ring, N), 0);
+}
+
+int zka_prove_batch_rings_hedged(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
+                                 const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which,
+                                 const uint8_t* seeds, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status) {
+  ProveRows r(proofs, proof_stride, proof_len_out, status);
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.ring_of = ring_of; r.seeds = seeds; r.hedge = true;
+  return prove_batch(ctx, P, B, r, RingSrc::pass(rings, 0), 0);
+}
+
+// The seeds a hedged call derives, B x 32 into `out` (host or device, any alignment: the kernel writes a staging buffer),
+// 1024 rows per launch
+static int hedge_seeds(zka_ctx* ctx, const zka_params* P, uint32_t B, const ProveRows& rows, const RingSrc& ring, uint8_t* out) {
+  if (!ctx || !P || !rows.msg_hash || !rows.sig || !rows.pk || !rows.which || !out) return ZKA_E_ARG;
+  if (!(ring.set ? (const void*)rows.ring_of : ring.ring)) return ZKA_E_ARG;
+  return ring_passes(ctx, ring, rows.ring_of, B, [](int) { return 0; }, [&](const RingSrc& pass) {
+    Stream& st = ctx->st;
+    pass.prepare(ctx, false, true);
+    const uint32_t rows_per = 1024;
+    for (uint32_t b0 = 0; b0 < B; b0 += rows_per) {
+      const uint32_t Bc = std::min(rows_per, B - b0);
+      const ProveRows r = rows.at(b0), e = rows.at(b0 + Bc);
+      Cursor in(ctx->in[0]), w(ctx->w);
+      auto stage = [&](auto* p, auto* end) { return stage_in(st, in.next(), p, (size_t)(end - p)); };
+      SeedHedgeTask ht{{}, pass.digests(ctx), stage(r.ring_of, e.ring_of), stage(r.seeds, e.seeds), stage(r.msg_hash, e.msg_hash),
+                       stage(r.sig, e.sig), stage(r.pk, e.pk), stage(r.which, e.which), w.take<uint8_t>((size_t)Bc * 32)};
+      memcpy(ht.params_digest, P->hedge_digest, 32);
+      launch(st, Bc, ht);
+      copy_d2h(st, out + (size_t)b0 * 32, ht.out, (size_t)Bc * 32);   // (cudaMemcpyDefault: host or device)
+      sync(st);
+    }
+    return 0;
+  });
+}
+
+int zka_hedge_seeds(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk,
+                    const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* seeds, uint8_t* out) {
+  ProveRows r;
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.seeds = seeds;
+  return hedge_seeds(ctx, P, B, r, RingSrc::one(ring, N), out);
+}
+
+int zka_hedge_seeds_rings(zka_ctx* ctx, const zka_params* P, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
+                          const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which, const uint8_t* seeds,
+                          uint8_t* out) {
+  ProveRows r;
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.ring_of = ring_of; r.seeds = seeds;
+  return hedge_seeds(ctx, P, B, r, RingSrc::pass(rings, 0), out);
 }
 
 // The tape a seed stands for (the rule of zk_seed.cuh): kind 0 all prove_draws(S, n, S) prover draws, kind 1 the verify
