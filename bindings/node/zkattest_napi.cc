@@ -38,6 +38,7 @@ const char* status_message(int s) {
     case ZKA_ERR_R_INFINITY: return "R is at infinity";            // zkpAttestList.ts:159
     case ZKA_ERR_MALFORMED: return "error deserializing Point";    // weier.ts:87
     case ZKA_ERR_PARAMS_NOT_FOUND: return "params not found";      // exp.ts:270
+    case ZKA_ERR_SELF_CHECK: return "zkattest: proof failed its self-check";
     default: return "zkattest: internal status";
   }
 }

@@ -74,6 +74,28 @@
  * their randomness rests on the secrecy of the signature alone: (r, s) with the message recovers the public key, so the
  * signature is as secret as the witness.  Derived seeds stay in library workspace; only zka_hedge_seeds copies them out.
  *
+ * Self-checked proving (zka_set_option(ctx, "self_check", 2); 1 = off, the default).  A fault during a prove call (one
+ * wrong commitment byte) changes the challenge of that run; a deterministic prover that also makes the correct proof of
+ * the same statement then reveals alpha_i in one and z = alpha_i - s1 in the other, as a reused seed does.  With the check
+ * on, every row of the six batched proveSignatureList calls (zka_prove_batch[_seeded|_hedged], zka_prove_batch_rings[_seeded|
+ * _hedged]) whose prover status is ZKA_OK is verified before the call releases it: verifySignatureList on the row's own
+ * ring with samples = sec_level, i.e. EVERY repetition (a faulty repetition missed by a partial check is exactly the one
+ * that leaks).  It also catches a `which` that is inside the ring but not the signer's key, which the reference proves
+ * without complaint.  A row passes when the check gives ok = 1 and status 0: its proof bytes, proof_len and status are
+ * those of the unchecked call.  Any other verdict (a verifier status included) gives the row ZKA_ERR_SELF_CHECK, its
+ * bytes zeroed and proof_len 0, as for a row the prover rejected.  The check's randomness, so that a checked call can be
+ * reproduced:
+ *   k_b  the 32-byte seed expanded for row b (seeded calls: the caller's seed; hedged calls: the derived seed), or for a
+ *        tape call the row's first 96 tape bytes (the blinders of comS1, keyXcom and keyYcom)
+ *   c_b  SHA-256("ZKAttest/check/v1" || k_b)
+ * and the verdict of row b is that of zka_verify_batch_seeded (zka_verify_batch_rings_seeded for a set) with
+ * samples = sec_level and seeds c on the unchecked proofs.  c_b IS AS SECRET AS THE WITNESS, like the seed it comes from;
+ * it stays in library workspace.  Checked calls are deterministic wherever the unchecked call is.  The check runs per
+ * chunk on the device, behind the prover's last kernel: no proof byte crosses PCIe twice, and a chunk reported by
+ * zka_set_progress holds checked proofs only.  zka_stat counts "self_check_rows" and "self_check_fail".  The stand-alone
+ * sub-proof provers (zka_prove_exp_batch, zka_prove_membership_batch, zka_prove_equality_batch, zka_prove_mult_batch,
+ * zka_prove_pointadd_batch) are never checked.
+ *
  * Pointers may be host or CUDA device pointers (detected per argument); host buffers are
  * staged through the library's stream.  The caller owns every buffer.
  * Return value: 0 on success, negative on a fatal (argument/CUDA) error — see zka_last_error.
@@ -104,7 +126,8 @@ enum {
   ZKA_ERR_IDENTITY_ENC = 7,      /* a P-256 proof point is the identity (1-byte encoding, weier.ts:247) */
   ZKA_ERR_R_INFINITY = 8,        /* 'R is at infinity'                           zkpAttestList.ts:159 */
   ZKA_ERR_MALFORMED = 9,         /* proof bytes do not parse (deserializePoint / deserializeScalar throw) */
-  ZKA_ERR_PARAMS_NOT_FOUND = 10  /* exp.ts:270,302 */
+  ZKA_ERR_PARAMS_NOT_FOUND = 10, /* exp.ts:270,302 */
+  ZKA_ERR_SELF_CHECK = 11        /* proof failed its self-check ("self_check" option, see "Self-checked proving") */
 };
 /* Precedence: a row with several defects gets the code of the one the reference meets first.
  *   verify (zka_verify_batch*, zka_verify_exp_batch):  ZKA_ERR_MALFORMED (the whole proof is parsed first, so it wins over
@@ -113,7 +136,8 @@ enum {
  *     range (ZKA_ERR_TAPE_RANGE); then the sampled repetitions in sample order (generateIndices on the tape), the first
  *     one with a defect deciding: ZKA_ERR_PARAMS_NOT_FOUND, its first draw out of range, ZKA_ERR_T_INFINITY /
  *     ZKA_ERR_T1_INFINITY, its later draws out of range.
- *   prove: ZKA_ERR_INVALID_PK, ZKA_ERR_BAD_INDEX, then the repetitions in order. */
+ *   prove: ZKA_ERR_INVALID_PK, ZKA_ERR_BAD_INDEX, then the repetitions in order; with the self-check on, a row that
+ *     carries none of these is checked and may get ZKA_ERR_SELF_CHECK; a row that carries one keeps it unchecked. */
 
 enum {
   ZKA_E_ARG = -1,     /* bad argument */
@@ -374,13 +398,16 @@ size_t zka_profile_json(zka_ctx* ctx, char* buf, size_t cap);
  *   ZKA_TRACE       per-chunk timeline of the host-buffer pipelines on stderr (adds synchronisations) */
 int zka_config(const zka_ctx* ctx, int* tom_w, int* tom_nwin, int* chunk);
 int zka_lanes(const zka_ctx* ctx);
-/* change a knob between calls: key in {"lanes", "chunk", "host_chunk", "agg" (1 = off, 2 = on), "agg_c" (4..16)}, value >= 1 */
+/* change a knob between calls: key in {"lanes", "chunk", "host_chunk", "agg" (1 = off, 2 = on), "agg_c" (4..16),
+ * "self_check" (1 = off, the default; 2 = on: see "Self-checked proving")}, value >= 1 */
 int zka_set_option(zka_ctx* ctx, const char* key, long value);
 /* counters since zka_init: "agg_pass" = verifier chunks accepted as a whole by the chunk-wide aggregate check (the
  * sum over all proofs of the chunk of the reference's three linear combinations, multimult.ts:147-174, evaluated as one
  * wide-window MSM; every relation carries its own random scalar, so the sum is the identity iff (w.h.p.) every
  * per-proof combination is), "agg_fail" = chunks that went on to the per-proof evaluation (some proof invalid or
- * already rejected by the parsers; verdicts and statuses are then exactly the per-proof ones).  Not counters:
+ * already rejected by the parsers; verdicts and statuses are then exactly the per-proof ones); both count verify calls
+ * only, not the chunks of the prover's self-check.  "self_check_rows" = rows the self-check verified, "self_check_fail" =
+ * rows it gave ZKA_ERR_SELF_CHECK.  Not counters:
  * "tom_n_lo" = how many of the tom_nwin windows zka_config reports have tom_w bits (the others have tom_w + 1),
  * "tom_fallback" = 1 when the tables asked for did not fit and the context walks one lookup more.  -1: unknown key.
  * ZKA_AGG=0 disables the aggregate check, ZKA_AGG_C=4..16 fixes its window bits. */

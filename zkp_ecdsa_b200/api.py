@@ -140,6 +140,12 @@ class Engine:
     def close(self):
         self.lib.close()
 
+    def set_self_check(self, on: bool) -> None:
+        """Verify every proof of the batched proveSignatureList calls over all sec_level repetitions before it is returned
+        (include/zkattest.h, "Self-checked proving"); a proof that fails raises ZkaProofError(11) in prove_signature_list
+        and has status 11 in the batch calls.  Off by default."""
+        self.lib.set_option('self_check', 2 if on else 1)
+
     # ------------------------------------------------------------------ reference API
     def generate_params_list(self, sec_level: int = 80, rnd: Optional[bytes] = None) -> SystemParametersList:
         """generateParamsList (zkpAttestList.ts:88-92).  `rnd` = the two rnd() draws (64 B)."""

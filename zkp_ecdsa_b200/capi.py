@@ -47,6 +47,7 @@ STATUS_MESSAGES = {
     8: 'R is at infinity',                   # zkpAttestList.ts:159
     9: 'malformed proof bytes',
     10: 'params not found',                  # exp.ts:270,302
+    11: 'proof failed its self-check',       # zka_set_option(ctx, "self_check", 2)
 }
 
 

@@ -19,6 +19,7 @@
 #include <string>
 #include <vector>
 
+#include "zk_check.cuh"
 #include "zk_launch.cuh"
 #include "zk_prove.cuh"
 #include "zk_seed.cuh"
@@ -288,6 +289,9 @@ struct Lane {
   DevBuf w[52];
   DevBuf in[2][10], out[2][3];
   DevBuf agg[9], agg_tom[5 + 2 * AGG_MAX_LEVELS], agg_nist[5 + 2 * AGG_MAX_LEVELS];
+  // the prover's self-check (check_chunk): c_b, the rows to check, the verify tape, ok and the verifier's statuses; and the
+  // lane's counts of rows checked / failed over one call
+  DevBuf chk[5], chk_count;
   std::string err;
   ~Lane() {
     for (int i = 0; i < 2; i++) {
@@ -324,6 +328,8 @@ struct zka_ctx : Lane {
   int agg = 1;            // verifier: chunk-wide aggregate check before the per-proof MSMs (ZKA_AGG=0 disables it)
   int agg_c = 0;          // window bits of the aggregate MSM (0: chosen from the chunk size; ZKA_AGG_C)
   uint64_t agg_pass = 0, agg_fail = 0;   // chunks decided by the aggregate / sent to the per-proof path (zka_stat)
+  int self_check = 0;     // prover: verify every proof with samples = sec_level before releasing it (check_chunk)
+  uint64_t self_check_rows = 0, self_check_fail = 0;   // rows checked / given ZKA_ERR_SELF_CHECK (zka_stat)
   std::mutex stat_mu;
   std::mutex copy_mu;     // keeps the copies of one chunk together on the shared copy-in stream (verify)
   int agg_c_last = 0;
@@ -860,6 +866,242 @@ void verify_gk(Stream& st, const VerifyCtx& c, uint32_t* gk_offs) {
   launch(st, (long long)c.B * ngk, VGkOffsetsTask{c, gk_offs});
 }
 
+// The stage chain of one verifier chunk on lane `ln`, from VLayoutTask to VFinalTask, with the chunk-wide aggregate check
+// first when `agg`.  c holds the chunk's inputs, ring and ok / status rows; its workspace is the lane's pool w (and the agg
+// pools).  Every stage ends on the lane's stream.  b0: the chunk's first row in the call (hashed into the aggregate's
+// weights); agg_c (may be null) receives the window bits of the tomEdwards256 aggregate MSM.  Returns the aggregate's
+// control words on the device (null without it).
+const uint32_t* verify_chunk(zka_ctx* ctx, Lane& ln, VerifyCtx& c, uint32_t b0, bool agg, int* agg_c) {
+  Stream& st = ln.st;
+  const int Bc = c.B, S = c.S, K = c.K, n = c.n, mode = c.mode;
+  const size_t ns = (size_t)Bc * K;
+  const int ET = c.ent_tom(), EN = c.ent_nist(), SG = c.segs();
+  const int ngk = 4 * n + 1;
+  Cursor w(ln.w);
+  c.rep_off = w.take<uint32_t>((size_t)Bc * S);
+  c.gk_off = w.take<uint32_t>(Bc);
+  c.tagbits = w.take<uint32_t>((size_t)Bc * 3);
+  c.chal = w.take<uint32_t>((size_t)Bc * 3);
+  c.gk_ok_len = w.take<uint8_t>(Bc);
+  c.r_aff = w.take<uint32_t>((size_t)Bc * 16);
+  c.q_aff = w.take<uint32_t>((size_t)Bc * 16);
+  c.q_inf = w.take<uint8_t>(Bc);
+  c.rpows = w.take<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
+  c.rrows = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_PROJ_WORDS);
+  c.rtab = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_AFF_WORDS);
+  c.samp_idx = w.take<uint32_t>(ns);
+  c.samp_draw = w.take<uint32_t>(ns);
+  c.sp_T = w.take<uint32_t>(ns * P256_PROJ_WORDS);
+  c.sp_T_aff = w.take<uint32_t>(ns * 16);
+  c.sp_T_inf = w.take<uint8_t>(ns);
+  c.ta_jv = w.take<uint32_t>(ns * 2 * 8);
+  c.ta_jr = w.take<uint32_t>(ns * 2 * 8);
+  c.ta_proj = w.take<uint32_t>(ns * 2 * TOM_E2_WORDS);
+  c.ta_aff = w.take<uint32_t>(ns * 2 * TOM_AFF_WORDS);
+  c.td_proj = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_PROJ_WORDS);
+  c.td_aff = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_AFF_WORDS);
+  c.td_bytes = w.take<uint8_t>(ns * DERS_PER_ITEM * BSTRIDE);
+  c.item_chal = w.take<uint32_t>(ns * HASHES_PER_ITEM * 3);
+  c.ent_scalar = w.take<uint32_t>((size_t)Bc * ET * 8);
+  c.ent_off = w.take<uint32_t>((size_t)Bc * ET);
+  c.ent_pre = w.take<uint32_t>((size_t)Bc * ET * TOM_PRE_WORDS);
+  c.ent_cnt = w.take<uint32_t>(ns);
+  c.part = w.take<uint32_t>(ns * V_PART_WORDS);
+  // the small per-proof arrays before the entries and windows: the prover of this lane has small arrays at the
+  // same places of the pool, so these share its buffers without growing them much
+  c.fx_jv = w.take<uint32_t>((size_t)Bc * 2 * 8);
+  c.fx_jr = w.take<uint32_t>((size_t)Bc * 2 * 8);
+  c.fx_proj = w.take<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
+  c.nfix = w.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
+  c.id_flags = w.take<uint8_t>((size_t)Bc * 3);
+  c.gk_tape_bad = w.take_if<uint8_t>(mode == 0, Bc);
+  c.vkey = w.take<int32_t>(Bc);
+  c.nent_scalar = w.take<uint32_t>((size_t)Bc * EN * 8);
+  c.nent_aff = w.take<uint32_t>((size_t)Bc * EN * 16);
+  c.nent_skip = w.take<uint8_t>((size_t)Bc * EN);
+  c.gk_scalar = w.take<uint32_t>((size_t)Bc * ngk * 8);
+  c.gk_pre = w.take<uint32_t>((size_t)Bc * ngk * TOM_PRE_WORDS);
+  uint32_t* gk_offs = w.take<uint32_t>((size_t)Bc * ngk);
+  c.win_w = w.take<uint32_t>((size_t)Bc * SG * MSM_NWIN * 36);
+  c.win_g = w.take<uint32_t>((size_t)Bc * MSM_NWIN * 36);
+  c.win_n = w.take<uint32_t>((size_t)Bc * MSM_NWIN_N * P256_PROJ_WORDS);
+  c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * gk_blocks(n) * 8);
+  const size_t agg_tape_len = verify_tape_len(n, S, K);
+  const int agg_tp = agg_tape_pieces(agg_tape_len), agg_np = agg_tp + K + 1;
+  uint32_t* agg_wt = w.take_if<uint32_t>(agg, (size_t)Bc * AGG_WT * 8);
+  uint32_t* agg_dig = w.take_if<uint32_t>(agg, (size_t)Bc * agg_np * 8);
+  c.chal_full = w.take_if<uint32_t>(agg, (size_t)Bc * 8);
+  c.nfix_k = w.take_if<uint32_t>(agg, (size_t)Bc * 16);
+
+  launch(st, Bc, VLayoutTask{c});
+  launch(st, (long long)Bc * (S + 1), VValidateTask{c});
+  {
+    // the per-proof tables of R (a 255-doubling chain per proof, rows, normalisation: no status writes) run beside the
+    // Fiat-Shamir hash of the repetitions (one thread per proof, 16 KB) unless per-kernel profiling is on
+    const bool fork = !st.profiling;
+    Stream& sr = fork ? ln.aux[0] : st;
+    if (fork) { ev_record(ln.ev_fork, st); ev_wait(sr, ln.ev_fork); }
+    launch(sr, Bc, P256PowsTask{c.r_aff, nullptr, c.rpows, Bc, RT_NWIN, RT_W});
+    launch(sr, (long long)Bc * RT_NWIN, P256RowsSignedTask{c.rpows, c.rrows});
+    launch_p256_norm(sr, c.rrows, c.rtab, nullptr, nullptr, (long long)Bc * RT_ENTRIES);
+    launch(st, Bc, VChallengeTask{c});
+    if (fork) { ev_record(ln.ev_join[0], sr); ev_wait(st, ln.ev_join[0]); }
+  }
+  // the Groth-Kohlweiss chain (ring polynomial, relations, offsets) only needs the layout: it runs on a side stream
+  // beside the sampled-repetition chain; its tape-range status is folded in by VReduceTask (same precedence)
+  const bool gk_fork = mode == 0 && !st.profiling;
+  if (gk_fork) {
+    ev_record(ln.ev_fork, st);
+    ev_wait(ln.aux[1], ln.ev_fork);
+  }
+  if (agg) {
+    // the aggregate's weights (zk_verify_agg.cuh) need the layout, the sampled repetitions and the exp challenge: they
+    // hash ahead of the GK chain on its side stream (joined before VReduceTask)
+    Stream& sw = gk_fork ? ln.aux[1] : st;
+    launch(sw, (long long)Bc * agg_np, AggPieceTask{c, agg_tape_len, agg_tp, agg_np, agg_dig});
+    launch(sw, Bc, AggWeightTask{c, c.chal_full, agg_dig, b0, agg_np, agg_wt});
+  }
+  if (gk_fork) {
+    verify_gk(ln.aux[1], c, gk_offs);
+    ev_record(ln.ev_join[1], ln.aux[1]);
+  }
+  launch(st, (long long)ns, VSampleP256Task{c});
+  launch_p256_norm(st, c.sp_T, c.sp_T_aff, nullptr, c.sp_T_inf, (long long)(ns));
+  launch(st, (long long)ns, VSampleJobsTask{c});
+  launch(st, (long long)ns * 2, TomCommitTask{c.ta_jv, c.ta_jr, c.tg_tab, c.th_tab, c.ta_proj, c.tom});
+  launch_tom_norm(st, c.ta_proj, c.ta_aff, nullptr, (long long)(ns * 2), 1);
+  launch(st, (long long)ns, VDerivedTask{c});
+  launch_tom_norm(st, c.td_proj, nullptr, c.td_bytes, (long long)(ns * DERS_PER_ITEM), 0);
+  launch(st, (long long)ns * HASHES_PER_ITEM, VItemHashTask{c});
+  dev_memset(st, c.ent_off, 0, (size_t)Bc * ET * 4);
+  launch(st, (long long)ns, VRelationsTask{c});
+  if (mode == 0) {
+    if (gk_fork) ev_wait(st, ln.ev_join[1]);
+    else verify_gk(st, c, gk_offs);
+  }
+  launch(st, Bc, VReduceTask{c});
+  launch(st, (long long)Bc * ET, VParseEntriesTask{c.proofs, c.proof_stride, c.ent_off, c.ent_pre, ET});
+  if (mode == 0) launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, c.proof_stride, gk_offs, c.gk_pre, ngk});
+  launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom, 1});
+  // chunk-wide aggregate check (zk_verify_agg.cuh): the sum over all proofs of the chunk of the three linear
+  // combinations, as ONE wide-window MSM per group; when both sums are the identity the per-proof MSMs below
+  // return at once
+  uint32_t* ctl = nullptr;
+  if (agg) {
+    Cursor A(ln.agg);
+    const int fgroups = (Bc * 2 + 63) / 64, ngroups = (Bc + 31) / 32, ngroups2 = (ngroups + 31) / 32;
+    ctl = A.take<uint32_t>(AGG_CTL_WORDS);
+#if !defined(ZKA_PG_WAR256)
+    uint32_t* tpart = A.take<uint32_t>((size_t)Bc * (K + 2) * 2 * PG_EXT_WORDS);
+#endif
+    uint32_t* fpart = A.take<uint32_t>((size_t)fgroups * 16);
+    uint32_t* fjv = A.take<uint32_t>(8);
+    uint32_t* fjr = A.take<uint32_t>(8);
+    uint32_t* fproj = A.take<uint32_t>(TOM_PROJ_WORDS);
+    uint32_t* nfix_w = A.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
+    uint32_t* npart = A.take<uint32_t>((size_t)ngroups * P256_PROJ_WORDS);
+    uint32_t* npart2 = A.take_if<uint32_t>(ngroups > 32, (size_t)ngroups2 * P256_PROJ_WORDS);
+    dev_memset(st, ctl, 0, AGG_CTL_WORDS * 4);
+    launch(st, Bc, AggGateTask{c, ctl});
+    const AggTomSrc tsrc{c.ent_scalar, c.ent_pre, c.ent_cnt, c.gk_scalar, c.gk_pre, Bc, ET, K, ngk, agg_wt};
+    const AggNistSrc nsrc{c.nent_scalar, c.nent_aff, c.nent_skip, Bc, EN, agg_wt};
+    // three independent chains from here to AggFinalTask: the tomEdwards256 MSM (this stream), the torsion guard and the
+    // P-256 MSM with its fixed parts (two side streams; with per-kernel profiling on, everything stays on one stream
+    // so that the event pairs time one kernel at a time).  A skip flag raised by the torsion guard may reach the MSM
+    // kernels late — they then only do work AggFinalTask discards.
+    const bool fork = !st.profiling;
+    Stream& sa = fork ? ln.aux[0] : st;
+    Stream& sb = fork ? ln.aux[1] : st;
+    if (fork) {
+      ev_record(ln.ev_fork, st);
+      ev_wait(sa, ln.ev_fork);
+      ev_wait(sb, ln.ev_fork);
+    }
+#if !defined(ZKA_PG_WAR256)
+    // cofactor 4: no small-order components, or the per-proof path decides
+    launch(sa, (long long)Bc * (K + 2) * 2, AggTorsionPartTask{tsrc, ctl, tpart});
+    launch(sa, (long long)Bc * 2, AggTorsionTask{tpart, ctl, K});
+#endif
+    const AggPlan tp = agg_plan((double)Bc * (0.5 * K * V_ENT_PER_SAMPLE + 2 + ngk), ctx->agg_c);
+    const AggPlan np = agg_plan((double)Bc * EN, 0);
+    if (agg_c) *agg_c = tp.D.c;
+    const uint32_t *tA, *tB, *nA, *nB;
+    agg_msm(st, Cursor(ln.agg_tom), tsrc, tp, ctl, &tA, &tB);
+    agg_msm(sb, Cursor(ln.agg_nist), nsrc, np, ctl, &nA, &nB);
+    // fixed-base parts: one commitment for the summed weighted tomEdwards256 scalars, a two-level sum of the weighted
+    // P-256 points
+    launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, agg_wt, fpart, Bc});
+    launch(st, 1, AggFixSumTask{ctl, fpart, fjv, fjr, fgroups});
+    launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom, 1});
+    launch(sb, Bc, AggNistFixWeightTask{ctl, c.nfix_k, agg_wt, c.rtab, c.h_tab8, c.h_w, nfix_w});
+    launch(sb, ngroups, AggNistFixPartTask{ctl, nfix_w, npart, Bc});
+    int nleft = ngroups;            // second level: at most Bc / 1024 partial sums reach the final thread
+    const uint32_t* nsum = npart;
+    if (nleft > 32) {
+      launch(sb, ngroups2, AggNistFixPartTask{ctl, npart, npart2, nleft});
+      nsum = npart2;
+      nleft = ngroups2;
+    }
+    if (fork) {
+      ev_record(ln.ev_join[0], sa);
+      ev_record(ln.ev_join[1], sb);
+      ev_wait(st, ln.ev_join[0]);
+      ev_wait(st, ln.ev_join[1]);
+    }
+    launch(st, 33, AggFinalTask{ctl, tA, tB, fproj, tp.D.nwin, tp.D.c, nA, nB, nsum, np.D.nwin, np.D.c, nleft});
+    c.agg_ctl = ctl;
+  }
+  {
+    const int nW = Bc * SG * MSM_NWIN, nWp = (nW + 31) & ~31, nG = Bc * MSM_NWIN;
+    launch(st, (long long)nWp + nG,
+           MsmTomWindowBothTask{MsmTomWindowTask{c.ent_scalar, c.ent_pre, c.ent_cnt, ET, K, V_ENT_PER_SAMPLE, 2, V_SEG, SG, c.win_w},
+                                MsmTomWindowTask{c.gk_scalar, c.gk_pre, nullptr, ngk, 0, 0, mode == 0 ? ngk : 0, V_SEG, 1, c.win_g}, nW, nWp, nG, ctl});
+  }
+  launch(st, (long long)Bc * MSM_NWIN_N, MsmP256WindowTask{c.nent_scalar, c.nent_aff, c.nent_skip, c.win_n, EN, ctl});
+  {
+    const int Bp = (Bc + 31) & ~31;
+    launch(st, 3ll * Bp, MsmCombineAllTask{MsmTomCombineTask{c.win_g, c.fx_proj, c.id_flags, 2, 0, 0},
+                                           MsmTomCombineTask{c.win_w, c.fx_proj, c.id_flags, 2, 1, 1, SG},
+                                           MsmP256CombineTask{c.win_n, c.nfix, c.id_flags}, Bc, Bp, ctl});
+  }
+  launch(st, Bc, VFinalTask{c});
+  return ctl;
+}
+
+// The prover's self-check of one chunk (include/zkattest.h, "Self-checked proving"), on the lane's stream behind
+// FinalizeTask: verifySignatureList with samples = sec_level over the rows pc just wrote, still on the device, against each
+// row's own ring; rows the prover accepted and the check does not are released like a row the prover rejected
+// (CheckReleaseTask).  key: k_b of row b at key + b * key_stride, key_len bytes; in: the chunk's inputs on the device;
+// counts: the lane's [checked, failed] rows of the call.
+void check_chunk(zka_ctx* ctx, const zka_params* P, Lane& ln, const ProveCtx& pc, const ProveRows& in, const RingSrc& ring,
+                 const uint32_t* ring_m, const uint8_t* key, size_t key_stride, int key_len, uint32_t b0, uint32_t* counts) {
+  Stream& st = ln.st;
+  const int Bc = pc.B, S = pc.S, n = pc.n;
+  const size_t tape_stride = verify_tape_len(n, S, S);   // a multiple of 16
+  Cursor k(ln.chk);
+  uint8_t* seeds = k.take<uint8_t>((size_t)Bc * 32);
+  uint8_t* todo = k.take<uint8_t>(Bc);
+  uint8_t* tape = k.take<uint8_t>((size_t)Bc * tape_stride);
+  uint8_t* ok = k.take<uint8_t>(Bc);
+  int32_t* vstatus = k.take<int32_t>(Bc);
+  // c_b before the verifier's chain takes the pool w: a hedged call's seeds live there
+  launch(st, Bc, CheckSeedTask{key, key_stride, key_len, pc.status, seeds, todo});
+  VerifyCtx c = verify_ctx(ctx, P, Bc, S, pc.N, n, S, 0);
+  c.msg_hash = in.msg_hash;
+  c.proofs = pc.proofs;
+  c.proof_stride = pc.proof_stride;
+  c.proof_len = pc.proof_len;
+  c.tape = tape;
+  c.tape_stride = tape_stride;
+  ring.fill(c, ring_m, in.ring_of);
+  const SeedVerifyTapeTask vt{seeds, tape, tape_stride, n, S, S, c.ring_of, c.ring_depth};
+  launch(st, (long long)Bc * vt.slots(), vt);
+  c.ok = ok;
+  c.status = vstatus;
+  verify_chunk(ctx, ln, c, b0, ctx->agg != 0, nullptr);
+  launch(st, (long long)Bc * FIN_PARTS, CheckReleaseTask{todo, ok, vstatus, pc.proofs, pc.proof_stride, pc.proof_len, pc.status, counts});
+}
+
 }  // namespace
 
 // =============================================================================== C ABI
@@ -897,7 +1139,7 @@ int zka_profile_reset(zka_ctx* ctx) {
   } catch (...) { return ZKA_E_CUDA; }
   return 0;
 }
-// knobs that may change between calls (tests, sweeps): "lanes", "chunk", "host_chunk"
+// knobs that may change between calls (tests, sweeps): "lanes", "chunk", "host_chunk", "agg", "agg_c", "self_check"
 int zka_set_option(zka_ctx* ctx, const char* key, long value) {
   if (!ctx || !key || value < 1) return ZKA_E_ARG;
   const std::string k(key);
@@ -921,6 +1163,9 @@ int zka_set_option(zka_ctx* ctx, const char* key, long value) {
       ctx->host_chunk = (int)value;
     } else if (k == "agg") {          // 1: off, 2: on (values start at 1)
       ctx->agg = (int)value - 1;
+    } else if (k == "self_check") {   // 1: off, 2: on
+      if (value > 2) return ZKA_E_ARG;
+      ctx->self_check = (int)value - 1;
     } else if (k == "agg_c") {
       if (value < 4 || value > 16) return ZKA_E_ARG;
       ctx->agg_c = (int)value;
@@ -936,6 +1181,8 @@ long long zka_stat(zka_ctx* ctx, const char* key) {
   std::lock_guard<std::mutex> g(ctx->stat_mu);
   if (k == "agg_pass") return (long long)ctx->agg_pass;
   if (k == "agg_fail") return (long long)ctx->agg_fail;
+  if (k == "self_check_rows") return (long long)ctx->self_check_rows;
+  if (k == "self_check_fail") return (long long)ctx->self_check_fail;
   if (k == "agg_c") return (long long)ctx->agg_c_last;        // window bits of the last tomEdwards256 aggregate MSM
   if (k == "tom_n_lo") return (long long)ctx->tom.n_lo;
   if (k == "tom_fallback") return ctx->tom_fallback ? 1 : 0;
@@ -1408,6 +1655,7 @@ int zka_key_to_int(zka_ctx* ctx, uint32_t count, const uint8_t* pk, uint8_t* x_o
 static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const ProveRows& rows, const RingSrc& ring, int mode) {
   const int S = (int)P->sec_level, n = ring.n;
   const bool hedge = rows.hedge, seeded = rows.seeds != nullptr || hedge;
+  const bool check = ctx->self_check && mode == 0;
   // seeded: the library's tape rows hold every draw a proof can read (a multiple of 32 bytes, so 16-byte aligned rows)
   const int seed_draws = prove_draws(S, n, S);
   const uint32_t* ring_m = ring.prepare(ctx, true, hedge);
@@ -1434,6 +1682,8 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
     Lane& ln = ctx->lane(li);
     Stream& st = ln.st;
     ProveRows cin[2];   // each slot's chunk, its inputs on the device
+    uint32_t* check_counts = check ? ln.chk_count.get<uint32_t>(2) : nullptr;   // copied back once, at the end of the call
+    if (check) dev_memset(st, check_counts, 0, 8);
     auto issue_inputs = [&](uint32_t k, int slot) {
       // the chunk's rows of an input: from its first row to the next chunk's
       const ProveRows r = rows.at(off[k]), e = rows.at(off[k + 1]);
@@ -1645,7 +1895,12 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
       launch(st, (long long)nA, RepEmitTask{c});
       if (mode == 0) launch(st, Bc, GkEmitTask{c});
       launch(st, (long long)Bc * FIN_PARTS, FinalizeTask{c});
-      // --- results: on the output stream, behind this chunk's last kernel
+      // --- self-check: k_b is the seed SeedProveTapeTask expanded, or the tape's first three draws
+      if (check) {
+        const uint8_t* key = seeded ? seeds : c.tape;
+        check_chunk(ctx, P, ln, c, cin[slot], ring, ring_m, key, seeded ? 32 : c.tape_stride, seeded ? 32 : 96, b0, check_counts);
+      }
+      // --- results: on the output stream, behind this chunk's last kernel (its self-check included)
       ev_record(ln.ev_done[slot], st);
       if (ctx->progress && k_this < ctx->progress_cap) notify_progress(st, ctx->progress + k_this);
       if (!po.dev || !lo.dev || !so.dev) {
@@ -1668,9 +1923,16 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
                 t_begin, t_mid, t_enq, t_comp, ms_now());
       }
     }
+    uint32_t counts[2] = {0, 0};
+    if (check) copy_d2h(st, counts, check_counts, sizeof(counts));
     sync(ln.cs_in);
     sync(ln.cs_out);
     sync(st);
+    if (check) {
+      std::lock_guard<std::mutex> g(ctx->stat_mu);
+      ctx->self_check_rows += counts[0];
+      ctx->self_check_fail += counts[1];
+    }
   };
   run_lanes(ctx, used, run_lane);
   return 0;
@@ -2101,201 +2363,10 @@ static int verify_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Veri
     }
     double t_in = 0.0;
     if (trace) { sync(st); t_in = ms_now(); }
-    const size_t ns = (size_t)Bc * K;
-    const int ET = c.ent_tom(), EN = c.ent_nist(), SG = c.segs();
-    const int ngk = 4 * n + 1;
-    Cursor w(ln.w);
-    c.rep_off = w.take<uint32_t>((size_t)Bc * S);
-    c.gk_off = w.take<uint32_t>(Bc);
-    c.tagbits = w.take<uint32_t>((size_t)Bc * 3);
-    c.chal = w.take<uint32_t>((size_t)Bc * 3);
-    c.gk_ok_len = w.take<uint8_t>(Bc);
-    c.r_aff = w.take<uint32_t>((size_t)Bc * 16);
-    c.q_aff = w.take<uint32_t>((size_t)Bc * 16);
-    c.q_inf = w.take<uint8_t>(Bc);
-    c.rpows = w.take<uint32_t>((size_t)Bc * RT_NWIN * P256_PROJ_WORDS);
-    c.rrows = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_PROJ_WORDS);
-    c.rtab = w.take<uint32_t>((size_t)Bc * RT_ENTRIES * P256_AFF_WORDS);
-    c.samp_idx = w.take<uint32_t>(ns);
-    c.samp_draw = w.take<uint32_t>(ns);
-    c.sp_T = w.take<uint32_t>(ns * P256_PROJ_WORDS);
-    c.sp_T_aff = w.take<uint32_t>(ns * 16);
-    c.sp_T_inf = w.take<uint8_t>(ns);
-    c.ta_jv = w.take<uint32_t>(ns * 2 * 8);
-    c.ta_jr = w.take<uint32_t>(ns * 2 * 8);
-    c.ta_proj = w.take<uint32_t>(ns * 2 * TOM_E2_WORDS);
-    c.ta_aff = w.take<uint32_t>(ns * 2 * TOM_AFF_WORDS);
-    c.td_proj = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_PROJ_WORDS);
-    c.td_aff = w.take<uint32_t>(ns * DERS_PER_ITEM * TOM_AFF_WORDS);
-    c.td_bytes = w.take<uint8_t>(ns * DERS_PER_ITEM * BSTRIDE);
-    c.item_chal = w.take<uint32_t>(ns * HASHES_PER_ITEM * 3);
-    c.ent_scalar = w.take<uint32_t>((size_t)Bc * ET * 8);
-    c.ent_off = w.take<uint32_t>((size_t)Bc * ET);
-    c.ent_pre = w.take<uint32_t>((size_t)Bc * ET * TOM_PRE_WORDS);
-    c.ent_cnt = w.take<uint32_t>(ns);
-    c.part = w.take<uint32_t>(ns * V_PART_WORDS);
-    // the small per-proof arrays before the entries and windows: the prover of this lane has small arrays at the
-    // same places of the pool, so these share its buffers without growing them much
-    c.fx_jv = w.take<uint32_t>((size_t)Bc * 2 * 8);
-    c.fx_jr = w.take<uint32_t>((size_t)Bc * 2 * 8);
-    c.fx_proj = w.take<uint32_t>((size_t)Bc * 2 * TOM_PROJ_WORDS);
-    c.nfix = w.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
-    c.id_flags = w.take<uint8_t>((size_t)Bc * 3);
-    c.gk_tape_bad = w.take_if<uint8_t>(mode == 0, Bc);
-    c.vkey = w.take<int32_t>(Bc);
-    c.nent_scalar = w.take<uint32_t>((size_t)Bc * EN * 8);
-    c.nent_aff = w.take<uint32_t>((size_t)Bc * EN * 16);
-    c.nent_skip = w.take<uint8_t>((size_t)Bc * EN);
-    c.gk_scalar = w.take<uint32_t>((size_t)Bc * ngk * 8);
-    c.gk_pre = w.take<uint32_t>((size_t)Bc * ngk * TOM_PRE_WORDS);
-    uint32_t* gk_offs = w.take<uint32_t>((size_t)Bc * ngk);
-    c.win_w = w.take<uint32_t>((size_t)Bc * SG * MSM_NWIN * 36);
-    c.win_g = w.take<uint32_t>((size_t)Bc * MSM_NWIN * 36);
-    c.win_n = w.take<uint32_t>((size_t)Bc * MSM_NWIN_N * P256_PROJ_WORDS);
-    c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * gk_blocks(n) * 8);
-    const bool agg = ctx->agg && mode == 0;
-    const size_t agg_tape_len = verify_tape_len(n, S, K);
-    const int agg_tp = agg_tape_pieces(agg_tape_len), agg_np = agg_tp + K + 1;
-    uint32_t* agg_wt = w.take_if<uint32_t>(agg, (size_t)Bc * AGG_WT * 8);
-    uint32_t* agg_dig = w.take_if<uint32_t>(agg, (size_t)Bc * agg_np * 8);
-    c.chal_full = w.take_if<uint32_t>(agg, (size_t)Bc * 8);
-    c.nfix_k = w.take_if<uint32_t>(agg, (size_t)Bc * 16);
     Cursor ob(ln.out[0]);
     c.ok = oo.rows(ob.next(), b0, Bc);
     c.status = so.rows(ob.next(), b0, Bc);
-
-    launch(st, Bc, VLayoutTask{c});
-    launch(st, (long long)Bc * (S + 1), VValidateTask{c});
-    {
-      // the per-proof tables of R (a 255-doubling chain per proof, rows, normalisation: no status writes) run beside the
-      // Fiat-Shamir hash of the repetitions (one thread per proof, 16 KB) unless per-kernel profiling is on
-      const bool fork = !st.profiling;
-      Stream& sr = fork ? ln.aux[0] : st;
-      if (fork) { ev_record(ln.ev_fork, st); ev_wait(sr, ln.ev_fork); }
-      launch(sr, Bc, P256PowsTask{c.r_aff, nullptr, c.rpows, Bc, RT_NWIN, RT_W});
-      launch(sr, (long long)Bc * RT_NWIN, P256RowsSignedTask{c.rpows, c.rrows});
-      launch_p256_norm(sr, c.rrows, c.rtab, nullptr, nullptr, (long long)Bc * RT_ENTRIES);
-      launch(st, Bc, VChallengeTask{c});
-      if (fork) { ev_record(ln.ev_join[0], sr); ev_wait(st, ln.ev_join[0]); }
-    }
-    // the Groth-Kohlweiss chain (ring polynomial, relations, offsets) only needs the layout: it runs on a side stream
-    // beside the sampled-repetition chain; its tape-range status is folded in by VReduceTask (same precedence)
-    const bool gk_fork = mode == 0 && !st.profiling;
-    if (gk_fork) {
-      ev_record(ln.ev_fork, st);
-      ev_wait(ln.aux[1], ln.ev_fork);
-    }
-    if (agg) {
-      // the aggregate's weights (zk_verify_agg.cuh) need the layout, the sampled repetitions and the exp challenge: they
-      // hash ahead of the GK chain on its side stream (joined before VReduceTask)
-      Stream& sw = gk_fork ? ln.aux[1] : st;
-      launch(sw, (long long)Bc * agg_np, AggPieceTask{c, agg_tape_len, agg_tp, agg_np, agg_dig});
-      launch(sw, Bc, AggWeightTask{c, c.chal_full, agg_dig, b0, agg_np, agg_wt});
-    }
-    if (gk_fork) {
-      verify_gk(ln.aux[1], c, gk_offs);
-      ev_record(ln.ev_join[1], ln.aux[1]);
-    }
-    launch(st, (long long)ns, VSampleP256Task{c});
-    launch_p256_norm(st, c.sp_T, c.sp_T_aff, nullptr, c.sp_T_inf, (long long)(ns));
-    launch(st, (long long)ns, VSampleJobsTask{c});
-    launch(st, (long long)ns * 2, TomCommitTask{c.ta_jv, c.ta_jr, c.tg_tab, c.th_tab, c.ta_proj, c.tom});
-    launch_tom_norm(st, c.ta_proj, c.ta_aff, nullptr, (long long)(ns * 2), 1);
-    launch(st, (long long)ns, VDerivedTask{c});
-    launch_tom_norm(st, c.td_proj, nullptr, c.td_bytes, (long long)(ns * DERS_PER_ITEM), 0);
-    launch(st, (long long)ns * HASHES_PER_ITEM, VItemHashTask{c});
-    dev_memset(st, c.ent_off, 0, (size_t)Bc * ET * 4);
-    launch(st, (long long)ns, VRelationsTask{c});
-    if (mode == 0) {
-      if (gk_fork) ev_wait(st, ln.ev_join[1]);
-      else verify_gk(st, c, gk_offs);
-    }
-    launch(st, Bc, VReduceTask{c});
-    launch(st, (long long)Bc * ET, VParseEntriesTask{c.proofs, c.proof_stride, c.ent_off, c.ent_pre, ET});
-    if (mode == 0) launch(st, (long long)Bc * ngk, VParseEntriesTask{c.proofs, c.proof_stride, gk_offs, c.gk_pre, ngk});
-    launch(st, (long long)Bc * 2, TomCommitTask{c.fx_jv, c.fx_jr, c.tg_tab, c.th_tab, c.fx_proj, c.tom, 1});
-    // chunk-wide aggregate check (zk_verify_agg.cuh): the sum over all proofs of the chunk of the three linear
-    // combinations, as ONE wide-window MSM per group; when both sums are the identity the per-proof MSMs below
-    // return at once
-    uint32_t* ctl = nullptr;
-    if (agg) {
-      Cursor A(ln.agg);
-      const int fgroups = (Bc * 2 + 63) / 64, ngroups = (Bc + 31) / 32, ngroups2 = (ngroups + 31) / 32;
-      ctl = A.take<uint32_t>(AGG_CTL_WORDS);
-#if !defined(ZKA_PG_WAR256)
-      uint32_t* tpart = A.take<uint32_t>((size_t)Bc * (K + 2) * 2 * PG_EXT_WORDS);
-#endif
-      uint32_t* fpart = A.take<uint32_t>((size_t)fgroups * 16);
-      uint32_t* fjv = A.take<uint32_t>(8);
-      uint32_t* fjr = A.take<uint32_t>(8);
-      uint32_t* fproj = A.take<uint32_t>(TOM_PROJ_WORDS);
-      uint32_t* nfix_w = A.take<uint32_t>((size_t)Bc * P256_PROJ_WORDS);
-      uint32_t* npart = A.take<uint32_t>((size_t)ngroups * P256_PROJ_WORDS);
-      uint32_t* npart2 = A.take_if<uint32_t>(ngroups > 32, (size_t)ngroups2 * P256_PROJ_WORDS);
-      dev_memset(st, ctl, 0, AGG_CTL_WORDS * 4);
-      launch(st, Bc, AggGateTask{c, ctl});
-      const AggTomSrc tsrc{c.ent_scalar, c.ent_pre, c.ent_cnt, c.gk_scalar, c.gk_pre, Bc, ET, K, ngk, agg_wt};
-      const AggNistSrc nsrc{c.nent_scalar, c.nent_aff, c.nent_skip, Bc, EN, agg_wt};
-      // three independent chains from here to AggFinalTask: the tomEdwards256 MSM (this stream), the torsion guard and the
-      // P-256 MSM with its fixed parts (two side streams; with per-kernel profiling on, everything stays on one stream
-      // so that the event pairs time one kernel at a time).  A skip flag raised by the torsion guard may reach the MSM
-      // kernels late — they then only do work AggFinalTask discards.
-      const bool fork = !st.profiling;
-      Stream& sa = fork ? ln.aux[0] : st;
-      Stream& sb = fork ? ln.aux[1] : st;
-      if (fork) {
-        ev_record(ln.ev_fork, st);
-        ev_wait(sa, ln.ev_fork);
-        ev_wait(sb, ln.ev_fork);
-      }
-#if !defined(ZKA_PG_WAR256)
-      // cofactor 4: no small-order components, or the per-proof path decides
-      launch(sa, (long long)Bc * (K + 2) * 2, AggTorsionPartTask{tsrc, ctl, tpart});
-      launch(sa, (long long)Bc * 2, AggTorsionTask{tpart, ctl, K});
-#endif
-      const AggPlan tp = agg_plan((double)Bc * (0.5 * K * V_ENT_PER_SAMPLE + 2 + ngk), ctx->agg_c);
-      const AggPlan np = agg_plan((double)Bc * EN, 0);
-      ctx->agg_c_last = tp.D.c;
-      const uint32_t *tA, *tB, *nA, *nB;
-      agg_msm(st, Cursor(ln.agg_tom), tsrc, tp, ctl, &tA, &tB);
-      agg_msm(sb, Cursor(ln.agg_nist), nsrc, np, ctl, &nA, &nB);
-      // fixed-base parts: one commitment for the summed weighted tomEdwards256 scalars, a two-level sum of the weighted
-      // P-256 points
-      launch(st, fgroups, AggFixPartTask{ctl, c.fx_jv, c.fx_jr, agg_wt, fpart, Bc});
-      launch(st, 1, AggFixSumTask{ctl, fpart, fjv, fjr, fgroups});
-      launch(st, 1, TomCommitTask{fjv, fjr, c.tg_tab, c.th_tab, fproj, c.tom, 1});
-      launch(sb, Bc, AggNistFixWeightTask{ctl, c.nfix_k, agg_wt, c.rtab, c.h_tab8, c.h_w, nfix_w});
-      launch(sb, ngroups, AggNistFixPartTask{ctl, nfix_w, npart, Bc});
-      int nleft = ngroups;            // second level: at most Bc / 1024 partial sums reach the final thread
-      const uint32_t* nsum = npart;
-      if (nleft > 32) {
-        launch(sb, ngroups2, AggNistFixPartTask{ctl, npart, npart2, nleft});
-        nsum = npart2;
-        nleft = ngroups2;
-      }
-      if (fork) {
-        ev_record(ln.ev_join[0], sa);
-        ev_record(ln.ev_join[1], sb);
-        ev_wait(st, ln.ev_join[0]);
-        ev_wait(st, ln.ev_join[1]);
-      }
-      launch(st, 33, AggFinalTask{ctl, tA, tB, fproj, tp.D.nwin, tp.D.c, nA, nB, nsum, np.D.nwin, np.D.c, nleft});
-      c.agg_ctl = ctl;
-    }
-    {
-      const int nW = Bc * SG * MSM_NWIN, nWp = (nW + 31) & ~31, nG = Bc * MSM_NWIN;
-      launch(st, (long long)nWp + nG,
-             MsmTomWindowBothTask{MsmTomWindowTask{c.ent_scalar, c.ent_pre, c.ent_cnt, ET, K, V_ENT_PER_SAMPLE, 2, V_SEG, SG, c.win_w},
-                                  MsmTomWindowTask{c.gk_scalar, c.gk_pre, nullptr, ngk, 0, 0, mode == 0 ? ngk : 0, V_SEG, 1, c.win_g}, nW, nWp, nG, ctl});
-    }
-    launch(st, (long long)Bc * MSM_NWIN_N, MsmP256WindowTask{c.nent_scalar, c.nent_aff, c.nent_skip, c.win_n, EN, ctl});
-    {
-      const int Bp = (Bc + 31) & ~31;
-      launch(st, 3ll * Bp, MsmCombineAllTask{MsmTomCombineTask{c.win_g, c.fx_proj, c.id_flags, 2, 0, 0},
-                                             MsmTomCombineTask{c.win_w, c.fx_proj, c.id_flags, 2, 1, 1, SG},
-                                             MsmP256CombineTask{c.win_n, c.nfix, c.id_flags}, Bc, Bp, ctl});
-    }
-    launch(st, Bc, VFinalTask{c});
+    const uint32_t* ctl = verify_chunk(ctx, ln, c, b0, ctx->agg && mode == 0, &ctx->agg_c_last);
     oo.copy_back(st, b0, c.ok, Bc);
     so.copy_back(st, b0, c.status, Bc);
     uint32_t hctl[AGG_CTL_WORDS] = {0, 0, 0, 0};
