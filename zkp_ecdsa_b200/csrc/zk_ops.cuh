@@ -386,32 +386,64 @@ ZK_HD void p256_accum_rtab(P256Pt& acc, const uint32_t* tab, const uint32_t* k) 
 }
 // Split commitments for the 34 jobs of a 0-bit repetition.  Several of them commit to the SAME value
 // with different blinders (proveMult: A_z and A_4_1 both commit k_z, mult.ts:112-113; proveEquality:
-// A_1 and A_2 both commit k, equality.ts:67-68), so the g-parts v*g are computed once per distinct
-// value (28 per item) and every job continues from its g-part with the 16 lookups of r*h:
-//   34 x 32 = 1088 lookups  ->  28 x 16 + 34 x 16 = 992.
+// A_1 and A_2 both commit k, equality.ts:67-68), and C4 of a MultProof commits x y, which is the value of another job:
+// i8 i9 = i10, i10 i10 = i11 and i10 i12 = i13 are computed as exactly these products (ItemScalarsTask), so C4 of
+// MultProofs 1..3 shares the g-part of C10, C11, C13; C4 of MultProof 0 commits i7 i8, which is 1, or 0 when x1 = x2
+// (invMod(0) = 0), and starts at its own value's table entry.  The g-parts v*g are computed once per distinct value
+// (24 per item) and every job continues from its g-part with the 11 lookups of r*h.
 #if defined(ZKA_PG_WAR256)
-enum : int { GJOBS_PER_ITEM = 28, TOM_EXT_WORDS = 24 };
+enum : int { GJOBS_PER_ITEM = 24, TOM_EXT_WORDS = 24 };
 #else
-enum : int { GJOBS_PER_ITEM = 28, TOM_EXT_WORDS = 36 };
+enum : int { GJOBS_PER_ITEM = 24, TOM_EXT_WORDS = 36 };
 #endif
-// job index (0..33) -> index of its g-part (0..27)
+// job index (0..33) -> index of its g-part (0..23), or -1: C4 of MultProof 0, whose value is 0 or 1
 ZK_HD int item_gpart_of_job(int j) {
   if (j < 6) return j;                       // T1x T1y C8 C10 C11 C13
-  if (j < 30) {                              // MultProof m: C4 Ax Ay Az A4_1 A4_2 -> 0 1 2 3 3 4
+  if (j < 30) {                              // MultProof m: C4 Ax Ay Az A4_1 A4_2 -> (C10 C11 C13 of m - 1) 0 1 2 2 3
     const int m = (j - 6) / 6, u = (j - 6) % 6;
-    return 6 + 5 * m + (u < 4 ? u : u - 1);
+    if (u == 0) return m ? 2 + m : -1;
+    return 6 + 4 * m + (u < 4 ? u - 1 : u - 2);
   }
-  return 26 + ((j - 30) >> 1);               // EqualityProof e: A1, A2 share k
+  return 22 + ((j - 30) >> 1);               // EqualityProof e: A1, A2 share k
 }
-// g-part index (0..27) -> a job that carries its value scalar
+// g-part index (0..23) -> a job that carries its value scalar
 ZK_HD int item_job_of_gpart(int g) {
   if (g < 6) return g;
-  if (g < 26) {
-    const int m = (g - 6) / 5, u = (g - 6) % 5;
-    return 6 + 6 * m + (u < 4 ? u : 5);
+  if (g < 22) {
+    const int m = (g - 6) / 4, u = (g - 6) % 4;
+    return 6 + 6 * m + (u < 3 ? u + 1 : 5);
   }
-  return 30 + 2 * (g - 26);
+  return 30 + 2 * (g - 22);
 }
+// Which g-part each job of a batch continues from, for the item jobs (gk_n = 0: items of JOBS_PER_ITEM jobs and
+// GJOBS_PER_ITEM g-parts) or for the Groth-Kohlweiss commitments (gk.ts:129-133, 173-176: rows of 4 gk_n slots cl, ca,
+// cb, cd of the row's depth n_r, zero jobs behind them, and 2 gk_n g-parts, those of ca_i at i and of cd_i at gk_n + i).
+// cl_i commits l_i in {0, 1} and cb_i commits l_i a_i, which is 0 or the value of ca_i, so only ca_i and cd_i are
+// walked over g.  A job whose value is 0 or 1 starts at that value's window-0 entry (the identity or g) whichever
+// g-part is named, and a job with no g-part (-1) always has such a value.
+struct GpartLayout {
+  int gk_n;                     // 0: item jobs; > 0: GK rows, the largest depth of the batch
+  const uint32_t* ring_of;      // GK rows of a ring set: the ring of each row and the depth of each ring (else null)
+  const uint32_t* ring_depth;
+  ZK_HD int jobs() const { return gk_n ? 4 * gk_n : JOBS_PER_ITEM; }      // per item or row
+  ZK_HD int gparts() const { return gk_n ? 2 * gk_n : GJOBS_PER_ITEM; }
+  ZK_HD int depth(int row) const { return ring_of ? (int)ring_depth[ring_of[row]] : gk_n; }
+  // the job whose value g-part g of `row` walks, or -1 (a row shallower than gk_n has no such g-part)
+  ZK_HD int job_of_gpart(int row, int g) const {
+    if (!gk_n) return item_job_of_gpart(g);
+    const int n = depth(row), i = g % gk_n;
+    return i < n ? (g < gk_n ? n : 3 * n) + i : -1;
+  }
+  // the g-part job j of `row` continues from, or -1
+  ZK_HD int gpart_of_job(int row, int j) const {
+    if (!gk_n) return item_gpart_of_job(j);
+    const int n = depth(row);
+    if (j < n || j >= 4 * n) return -1;     // cl_i, and the zero jobs
+    const int i = j % n;
+    return j < 3 * n ? i : gk_n + i;          // ca_i and cb_i: ca_i's g-part; cd_i: its own
+  }
+};
+ZK_HD bool scalar_le_one(const uint32_t* v) { return (v[0] >> 1 | v[1] | v[2] | v[3] | v[4] | v[5] | v[6] | v[7]) == 0; }
 #if defined(ZKA_PG_WAR256)
 #include "zk_ops_war.cuh"
 #else
@@ -685,15 +717,17 @@ struct TomCommitTask {
   }
 };
 
-struct TomCommitGTask {   // one thread per (item, g-part): K = v*g as an extended E2 point, from v's first entry
-  const uint32_t* jv;     // [items*34][8]
+struct TomCommitGTask {   // one thread per g-part of GpartLayout: K = v*g as an extended E2 point, from v's first entry
+  const uint32_t* jv;     // [rows * lay.jobs()][8]
   const uint32_t* gtab;
-  uint32_t* ext;          // [items*28][36]
+  uint32_t* ext;          // [rows * lay.gparts()][36]
   FbShape sh;
+  GpartLayout lay;
   ZK_HD void operator()(int t) const {
-    const int item = t / GJOBS_PER_ITEM, g = t % GJOBS_PER_ITEM;
+    const int row = t / lay.gparts(), jb = lay.job_of_gpart(row, t % lay.gparts());
+    if (jb < 0) return;
     uint32_t v[8];
-    ld<8>(v, jv + ((size_t)item * JOBS_PER_ITEM + item_job_of_gpart(g)) * 8);
+    ld<8>(v, jv + ((size_t)row * lay.jobs() + jb) * 8);
     uint32_t carry = 0;
     bool neg;
     TomPre q;
@@ -712,21 +746,30 @@ struct TomCommitGTask {   // one thread per (item, g-part): K = v*g as an extend
   }
 };
 struct TomCommitHTask {   // one thread per job: C = K + r*h, ending in tom2_madd_end for the normaliser
-  const uint32_t* jr;     // [items*34][8]
+  const uint32_t* jv;     // [rows * lay.jobs()][8]
+  const uint32_t* jr;
+  const uint32_t* gtab;
   const uint32_t* htab;
-  const uint32_t* ext;    // [items*28][36]
-  uint32_t* proj;         // [items*34][TOM_E2_WORDS]  (E, F, G, H) -> TomNormTask{e2 = 1}
+  const uint32_t* ext;    // [rows * lay.gparts()][36]
+  uint32_t* proj;         // [rows * lay.jobs()][TOM_E2_WORDS]  (E, F, G, H) -> TomNormTask{e2 = 1}
   FbShape sh;
+  GpartLayout lay;
   ZK_HD void operator()(int t) const {
-    const int item = t / JOBS_PER_ITEM, jb = t % JOBS_PER_ITEM;
-    uint32_t r[8];
-    ld<8>(r, jr + (size_t)t * 8);
+    const int row = t / lay.jobs(), g = lay.gpart_of_job(row, t % lay.jobs());
+    uint32_t v[8], r[8];
+    ld<8>(v, jv + (size_t)t * 8);
     TomPt acc;
-    const uint32_t* s = ext + ((size_t)item * GJOBS_PER_ITEM + item_gpart_of_job(jb)) * TOM_EXT_WORDS;
-    ld<9>(acc.x, s); ld<9>(acc.y, s + 9); ld<9>(acc.t, s + 18); ld<9>(acc.z, s + 27);
+    TomPre q;
+    if (g < 0 || scalar_le_one(v)) {   // K = v*g is the entry of v in window 0 (entry 0 is the identity)
+      tom2_ld_entry(q, gtab, sh, 0, v[0], false);
+      tom2_from_pre<TompCommit>(acc, q);
+    } else {
+      const uint32_t* s = ext + ((size_t)row * lay.gparts() + g) * TOM_EXT_WORDS;
+      ld<9>(acc.x, s); ld<9>(acc.y, s + 9); ld<9>(acc.t, s + 18); ld<9>(acc.z, s + 27);
+    }
+    ld<8>(r, jr + (size_t)t * 8);
     uint32_t carry = 0;
     bool neg;
-    TomPre q;
 #pragma unroll 1
     for (int j = 0; j < sh.nwin - 1; j++) {
       const uint32_t d = signed_digit(r, j, sh, carry, neg);

@@ -105,36 +105,47 @@ struct TomCommitTask {
     war_st_proj(proj + (size_t)t * TOM_PROJ_WORDS, acc);
   }
 };
-// the 34 jobs of a 0-bit repetition share 28 g-parts (see zk_ops.cuh)
-struct TomCommitGTask {   // one thread per (item, g-part): K = v*g
-  const uint32_t* jv;     // [items*34][8]
+// the jobs of a batch share g-parts as GpartLayout says (see zk_ops.cuh)
+ZK_HD void war_gpart(WarPt& acc, const uint32_t* gtab, const uint32_t* v, int w) {   // v*g
+  WarJac aj;
+  war_set_identity_jac(aj);
+  war_accum_fixed_jac(aj, gtab, v, w);
+  war_jac_to_hom(acc, aj);
+}
+struct TomCommitGTask {   // one thread per g-part of GpartLayout: K = v*g
+  const uint32_t* jv;     // [rows * lay.jobs()][8]
   const uint32_t* gtab;
-  uint32_t* ext;          // [items*28][24]
+  uint32_t* ext;          // [rows * lay.gparts()][24]
   FbShape sh;             // always uniform in this build: sh.w bits in every window
+  GpartLayout lay;
   ZK_HD void operator()(int t) const {
-    const int item = t / GJOBS_PER_ITEM, g = t % GJOBS_PER_ITEM;
+    const int row = t / lay.gparts(), jb = lay.job_of_gpart(row, t % lay.gparts());
+    if (jb < 0) return;
     uint32_t v[8];
-    ld<8>(v, jv + ((size_t)item * JOBS_PER_ITEM + item_job_of_gpart(g)) * 8);
-    WarJac aj;
-    war_set_identity_jac(aj);
-    war_accum_fixed_jac(aj, gtab, v, sh.w);
+    ld<8>(v, jv + ((size_t)row * lay.jobs() + jb) * 8);
     WarPt acc;
-    war_jac_to_hom(acc, aj);
+    war_gpart(acc, gtab, v, sh.w);
     war_st_proj(ext + (size_t)t * TOM_EXT_WORDS, acc);
   }
 };
 struct TomCommitHTask {   // one thread per job: C = K + r*h
-  const uint32_t* jr;     // [items*34][8]
+  const uint32_t* jv;     // [rows * lay.jobs()][8]
+  const uint32_t* jr;
+  const uint32_t* gtab;
   const uint32_t* htab;
-  const uint32_t* ext;    // [items*28][24]
-  uint32_t* proj;         // [items*34][24]
+  const uint32_t* ext;    // [rows * lay.gparts()][24]
+  uint32_t* proj;         // [rows * lay.jobs()][24]
   FbShape sh;             // always uniform in this build: sh.w bits in every window
+  GpartLayout lay;
   ZK_HD void operator()(int t) const {
-    const int item = t / JOBS_PER_ITEM, jb = t % JOBS_PER_ITEM;
-    uint32_t r[8];
+    const int row = t / lay.jobs(), g = lay.gpart_of_job(row, t % lay.jobs());
+    uint32_t v[8], r[8];
+    ld<8>(v, jv + (size_t)t * 8);
     ld<8>(r, jr + (size_t)t * 8);
     WarPt acc;
-    war_ld_proj(acc, ext + ((size_t)item * GJOBS_PER_ITEM + item_gpart_of_job(jb)) * TOM_EXT_WORDS);
+    // a value of 0 or 1: one table entry taken as (x : y : 1), or the identity
+    if (g < 0 || scalar_le_one(v)) war_gpart(acc, gtab, v, sh.w);
+    else war_ld_proj(acc, ext + ((size_t)row * lay.gparts() + g) * TOM_EXT_WORDS);
     war_accum_fixed(acc, htab, r, sh.w);
     war_st_proj(proj + (size_t)t * TOM_PROJ_WORDS, acc);
   }

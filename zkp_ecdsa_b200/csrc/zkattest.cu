@@ -821,13 +821,17 @@ void prove_store1(Stream& st, const ProveCtx& c) {
 // The c.M items of the 0-bit repetitions (pointAdd.ts:92-163 each), from their secrets to their bytes in the proof rows,
 // and the Groth-Kohlweiss commitments of the membership proof (gk.ts:129-176) with their encodings, behind the items in
 // the s2 arrays.  The stages of the two alternate (with host buffers the batched prover was measurably slower with one
-// chain after the other); provePointAdd alone runs only the items, proveMembership alone only the GK part.  gext: [M][GJOBS_PER_ITEM] g-parts of the item commitments;
-// c.gk_part: the block sums when the ring is cut into blocks.
+// chain after the other); provePointAdd alone runs only the items, proveMembership alone only the GK part.  gext:
+// prove_gext_words(c) words for the g-parts of the commitments (GpartLayout), [M][GJOBS_PER_ITEM] of the items and
+// behind them [B][2n] of the GK rows; c.gk_part: the block sums when the ring is cut into blocks.
+size_t prove_gext_words(const ProveCtx& c) { return ((size_t)c.M * GJOBS_PER_ITEM + (size_t)c.B * 2 * c.n) * TOM_EXT_WORDS; }
 void prove_items_gk(Stream& st, const ProveCtx& c, uint32_t* gext, bool items, bool gk) {
   const long long M = c.M, nj = M * JOBS_PER_ITEM, nd = M * DERS_PER_ITEM;
   const long long Bn = (long long)c.B * c.n, ng = 4 * Bn;
   const int nblk = gk_blocks(c.n);
   const size_t g0 = c.s2_gk(0, 0);
+  const GpartLayout item_lay{0, nullptr, nullptr}, gk_lay{c.n, c.ring_of, c.ring_depth};
+  uint32_t* gk_ext = gext + (size_t)M * GJOBS_PER_ITEM * TOM_EXT_WORDS;
   if (items) {
     launch(st, (M + ITEM_INV_CHUNK - 1) / ITEM_INV_CHUNK, ItemInvTask{c});
     launch(st, M, ItemScalarsTask{c});
@@ -839,11 +843,14 @@ void prove_items_gk(Stream& st, const ProveCtx& c, uint32_t* gext, bool items, b
     launch(st, Bn, GkCdJobsTask{c});
   }
   if (items) {   // item jobs: g-parts once per distinct committed value, then r*h on top (TomCommitG/HTask)
-    launch(st, M * GJOBS_PER_ITEM, TomCommitGTask{c.s2_jv, c.tg_tab, gext, c.tom});
-    launch(st, nj, TomCommitHTask{c.s2_jr, c.th_tab, gext, c.s2_proj, c.tom});
+    launch(st, M * GJOBS_PER_ITEM, TomCommitGTask{c.s2_jv, c.tg_tab, gext, c.tom, item_lay});
+    launch(st, nj, TomCommitHTask{c.s2_jv, c.s2_jr, c.tg_tab, c.th_tab, gext, c.s2_proj, c.tom, item_lay});
   }
-  if (gk)
-    launch(st, ng, TomCommitTask{c.s2_jv + g0 * 8, c.s2_jr + g0 * 8, c.tg_tab, c.th_tab, c.s2_proj + g0 * TOM_E2_WORDS, c.tom});
+  if (gk) {      // GK jobs: g-parts of ca_i and cd_i only
+    launch(st, 2 * Bn, TomCommitGTask{c.s2_jv + g0 * 8, c.tg_tab, gk_ext, c.tom, gk_lay});
+    launch(st, ng, TomCommitHTask{c.s2_jv + g0 * 8, c.s2_jr + g0 * 8, c.tg_tab, c.th_tab, gk_ext, c.s2_proj + g0 * TOM_E2_WORDS,
+                                  c.tom, gk_lay});
+  }
   if (items) {
     // only T1x, T1y (jobs 0, 1 of each item) are needed again as points (DerivedTask)
     launch_tom_norm(st, c.s2_proj, c.s2_aff, c.s2_bytes, nj, 1, JOBS_PER_ITEM, 2);
@@ -1886,7 +1893,7 @@ static int prove_impl(zka_ctx* ctx, const zka_params* P, uint32_t B, const Prove
       c.item_inv = w.take<uint32_t>((size_t)M * 8);
       c.item_chal = w.take<uint32_t>((size_t)M * HASHES_PER_ITEM * 3);
       c.gk_part = w.take_if<uint32_t>(gk_blocks(n) > 1, (size_t)Bc * n * gk_blocks(n) * 8);
-      uint32_t* gext = w.take<uint32_t>((size_t)M * GJOBS_PER_ITEM * TOM_EXT_WORDS);
+      uint32_t* gext = w.take<uint32_t>(prove_gext_words(c));
       launch(st, Bc, ItemsTask{c});
       // --- phase B
       launch(st, M, PhaseBP256Task{c});
@@ -2135,8 +2142,9 @@ int zka_prove_membership_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, co
       c.proofs = po.rows(ob.next(), b0, Bc);
       c.proof_len = lo.rows(ob.next(), b0, Bc);
       c.status = so.rows(ob.next(), b0, Bc);
+      uint32_t* gext = w.take<uint32_t>(prove_gext_words(c));
       launch(st, Bc, GkAloneSetupTask{c, d_cr, d_tape, tape_stride, itape});
-      prove_items_gk(st, c, nullptr, false, true);
+      prove_items_gk(st, c, gext, false, true);
       launch(st, Bc, GkEmitTask{c});
       launch(st, (long long)Bc * FIN_PARTS, FinalizeTask{c});
       po.copy_back_2d(st, b0, c.proofs, Bc, (size_t)gk_len(n));
@@ -2246,7 +2254,7 @@ int zka_prove_pointadd_batch(zka_ctx* ctx, const zka_params* P, uint32_t B, cons
       c.secrets = w.take<uint32_t>((size_t)Bc * SECRETS_PER_ITEM * 8);
       c.item_inv = w.take<uint32_t>((size_t)Bc * 8);
       c.item_chal = w.take<uint32_t>((size_t)Bc * HASHES_PER_ITEM * 3);
-      uint32_t* gext = w.take<uint32_t>((size_t)Bc * GJOBS_PER_ITEM * TOM_EXT_WORDS);
+      uint32_t* gext = w.take<uint32_t>(prove_gext_words(c));
       c.proof_stride = row_stride;
       c.proofs = w.take<uint8_t>((size_t)Bc * row_stride);
       c.proof_len = w.take<uint32_t>(Bc);
