@@ -96,6 +96,31 @@
  * sub-proof provers (zka_prove_exp_batch, zka_prove_membership_batch, zka_prove_equality_batch, zka_prove_mult_batch,
  * zka_prove_pointadd_batch) are never checked.
  *
+ * Traceable proofs (zka_prove_batch_traced[_seeded], zka_verify_batch_traced[_seeded], zka_open_batch).  An opener with
+ * the key sk in [1, q) and Y = sk g (zka_trace_pubkey) can say which ring member made a traced proof; without sk the proof
+ * stays anonymous in its ring.  g, h are the proof group's generator and params' ProofGroup.h, q its order (= p256.p), PB /
+ * SB its point / scalar bytes (67 / 33 tomEdwards256, 65 / 32 war256), || concatenation.  A traced row is the untraced row
+ * of the same call, byte for byte, followed by a trace block of zka_trace_len() = 5 PB + 3 SB bytes (434 / 421):
+ *   witness   x = the x-coordinate of pk (the value keyXcom commits to), r = the blinder of keyXcom (prover draw 1)
+ *   draws     k, a, beta, c in [0, q): tape calls read four 32-byte big-endian draws at tape bytes [L, L + 128),
+ *             L = zka_prove_tape_len(N, S) (a draw >= q gives ZKA_ERR_TAPE_RANGE); seeded calls draw t = 0..3 as rnd(q) on
+ *             stream(seed, 4, t) (the rule of "Seeded randomness", domain 4)
+ *   block     C1 = k g, C2 = x g + k Y, A0 = a g + beta h, A1 = c g, A2 = a g + c Y,
+ *             e = SHA-256("ZKAttest/trace/v1" || params digest (32, "Hedged seeds") || Y || msg_hash || proof bytes
+ *                 [0, HEAD_LEN) (R comS1 keyXcom keyYcom) || C1 || C2 || A0 || A1 || A2) big-endian mod q,
+ *             s_x = a + e x, s_r = beta + e r, s_k = c + e k (mod q);  block = C1 C2 A0 A1 A2 s_x s_r s_k
+ * Only rows the untraced call accepted get a block (proof_len grows by zka_trace_len()); a rejected row stays zeroed with
+ * its status.  A trace point that is the war256 identity gives ZKA_ERR_IDENTITY_ENC.  With "self_check" on, every block is
+ * also checked on the device and a row whose block fails gets ZKA_ERR_SELF_CHECK (counted in "self_check_fail").
+ * Verify: a row shorter than the block, or whose block does not parse (points as the proof parser demands, scalars < q),
+ * gives ZKA_ERR_MALFORMED (top precedence); otherwise the row gets the untraced verdict of its first proof_len -
+ * zka_trace_len() bytes, and an accepted row also needs s_x g + s_r h = A0 + e keyXcom, s_k g = A1 + e C1 and
+ * s_x g + s_k Y = A2 + e C2, or it gets ok = 0 with status 0.  The check is exact and uses no randomness.
+ * Open: the block is parsed (ZKA_ERR_MALFORMED) and its relations checked (ZKA_ERR_TRACE_INVALID); the base proof is not
+ * verified (verify first).  D = C2 - sk C1 = x g, and the row's index is the smallest j < N with (ring[j] mod q) g = D,
+ * or 0xFFFFFFFF with ZKA_ERR_NOT_IN_RING.  Hashing the header binds a block to its proof's keyXcom, whose blinder is fresh.
+ * Not covered: ring sets, hedged calls, the stand-alone sub-proofs, and a proof that an opening is correct.
+ *
  * Pointers may be host or CUDA device pointers (detected per argument); host buffers are
  * staged through the library's stream.  The caller owns every buffer.
  * Return value: 0 on success, negative on a fatal (argument/CUDA) error — see zka_last_error.
@@ -127,7 +152,9 @@ enum {
   ZKA_ERR_R_INFINITY = 8,        /* 'R is at infinity'                           zkpAttestList.ts:159 */
   ZKA_ERR_MALFORMED = 9,         /* proof bytes do not parse (deserializePoint / deserializeScalar throw) */
   ZKA_ERR_PARAMS_NOT_FOUND = 10, /* exp.ts:270,302 */
-  ZKA_ERR_SELF_CHECK = 11        /* proof failed its self-check ("self_check" option, see "Self-checked proving") */
+  ZKA_ERR_SELF_CHECK = 11,       /* proof failed its self-check ("self_check" option, see "Self-checked proving") */
+  ZKA_ERR_TRACE_INVALID = 12,    /* zka_open_batch: the trace block fails a relation under Y = sk g ("Traceable proofs") */
+  ZKA_ERR_NOT_IN_RING = 13       /* zka_open_batch: the traced key is no entry of the ring */
 };
 /* Precedence: a row with several defects gets the code of the one the reference meets first.
  *   verify (zka_verify_batch*, zka_verify_exp_batch):  ZKA_ERR_MALFORMED (the whole proof is parsed first, so it wins over
@@ -291,6 +318,36 @@ int zka_hedge_seeds(zka_ctx* ctx, const zka_params* params, uint32_t B, const ui
 int zka_hedge_seeds_rings(zka_ctx* ctx, const zka_params* params, const zka_rings* rings, const uint32_t* ring_of, uint32_t B,
                           const uint8_t* msg_hash, const uint8_t* sig, const uint8_t* pk, const uint32_t* which,
                           const uint8_t* seeds /* B x 32 or NULL */, uint8_t* out /* B x 32 */);
+
+/* ---- traceable proofs (rule under "Traceable proofs" above) ----
+ * zka_trace_pubkey: Y = sk g (sk: 32 bytes big-endian in [1, q)).  zka_prove_batch_traced[_seeded]: the arguments of
+ * zka_prove_batch[_seeded] plus Y; tape_stride must be >= zka_prove_tape_len(N, S) + 128 and proof_stride >=
+ * zka_proof_max_len(N, S) + zka_trace_len().  zka_verify_batch_traced[_seeded]: the arguments of zka_verify_batch_ex /
+ * zka_verify_batch_seeded plus Y.  zka_open_batch: sk, and per row the message hash the proof was made for (it is hashed
+ * into e), the ring and the traced proofs; index[i] and status[i] per row.  A Y that does not parse as a point, or an sk of
+ * 0 or >= q, gives ZKA_E_ARG.  Chunk schedule and progress flags are those of the untraced call (a flag is raised once
+ * its chunk's blocks are in place). */
+size_t zka_trace_len(void);
+int zka_trace_pubkey(zka_ctx* ctx, const uint8_t sk[32], uint8_t* Y /* point_bytes */);
+int zka_prove_batch_traced(zka_ctx* ctx, const zka_params* params, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
+                           const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* tape,
+                           size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len, int32_t* status,
+                           const uint8_t* Y);
+int zka_prove_batch_traced_seeded(zka_ctx* ctx, const zka_params* params, uint32_t B, const uint8_t* msg_hash,
+                                  const uint8_t* sig, const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N,
+                                  const uint8_t* seeds, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len,
+                                  int32_t* status, const uint8_t* Y);
+int zka_verify_batch_traced(zka_ctx* ctx, const zka_params* params, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
+                            uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                            const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples,
+                            const uint8_t* Y);
+int zka_verify_batch_traced_seeded(zka_ctx* ctx, const zka_params* params, uint32_t B, const uint8_t* msg_hash,
+                                   const uint8_t* ring, uint32_t N, const uint8_t* proofs, size_t proof_stride,
+                                   const uint32_t* proof_len, const uint8_t* seeds, uint32_t samples, uint8_t* ok,
+                                   int32_t* status, const uint8_t* Y);
+int zka_open_batch(zka_ctx* ctx, const zka_params* params, const uint8_t sk[32], uint32_t B, const uint8_t* msg_hash /* B x 32 */,
+                   const uint8_t* ring /* N x 32 */, uint32_t N, const uint8_t* proofs, size_t proof_stride,
+                   const uint32_t* proof_len, uint32_t* index /* B */, int32_t* status /* B */);
 
 /* ---- stand-alone sub-proof verifiers: the surface of the reference's own unit tests and benches ----
  * verifyExp(paramsNIST, paramsWario, Clambda, Px, Py, pi, secparam, Q?)   /root/reference/src/exp/exp.ts:233-349

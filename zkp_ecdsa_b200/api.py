@@ -375,6 +375,69 @@ class Engine:
                                            samples, ok, status)
         return ok, status
 
+    # ------------------------------------------------------------------ traceable proofs (include/zkattest.h)
+    def trace_keypair(self, sk: Optional[int] = None):
+        """(sk, Y): an opener key sk in [1, q) (default: from the OS CSPRNG) and its public key Y = sk g (point bytes).
+        Whoever holds sk can open every traced proof made to Y to its signer's ring index."""
+        if sk is None:
+            while True:
+                sk = int.from_bytes(os.urandom(32), 'big')
+                if 0 < sk < TOM_ORDER:
+                    break
+        return sk, self.lib.trace_pubkey(np.frombuffer(int(sk).to_bytes(32, 'big'), np.uint8).copy())
+
+    def _traced_rows(self, B, N, params, proofs):
+        stride = self.lib.proof_max_len(N, params.sec_level) + self.lib.trace_len()
+        if proofs is None:
+            proofs = np.zeros((B, stride), np.uint8)
+        return proofs, np.zeros(B, np.uint32), np.zeros(B, np.int32)
+
+    def prove_batch_traced(self, params, msg_hash, sig, pk, which, ring, tape, Y: bytes, proofs=None) -> ProveResult:
+        """prove_batch whose accepted rows also carry a trace block to the opener key Y; tape rows need
+        zka_prove_tape_len + 128 bytes (the four trace draws behind the prover's)."""
+        B, N = msg_hash.shape[0], ring.shape[0]
+        proofs, plen, status = self._traced_rows(B, N, params, proofs)
+        self.lib.prove_batch_traced(params.handle, B, msg_hash, sig, pk, which, ring, N, tape, tape.shape[1], proofs, proofs.shape[1],
+                                    plen, status, Y)
+        return ProveResult(proofs, plen, status)
+
+    def prove_batch_traced_seeded(self, params, msg_hash, sig, pk, which, ring, Y: bytes, seeds=None, proofs=None) -> ProveResult:
+        """prove_batch_seeded with trace blocks to the opener key Y.  Default seeds: os.urandom(32 * B)."""
+        B, N = msg_hash.shape[0], ring.shape[0]
+        seeds = _seed_rows(os.urandom(32 * B), B) if seeds is None else seeds
+        proofs, plen, status = self._traced_rows(B, N, params, proofs)
+        self.lib.prove_batch_traced_seeded(params.handle, B, msg_hash, sig, pk, which, ring, N, seeds, proofs, proofs.shape[1], plen,
+                                           status, Y)
+        return ProveResult(proofs, plen, status)
+
+    def verify_batch_traced(self, params, msg_hash, ring, proofs, proof_len, tape, Y: bytes, samples: int = 20):
+        """verify_batch_ex of traced rows: the untraced verdict of each row's proof and the check of its trace block."""
+        B = msg_hash.shape[0]
+        ok = np.zeros(B, np.uint8)
+        status = np.zeros(B, np.int32)
+        self.lib.verify_batch_traced(params.handle, B, msg_hash, ring, ring.shape[0], proofs, proofs.shape[1], proof_len, tape,
+                                     tape.shape[1], ok, status, samples, Y)
+        return ok, status
+
+    def verify_batch_traced_seeded(self, params, msg_hash, ring, proofs, proof_len, Y: bytes, seeds=None, samples: int = 20):
+        B = msg_hash.shape[0]
+        seeds = _seed_rows(os.urandom(32 * B), B) if seeds is None else seeds
+        ok = np.zeros(B, np.uint8)
+        status = np.zeros(B, np.int32)
+        self.lib.verify_batch_traced_seeded(params.handle, B, msg_hash, ring, ring.shape[0], proofs, proofs.shape[1], proof_len, seeds,
+                                            samples, ok, status, Y)
+        return ok, status
+
+    def open_batch(self, params, sk: int, msg_hash, ring, proofs, proof_len):
+        """(index, status) per traced row: the smallest ring index whose key made the proof (status 0), or 0xFFFFFFFF
+        with status 9 (block does not parse), 12 (block fails its relations) or 13 (key not in the ring / wrong sk)."""
+        B = msg_hash.shape[0]
+        index = np.zeros(B, np.uint32)
+        status = np.zeros(B, np.int32)
+        self.lib.open_batch(params.handle, np.frombuffer(int(sk).to_bytes(32, 'big'), np.uint8).copy(), B, msg_hash, ring,
+                            ring.shape[0], proofs, proofs.shape[1], proof_len, index, status)
+        return index, status
+
 
 def _seed_rows(seed: bytes, rows: int) -> np.ndarray:
     if len(seed) != 32 * rows:

@@ -32,7 +32,8 @@ SYMBOLS = [
     'zka_prove_batch_seeded', 'zka_verify_batch_seeded', 'zka_seed_tape',
     'zka_rings_create', 'zka_rings_destroy', 'zka_prove_batch_rings', 'zka_prove_batch_rings_seeded', 'zka_verify_batch_rings',
     'zka_verify_batch_rings_seeded', 'zka_prove_batch_hedged', 'zka_prove_batch_rings_hedged', 'zka_hedge_seeds',
-    'zka_hedge_seeds_rings',
+    'zka_hedge_seeds_rings', 'zka_trace_len', 'zka_trace_pubkey', 'zka_prove_batch_traced', 'zka_prove_batch_traced_seeded',
+    'zka_verify_batch_traced', 'zka_verify_batch_traced_seeded', 'zka_open_batch',
 ]
 
 STATUS_MESSAGES = {
@@ -48,6 +49,8 @@ STATUS_MESSAGES = {
     9: 'malformed proof bytes',
     10: 'params not found',                  # exp.ts:270,302
     11: 'proof failed its self-check',       # zka_set_option(ctx, "self_check", 2)
+    12: 'trace block fails its relations',   # zka_open_batch
+    13: 'traced key is not in the ring',     # zka_open_batch
 }
 
 
@@ -180,6 +183,16 @@ class ZkaLib:
             L.zka_prove_batch_rings_hedged.argtypes = L.zka_prove_batch_rings_seeded.argtypes
             L.zka_hedge_seeds.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 5 + [C.c_uint32, C.c_void_p, C.c_void_p]
             L.zka_hedge_seeds_rings.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 6
+        if hasattr(L, 'zka_open_batch'):
+            L.zka_trace_len.restype = C.c_size_t
+            L.zka_trace_len.argtypes = []
+            L.zka_trace_pubkey.argtypes = [C.c_void_p] * 3
+            L.zka_prove_batch_traced.argtypes = L.zka_prove_batch.argtypes + [C.c_void_p]
+            L.zka_prove_batch_traced_seeded.argtypes = L.zka_prove_batch_seeded.argtypes + [C.c_void_p]
+            L.zka_verify_batch_traced.argtypes = L.zka_verify_batch_ex.argtypes + [C.c_void_p]
+            L.zka_verify_batch_traced_seeded.argtypes = L.zka_verify_batch_seeded.argtypes + [C.c_void_p]
+            L.zka_open_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
+                                         C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
         ctx = C.c_void_p()
         rc = L.zka_init(device, C.byref(ctx))
         if rc != 0 or not ctx:
@@ -381,6 +394,41 @@ class ZkaLib:
         self._check(self.lib.zka_hedge_seeds_rings(self.ctx, params, rings, _ptr(ring_of), B, _ptr(msg_hash), _ptr(sig), _ptr(pk),
                                                    _ptr(which), _ptr(seeds), _ptr(out)), 'zka_hedge_seeds_rings')
         return out
+
+    # ------------------------------------------------------------------ traceable proofs (Y: the opener key, point bytes)
+    def trace_len(self) -> int:
+        return int(self.lib.zka_trace_len())
+
+    def trace_pubkey(self, sk) -> bytes:
+        Y = np.zeros(self.wp, np.uint8)
+        self._check(self.lib.zka_trace_pubkey(self.ctx, _ptr(sk), _ptr(Y)), 'zka_trace_pubkey')
+        return Y.tobytes()
+
+    def prove_batch_traced(self, params, B, msg_hash, sig, pk, which, ring, N, tape, tape_stride, proofs, proof_stride, proof_len,
+                           status, Y):
+        self._check(self.lib.zka_prove_batch_traced(self.ctx, params, B, _ptr(msg_hash), _ptr(sig), _ptr(pk), _ptr(which), _ptr(ring),
+                                                    N, _ptr(tape), tape_stride, _ptr(proofs), proof_stride, _ptr(proof_len),
+                                                    _ptr(status), _ptr(Y)), 'zka_prove_batch_traced')
+
+    def prove_batch_traced_seeded(self, params, B, msg_hash, sig, pk, which, ring, N, seeds, proofs, proof_stride, proof_len, status, Y):
+        self._check(self.lib.zka_prove_batch_traced_seeded(self.ctx, params, B, _ptr(msg_hash), _ptr(sig), _ptr(pk), _ptr(which),
+                                                           _ptr(ring), N, _ptr(seeds), _ptr(proofs), proof_stride, _ptr(proof_len),
+                                                           _ptr(status), _ptr(Y)), 'zka_prove_batch_traced_seeded')
+
+    def verify_batch_traced(self, params, B, msg_hash, ring, N, proofs, proof_stride, proof_len, tape, tape_stride, ok, status, samples,
+                            Y):
+        self._check(self.lib.zka_verify_batch_traced(self.ctx, params, B, _ptr(msg_hash), _ptr(ring), N, _ptr(proofs), proof_stride,
+                                                     _ptr(proof_len), _ptr(tape), tape_stride, _ptr(ok), _ptr(status), samples, _ptr(Y)),
+                    'zka_verify_batch_traced')
+
+    def verify_batch_traced_seeded(self, params, B, msg_hash, ring, N, proofs, proof_stride, proof_len, seeds, samples, ok, status, Y):
+        self._check(self.lib.zka_verify_batch_traced_seeded(self.ctx, params, B, _ptr(msg_hash), _ptr(ring), N, _ptr(proofs),
+                                                            proof_stride, _ptr(proof_len), _ptr(seeds), samples, _ptr(ok), _ptr(status),
+                                                            _ptr(Y)), 'zka_verify_batch_traced_seeded')
+
+    def open_batch(self, params, sk, B, msg_hash, ring, N, proofs, proof_stride, proof_len, index, status):
+        self._check(self.lib.zka_open_batch(self.ctx, params, _ptr(sk), B, _ptr(msg_hash), _ptr(ring), N, _ptr(proofs), proof_stride,
+                                            _ptr(proof_len), _ptr(index), _ptr(status)), 'zka_open_batch')
 
     # ------------------------------------------------------------------ stand-alone sub-proof verifiers
     def verify_exp_batch(self, params, base, com, px, py, q, proofs, proof_len, tape, samples):

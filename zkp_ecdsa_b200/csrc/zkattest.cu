@@ -23,7 +23,11 @@
 #include "zk_launch.cuh"
 #include "zk_prove.cuh"
 #include "zk_seed.cuh"
+#include "zk_trace.cuh"
 #include "zk_verify_agg.cuh"
+#if !defined(ZKA_HOSTSIM)
+#include <cub/device/device_radix_sort.cuh>
+#endif
 
 namespace zk {
 // ---- small helper tasks of the C ABI layer (namespace scope: kernel template arguments) ----
@@ -343,6 +347,7 @@ struct zka_ctx : Lane {
   DevBuf tg_bytes;        // 67-byte encoding of g
   DevBuf lag;             // GK Lagrange matrix cache
   int lag_n = -1;
+  DevBuf trace[32];       // workspace of the trace stages (zk_trace.cuh), which run after the untraced passes
 };
 
 struct zka_params {
@@ -2646,6 +2651,383 @@ int zka_proofs_pack(zka_ctx* ctx, uint32_t B, const uint8_t* proofs, size_t proo
 int zka_proofs_unpack(zka_ctx* ctx, uint32_t B, const uint8_t* packed, size_t cap, const uint32_t* proof_len, uint8_t* proofs,
                       size_t proof_stride, uint64_t* offsets, void* stream) {
   return pack_common(ctx, B, proofs, proof_stride, proof_len, const_cast<uint8_t*>(packed), cap, offsets, stream, 1);
+}
+
+
+// ---------------------------------------------------------------------------- traceable proofs (zk_trace.cuh)
+// The trace stages run on the context's stream after the untraced pass of the call, TRACE_CHUNK rows at a time (the
+// prover: over the untraced call's own chunks, whose progress flags are raised once their blocks are in place).
+namespace {
+constexpr uint32_t TRACE_CHUNK = 4096;
+
+// the opener key Y on the device when it parses as a point of the proof group, else null
+const uint8_t* trace_y(zka_ctx* ctx, DevBuf& buf, const uint8_t* Y) {
+  Stream& st = ctx->st;
+  uint8_t* d = buf.get<uint8_t>(WP + 16);
+  uint32_t* aff = reinterpret_cast<uint32_t*>(ctx->trace[0].get<uint32_t>(TOM_AFF_WORDS));
+  copy_h2d(st, d, Y, WP);
+  launch(st, 1, ParsePointsTask{nullptr, d, nullptr, aff, d + WP, nullptr});
+  uint8_t bad = 1;
+  copy_d2h(st, &bad, d + WP, 1);
+  sync(st);
+  return bad ? nullptr : d;
+}
+// sk (32 bytes big-endian, host or device) as limbs; false unless 1 <= sk < q
+bool trace_sk(zka_ctx* ctx, const uint8_t* sk, uint32_t* out) {
+  uint8_t h[32];
+  copy_d2h(ctx->st, h, sk, 32);
+  sync(ctx->st);
+  limbs_from_be<8>(out, h, 32);
+  return !is_zero_n<8>(out) && lt_p<FpP256>(out);
+}
+// the encoding of sk g on the device (BSTRIDE bytes)
+uint8_t* trace_pubkey_dev(zka_ctx* ctx, const uint32_t* skl, Cursor& w) {
+  Stream& st = ctx->st;
+  uint32_t* jv = w.take<uint32_t>(8);
+  uint32_t* jr = w.take<uint32_t>(8);
+  uint32_t* proj = w.take<uint32_t>(TOM_PROJ_WORDS);
+  uint8_t* bytes = w.take<uint8_t>(BSTRIDE);
+  copy_h2d(st, jv, skl, 32);
+  dev_memset(st, jr, 0, 32);
+  launch(st, 1, TomCommitTask{jv, jr, ctx->tg.tab, ctx->tg.tab, proj, ctx->tom, 1});
+  launch(st, 1, TraceToE1Task{proj});
+  launch_tom_norm(st, proj, nullptr, bytes, 1, 0);
+  return bytes;
+}
+// headers and blocks of rows [b0, b0 + Bc) on the device: device rows through TraceGatherTask; host rows are gathered on
+// the host, so that only the header and the block of each row cross PCIe
+void trace_gather(zka_ctx* ctx, Cursor& w, const uint8_t* proofs, size_t stride, const uint32_t* len, uint32_t b0, int Bc,
+                  uint8_t** hdr, uint8_t** blk, uint8_t** shortrow) {
+  Stream& st = ctx->st;
+  *hdr = w.take<uint8_t>((size_t)Bc * HEAD_LEN);
+  *blk = w.take<uint8_t>((size_t)Bc * TRACE_LEN);
+  *shortrow = w.take<uint8_t>(Bc);
+  DevBuf& lb = w.next();
+  if (is_device_ptr(proofs)) {
+    const uint32_t* dl = stage_in(st, lb, len + b0, (size_t)Bc);
+    launch(st, Bc, TraceGatherTask{proofs + (size_t)b0 * stride, stride, dl, *hdr, *blk, *shortrow});
+    return;
+  }
+  std::vector<uint32_t> hl((size_t)Bc);
+  copy_d2h(st, hl.data(), len + b0, (size_t)Bc * 4);
+  sync(st);
+  std::vector<uint8_t> h((size_t)Bc * (HEAD_LEN + TRACE_LEN + 1), 0);
+  uint8_t *hh = h.data(), *hb = hh + (size_t)Bc * HEAD_LEN, *hs = hb + (size_t)Bc * TRACE_LEN;
+  for (int b = 0; b < Bc; b++) {
+    const uint8_t* row = proofs + (size_t)(b0 + b) * stride;
+    memcpy(hh + (size_t)b * HEAD_LEN, row, std::min<size_t>(HEAD_LEN, stride));
+    hs[b] = (hl[b] < (uint32_t)TRACE_LEN || hl[b] > stride) ? 1 : 0;
+    if (!hs[b]) memcpy(hb + (size_t)b * TRACE_LEN, row + hl[b] - TRACE_LEN, TRACE_LEN);
+  }
+  copy_h2d(st, *hdr, h.data(), h.size() - Bc * (size_t)(TRACE_LEN + 1));
+  copy_h2d(st, *blk, hb, (size_t)Bc * TRACE_LEN);
+  copy_h2d(st, *shortrow, hs, (size_t)Bc);
+  sync(st);
+}
+// the three relations of each staged block: bad[b] (the block does not parse) and rel_ok[3 b + i] on the device
+void trace_check(zka_ctx* ctx, const zka_params* P, Cursor& w, int Bc, const uint8_t* y, const uint8_t* msg, const uint8_t* hdr,
+                 const uint8_t* blk, const uint8_t* shortrow, uint8_t** bad, uint8_t** rel_ok) {
+  Stream& st = ctx->st;
+  uint32_t* jv = w.take<uint32_t>((size_t)Bc * 3 * 8);
+  uint32_t* jr = w.take<uint32_t>((size_t)Bc * 3 * 8);
+  uint32_t* sc = w.take<uint32_t>((size_t)Bc * 4 * 8);
+  uint32_t* cproj = w.take<uint32_t>((size_t)Bc * 3 * TOM_PROJ_WORDS);
+  *bad = w.take<uint8_t>(Bc);
+  *rel_ok = w.take<uint8_t>((size_t)Bc * 3);
+  TraceVJobsTask vj{{}, y, msg, hdr, blk, shortrow, jv, jr, sc, *bad};
+  memcpy(vj.digest, P->hedge_digest, 32);
+  launch(st, Bc, vj);
+  launch(st, 3ll * Bc, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, cproj, ctx->tom, 1});
+  launch(st, 3ll * Bc, TraceVCheckTask{cproj, hdr, blk, y, sc, *rel_ok});
+}
+
+// The blocks of rows [b0, b0 + Bc) of a prove call whose untraced pass is complete, appended in the caller's rows
+void trace_prove_chunk(zka_ctx* ctx, const zka_params* P, const ProveRows& rows, const uint8_t* y, size_t L, uint32_t b0, int Bc) {
+  Stream& st = ctx->st;
+  Cursor w(ctx->trace);
+  const ProveRows r = rows.at(b0), e = rows.at(b0 + Bc);
+  auto stage = [&](auto* p, auto* end) { return stage_in(st, w.next(), p, (size_t)(end - p)); };
+  uint8_t* hdr = w.take<uint8_t>((size_t)Bc * HEAD_LEN);
+  copy_d2h_2d(st, hdr, HEAD_LEN, r.proofs, rows.proof_stride, HEAD_LEN, Bc);
+  const int32_t* d_status = stage(r.status, e.status);
+  const uint8_t* d_pk = stage(r.pk, e.pk);
+  const uint8_t* d_msg = stage(r.msg_hash, e.msg_hash);
+  const uint8_t* d_seeds = stage(r.seeds, e.seeds);
+  // tape rows: draw 1 (r) and the four trace draws; a host tape sends only these 160 bytes of each row
+  const uint8_t* tape = r.tape;
+  size_t ts = rows.tape_stride, r_off = 32, t_off = L;
+  DevBuf& tb = w.next();
+  if (tape && !is_device_ptr(tape)) {
+    uint8_t* d = tb.get<uint8_t>((size_t)Bc * 160);
+    copy_d2h_2d(st, d, 160, r.tape + 32, rows.tape_stride, 32, Bc);
+    copy_d2h_2d(st, d + 32, 160, r.tape + L, rows.tape_stride, 128, Bc);
+    tape = d; ts = 160; r_off = 0; t_off = 32;
+  }
+  uint32_t* jv = w.take<uint32_t>((size_t)Bc * 5 * 8);
+  uint32_t* jr = w.take<uint32_t>((size_t)Bc * 5 * 8);
+  uint32_t* sec = w.take<uint32_t>((size_t)Bc * 6 * 8);
+  int32_t* tstat = w.take<int32_t>(Bc);
+  uint32_t* cproj = w.take<uint32_t>((size_t)Bc * TRACE_PTS * TOM_PROJ_WORDS);
+  uint32_t* pproj = w.take<uint32_t>((size_t)Bc * TRACE_PTS * TOM_PROJ_WORDS);
+  uint8_t* pbytes = w.take<uint8_t>((size_t)Bc * TRACE_PTS * BSTRIDE);
+  uint8_t* blk = w.take<uint8_t>((size_t)Bc * TRACE_LEN);
+  launch(st, Bc, TraceJobsTask{d_status, d_pk, tape, ts, r_off, t_off, d_seeds, jv, jr, sec, tstat});
+  launch(st, (long long)Bc * TRACE_PTS, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, cproj, ctx->tom, 1});
+  launch(st, (long long)Bc * TRACE_PTS, TracePointsTask{cproj, sec, y, pproj});
+  launch_tom_norm(st, pproj, nullptr, pbytes, (long long)Bc * TRACE_PTS, 0);
+  TraceFinishTask fin{{}, y, d_msg, hdr, pbytes, sec, tstat, blk};
+  memcpy(fin.digest, P->hedge_digest, 32);
+  launch(st, Bc, fin);
+  uint8_t* chk = nullptr;
+  if (ctx->self_check) {
+    uint8_t *bad, *rel;
+    trace_check(ctx, P, w, Bc, y, d_msg, hdr, blk, nullptr, &bad, &rel);
+    chk = w.take<uint8_t>(Bc);
+    launch(st, Bc, TraceSelfCheckTask{bad, rel, tstat, chk});
+  }
+  // each row's fate is decided on the host: block appended, or the row released like one the prover rejected
+  std::vector<int32_t> hts((size_t)Bc), hst((size_t)Bc);
+  std::vector<uint32_t> hl((size_t)Bc);
+  std::vector<uint8_t> hchk((size_t)Bc, 0);
+  copy_d2h(st, hts.data(), tstat, (size_t)Bc * 4);
+  copy_d2h(st, hst.data(), r.status, (size_t)Bc * 4);
+  copy_d2h(st, hl.data(), r.proof_len, (size_t)Bc * 4);
+  if (chk) copy_d2h(st, hchk.data(), chk, (size_t)Bc);
+  const bool dev = is_device_ptr(rows.proofs);
+  std::vector<uint8_t> hblk(dev ? 0 : (size_t)Bc * TRACE_LEN);
+  if (!dev) copy_d2h(st, hblk.data(), blk, hblk.size());
+  sync(st);
+  std::vector<int64_t> off((size_t)Bc, -1);
+  uint64_t failed = 0;
+  for (int b = 0; b < Bc; b++) {
+    failed += hchk[b] == 2;
+    if (hst[b] != ZKA_OK) continue;
+    uint8_t* row = r.proofs + (size_t)b * rows.proof_stride;
+    if (hts[b] != ZKA_OK) {
+      if (dev) dev_memset(st, row, 0, rows.proof_stride); else memset(row, 0, rows.proof_stride);
+      hl[b] = 0;
+      hst[b] = hts[b];
+      continue;
+    }
+    off[b] = hl[b];
+    if (!dev) memcpy(row + hl[b], hblk.data() + (size_t)b * TRACE_LEN, TRACE_LEN);
+    hl[b] += TRACE_LEN;
+  }
+  if (dev) {
+    int64_t* d_off = w.take<int64_t>(Bc);
+    copy_h2d(st, d_off, off.data(), (size_t)Bc * 8);
+    launch(st, Bc, TraceApplyTask{r.proofs, rows.proof_stride, blk, d_off});
+  }
+  copy_h2d(st, r.proof_len, hl.data(), (size_t)Bc * 4);
+  copy_h2d(st, r.status, hst.data(), (size_t)Bc * 4);
+  sync(st);
+  if (failed) {
+    std::lock_guard<std::mutex> g(ctx->stat_mu);
+    ctx->self_check_fail += failed;
+  }
+}
+
+int prove_traced(zka_ctx* ctx, const zka_params* P, uint32_t B, const ProveRows& rows, const uint8_t* ring, uint32_t N,
+                 const uint8_t* Y) {
+  if (!ctx || !P || !Y || !rows.proofs || !rows.proof_len || !rows.status || !rows.pk || !rows.msg_hash) return ZKA_E_ARG;
+  const int S = (int)P->sec_level, n = ceil_log2(N);
+  const size_t L = (size_t)32 * prove_draws(S, n, S);
+  if (rows.tape && rows.tape_stride < L + 32 * TRACE_DRAWS) return fail(ctx, ZKA_E_ARG, "tape_stride < zka_prove_tape_len + 128");
+  if (rows.proof_stride < (size_t)proof_len(S, n, S) + TRACE_LEN)
+    return fail(ctx, ZKA_E_ARG, "proof_stride < zka_proof_max_len + zka_trace_len");
+  return guarded(ctx, [&] {
+    DevBuf ybuf;
+    const uint8_t* y = trace_y(ctx, ybuf, Y);
+    if (!y) return fail(ctx, ZKA_E_ARG, "Y is not a point of the proof group");
+    volatile uint32_t* flags = ctx->progress;
+    const uint32_t cap = ctx->progress_cap;
+    ctx->progress = nullptr;
+    ctx->progress_cap = 0;
+    const int rc = prove_batch(ctx, P, B, rows, RingSrc::one(ring, N), 0);
+    ctx->progress = flags;
+    ctx->progress_cap = cap;
+    if (rc || B == 0) return rc;
+    // the chunks of the untraced pass (prove_impl's schedule)
+    const uint8_t* rnd_in = rows.seeds ? rows.seeds : rows.tape;
+    const bool all_dev = is_device_ptr(rows.proofs) && is_device_ptr(rnd_in);
+    const std::vector<uint32_t> off =
+        chunk_schedule(B, (uint32_t)(all_dev ? ctx->chunk : std::min(ctx->chunk, ctx->host_chunk)), ctx->nlanes, !all_dev);
+    for (size_t k = 0; k + 1 < off.size(); k++) {
+      for (uint32_t b0 = off[k]; b0 < off[k + 1]; b0 += TRACE_CHUNK)
+        trace_prove_chunk(ctx, P, rows, y, L, b0, (int)std::min<uint32_t>(TRACE_CHUNK, off[k + 1] - b0));
+      if (flags && k < cap) flags[k] = 1u;
+    }
+    return 0;
+  });
+}
+
+int verify_traced(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring, uint32_t N,
+                  const uint8_t* proofs, size_t stride, const uint32_t* proof_len, const uint8_t* tape, size_t tape_stride,
+                  const uint8_t* seeds, uint32_t samples, uint8_t* ok, int32_t* status, const uint8_t* Y) {
+  if (!ctx || !P || !Y || !msg_hash || !proofs || !proof_len || !ok || !status || (!tape && !seeds)) return ZKA_E_ARG;
+  return guarded(ctx, [&] {
+    Stream& st = ctx->st;
+    DevBuf ybuf, lbuf;
+    const uint8_t* y = trace_y(ctx, ybuf, Y);
+    if (!y) return fail(ctx, ZKA_E_ARG, "Y is not a point of the proof group");
+    if (B == 0) return 0;
+    // the untraced verdict of every row's first proof_len - TRACE_LEN bytes
+    std::vector<uint32_t> hl(B);
+    copy_d2h(st, hl.data(), proof_len, (size_t)B * 4);
+    sync(st);
+    for (auto& l : hl) l = l >= (uint32_t)TRACE_LEN ? l - TRACE_LEN : 0;
+    const uint32_t* base_len = hl.data();
+    if (is_device_ptr(proof_len)) {
+      uint32_t* d = lbuf.get<uint32_t>(B);
+      copy_h2d(st, d, hl.data(), (size_t)B * 4);
+      sync(st);
+      base_len = d;
+    }
+    const int rc = seeds ? zka_verify_batch_seeded(ctx, P, B, msg_hash, ring, N, proofs, stride, base_len, seeds, samples, ok, status)
+                         : zka_verify_batch_ex(ctx, P, B, msg_hash, ring, N, proofs, stride, base_len, tape, tape_stride, ok, status,
+                                               samples);
+    if (rc) return rc;
+    const Output<uint8_t> oo(ok, 1);
+    const Output<int32_t> so(status, 1);
+    for (uint32_t b0 = 0; b0 < B; b0 += TRACE_CHUNK) {
+      const int Bc = (int)std::min<uint32_t>(TRACE_CHUNK, B - b0);
+      Cursor w(ctx->trace);
+      uint8_t *hdr, *blk, *sh, *bad, *rel;
+      trace_gather(ctx, w, proofs, stride, proof_len, b0, Bc, &hdr, &blk, &sh);
+      const uint8_t* d_msg = stage_in(st, w.next(), msg_hash + (size_t)b0 * 32, (size_t)Bc * 32);
+      trace_check(ctx, P, w, Bc, y, d_msg, hdr, blk, sh, &bad, &rel);
+      uint8_t* d_ok = oo.rows(w.next(), b0, Bc);
+      int32_t* d_st = so.rows(w.next(), b0, Bc);
+      if (!oo.dev) copy_h2d(st, d_ok, ok + b0, (size_t)Bc);
+      if (!so.dev) copy_h2d(st, d_st, status + b0, (size_t)Bc * 4);
+      launch(st, Bc, TraceVerdictTask{bad, rel, d_ok, d_st});
+      oo.copy_back(st, b0, d_ok, Bc);
+      so.copy_back(st, b0, d_st, Bc);
+      sync(st);
+    }
+    return 0;
+  });
+}
+}  // namespace
+
+size_t zka_trace_len(void) { return TRACE_LEN; }
+
+int zka_trace_pubkey(zka_ctx* ctx, const uint8_t sk[32], uint8_t* Y) {
+  if (!ctx || !sk || !Y) return ZKA_E_ARG;
+  return guarded(ctx, [&] {
+    uint32_t skl[8];
+    if (!trace_sk(ctx, sk, skl)) return fail(ctx, ZKA_E_ARG, "sk must be in [1, q)");
+    Cursor w(ctx->trace);
+    const uint8_t* bytes = trace_pubkey_dev(ctx, skl, w);
+    copy_d2h(ctx->st, Y, bytes, WP);
+    sync(ctx->st);
+    return 0;
+  });
+}
+
+int zka_prove_batch_traced(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
+                           const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* tape,
+                           size_t tape_stride, uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status,
+                           const uint8_t* Y) {
+  if (!tape) return ZKA_E_ARG;
+  ProveRows r(proofs, proof_stride, proof_len_out, status);
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.tape = tape; r.tape_stride = tape_stride;
+  return prove_traced(ctx, P, B, r, ring, N, Y);
+}
+
+int zka_prove_batch_traced_seeded(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* sig,
+                                  const uint8_t* pk, const uint32_t* which, const uint8_t* ring, uint32_t N, const uint8_t* seeds,
+                                  uint8_t* proofs, size_t proof_stride, uint32_t* proof_len_out, int32_t* status, const uint8_t* Y) {
+  if (!seeds) return ZKA_E_ARG;
+  ProveRows r(proofs, proof_stride, proof_len_out, status);
+  r.msg_hash = msg_hash; r.sig = sig; r.pk = pk; r.which = which; r.seeds = seeds;
+  return prove_traced(ctx, P, B, r, ring, N, Y);
+}
+
+int zka_verify_batch_traced(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
+                            uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                            const uint8_t* tape, size_t tape_stride, uint8_t* ok, int32_t* status, uint32_t samples,
+                            const uint8_t* Y) {
+  if (!tape) return ZKA_E_ARG;
+  return verify_traced(ctx, P, B, msg_hash, ring, N, proofs, proof_stride, proof_len, tape, tape_stride, nullptr, samples, ok,
+                       status, Y);
+}
+
+int zka_verify_batch_traced_seeded(zka_ctx* ctx, const zka_params* P, uint32_t B, const uint8_t* msg_hash, const uint8_t* ring,
+                                   uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                                   const uint8_t* seeds, uint32_t samples, uint8_t* ok, int32_t* status, const uint8_t* Y) {
+  if (!seeds) return ZKA_E_ARG;
+  return verify_traced(ctx, P, B, msg_hash, ring, N, proofs, proof_stride, proof_len, nullptr, 0, seeds, samples, ok, status, Y);
+}
+
+// The opener: the ring's points (ring[j] mod q) g, sorted by a 64-bit key of their encodings (CUB radix sort; std::sort in
+// the host simulator), then per row D = C2 - sk C1 and a binary search (TraceFindTask)
+int zka_open_batch(zka_ctx* ctx, const zka_params* P, const uint8_t sk[32], uint32_t B, const uint8_t* msg_hash,
+                   const uint8_t* ring, uint32_t N, const uint8_t* proofs, size_t proof_stride, const uint32_t* proof_len,
+                   uint32_t* index, int32_t* status) {
+  if (!ctx || !P || !sk || !msg_hash || !ring || !proofs || !proof_len || !index || !status) return ZKA_E_ARG;
+  if (N < 2 || N > (1u << 20)) return fail(ctx, ZKA_E_ARG, "ring size must be in [2, 2^20]");
+  return guarded(ctx, [&] {
+    uint32_t skl[8];
+    if (!trace_sk(ctx, sk, skl)) return fail(ctx, ZKA_E_ARG, "sk must be in [1, q)");
+    if (B == 0) return 0;
+    Stream& st = ctx->st;
+    DevBuf ybuf[4], rin, rjv, rjr, rproj, rbytes, keys, idx, keys2, idx2, tmp;
+    Cursor yw(ybuf);
+    const uint8_t* y = trace_pubkey_dev(ctx, skl, yw);
+    const uint8_t* d_ring = stage_in(st, rin, ring, (size_t)N * 32);
+    uint32_t* jv = rjv.get<uint32_t>((size_t)N * 8);
+    uint32_t* jr = rjr.get<uint32_t>((size_t)N * 8);
+    uint32_t* proj = rproj.get<uint32_t>((size_t)N * TOM_PROJ_WORDS);
+    uint8_t* rb = rbytes.get<uint8_t>((size_t)N * BSTRIDE);
+    uint64_t* k1 = keys.get<uint64_t>(N);
+    uint32_t* i1 = idx.get<uint32_t>(N);
+    uint64_t* k2 = keys2.get<uint64_t>(N);
+    uint32_t* i2 = idx2.get<uint32_t>(N);
+    launch(st, N, TraceRingJobsTask{d_ring, jv, jr});
+    launch(st, N, TomCommitTask{jv, jr, ctx->tg.tab, P->th.tab, proj, ctx->tom, 1});
+    launch(st, N, TraceToE1Task{proj});
+    launch_tom_norm(st, proj, nullptr, rb, (long long)N, 0);
+    launch(st, N, TraceKeyTask{rb, k1, i1});
+#if defined(ZKA_HOSTSIM)
+    {
+      std::vector<std::pair<uint64_t, uint32_t>> v(N);
+      for (uint32_t j = 0; j < N; j++) v[j] = {k1[j], i1[j]};
+      std::sort(v.begin(), v.end());
+      for (uint32_t j = 0; j < N; j++) { k2[j] = v[j].first; i2[j] = v[j].second; }
+    }
+#else
+    {
+      size_t tb = 0;
+      ZK_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(nullptr, tb, k1, k2, i1, i2, (int)N, 0, 64, st.s));
+      void* t = tmp.get<uint8_t>(tb);
+      ZK_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(t, tb, k1, k2, i1, i2, (int)N, 0, 64, st.s));
+    }
+#endif
+    const Output<uint32_t> io(index, 1);
+    const Output<int32_t> so(status, 1);
+    for (uint32_t b0 = 0; b0 < B; b0 += TRACE_CHUNK) {
+      const int Bc = (int)std::min<uint32_t>(TRACE_CHUNK, B - b0);
+      Cursor w(ctx->trace);
+      uint8_t *hdr, *blk, *sh, *bad, *rel;
+      trace_gather(ctx, w, proofs, proof_stride, proof_len, b0, Bc, &hdr, &blk, &sh);
+      const uint8_t* d_msg = stage_in(st, w.next(), msg_hash + (size_t)b0 * 32, (size_t)Bc * 32);
+      trace_check(ctx, P, w, Bc, y, d_msg, hdr, blk, sh, &bad, &rel);
+      uint32_t* dproj = w.take<uint32_t>((size_t)Bc * TOM_PROJ_WORDS);
+      uint8_t* dbytes = w.take<uint8_t>((size_t)Bc * BSTRIDE);
+      TraceOpenDTask od{{}, blk, dproj};
+      memcpy(od.sk, skl, 32);
+      launch(st, Bc, od);
+      launch_tom_norm(st, dproj, nullptr, dbytes, Bc, 0);
+      uint32_t* d_idx = io.rows(w.next(), b0, Bc);
+      int32_t* d_st = so.rows(w.next(), b0, Bc);
+      launch(st, Bc, TraceFindTask{bad, rel, dbytes, rb, k2, i2, N, d_idx, d_st});
+      io.copy_back(st, b0, d_idx, Bc);
+      so.copy_back(st, b0, d_st, Bc);
+      sync(st);
+    }
+    return 0;
+  });
 }
 
 }  // extern "C"
